@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- Waymo-shape frames/sec through the B200-native DetZero hot path (BASELINE.json).
+"""bench.py -- Waymo-shape frames/sec through the H100-native DetZero hot path (BASELINE.json).
 
     python bench.py --gpus N --steps K --warmup W             # BASELINE configs[1] (default): this framework, one rank per GPU
     python bench.py --impl reference --steps K --warmup W      # the reference algorithm's CPU path (oracle port), same config
@@ -48,9 +48,9 @@ def parse():
     ap.add_argument('--config', type=int, default=2, choices=[2, 3, 4, 5], help='BASELINE.json configs[config-1]')
     ap.add_argument('--backbone', default=None, choices=['VoxelBackBone8x', 'VoxelResBackBone8x'])
     ap.add_argument('--mode', default=os.environ.get('DZ_MODE', 'tf32'),
-                    help='dense BEV/head convs: tf32 (tcgen05; what the reference gets from cuDNN by default, SURVEY A.6) | fp32 (exact FMA)')
+                    help='dense BEV/head convs: tf32 (wgmma; what the reference gets from cuDNN by default, SURVEY A.6) | fp32 (exact FMA)')
     ap.add_argument('--sp-mode', default=os.environ.get('DZ_SP_MODE'),
-                    help='sparse-conv arithmetic: bf16x2 (default: fp32-level, 2 bf16 planes, tcgen05) | tf32x3 (fp32-level, 3 TF32 passes) | '
+                    help='sparse-conv arithmetic: bf16x2 (default: fp32-level, 2 bf16 planes, wgmma) | tf32x3 (fp32-level, 3 TF32 passes) | '
                          'fp32 (exact FMA, spconv default) | tf32 | bf16')
     ap.add_argument('--batch', type=int, default=None,
                     help='frames per step and GPU; config 2 default 8 = the reference config (centerpoint_1sweep.yaml:88 BATCH_SIZE_PER_GPU)')
@@ -60,7 +60,31 @@ def parse():
     ap.add_argument('--no-schedule', action='store_true', help='run the tensor-core sparse convs without the mask-grouped tile schedule')
     ap.add_argument('--layer-times', action='store_true', help='print per-layer sparse-conv times of the traced step to stderr')
     ap.add_argument('--stage-times', action='store_true', help='print a per-stage device time table to stderr')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the timed path returned in its last step as DIR/<name>.npy (float32)')
     return ap.parse_args()
+
+
+DUMP_LIMIT_BYTES = 64 * 1024 * 1024          # --dump-outputs writes at most this much in all
+
+
+def dump_outputs(dirname, arrays):
+    """--dump-outputs: the arrays a caller of the timed path receives, as float32 .npy files (inputs and weights are seeded, so two
+    builds given the same arguments can be compared output for output)"""
+    if not dirname:
+        return
+    os.makedirs(dirname, exist_ok=True)
+    arrays = {k: (a.detach().cpu().numpy() if hasattr(a, 'detach') else np.asarray(a)).astype(np.float32) for k, a in arrays.items()}
+    total = sum(a.nbytes for a in arrays.values())
+    for name, a in arrays.items():
+        if total > DUMP_LIMIT_BYTES:
+            # over the limit: a fixed, seeded sample of the flattened array (same elements for every build given the same shapes),
+            # saved with the sampled flat indices
+            keep = max(1, int(0.99 * a.size * DUMP_LIMIT_BYTES / total) // 3)       # 4-byte value + 8-byte index per element
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=min(keep, a.size), replace=False))
+            np.save(os.path.join(dirname, name + '_sample_index.npy'), idx.astype(np.float64))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(dirname, name + '.npy'), a)
 
 
 def make_model_cfg(backbone, mode, sp_mode, vfe='MeanVFE'):
@@ -137,7 +161,8 @@ def hbm_peak():
     peaks_path = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(peaks_path):
         return json.load(open(peaks_path)), 'measured'
-    return {'hbm_gbs': 6650.0, 'bf16_tflops_sustained': 1450.0}, 'fallback'
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s -- never reached, an upper bound
+    return {'hbm_gbs': 3350.0, 'bf16_tflops_sustained': 989.0}, 'H100 SXM data sheet'
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -337,6 +362,7 @@ class Detector:
                 out = self.model.forward_device(self.batch_dict(i, self.dev_pts[k]))
         if self.gather is not None:
             self.gathered = self.gather.gather()                           # ONE NCCL all-gather, inside the timed region
+        self.last_out = out
         return out
 
     def _prefetch(self, i):
@@ -429,24 +455,9 @@ def sparse_conv_roofline(det, layer_times, batch, storage_bytes=4):
     achieved = tot_bytes / (tot_ms / 1000.0) / 1e9 if tot_ms > 0 else 0.0
     return {'bound': 'hbm', 'kernel': 'sparse conv (all %d sparse-conv launches of one step)' % len(rec), 'achieved': achieved,
             'peak': peak, 'peak_source': which, 'unit': 'GB/s', 'frac': achieved / peak,
-            'traffic': committed_traffic(det, batch), 'traffic_source': 'committed ncu --set full capture of the same 14 launches '
-            '(profiles/r02_ncu_full_spconv_bf16x2_batch8.json, dram__bytes_read.sum + dram__bytes_write.sum); NOT measured in this run -- null for '
-            'any other mode / batch / backbone',
+            'traffic': None,
             'algorithmic_bytes_per_step': tot_bytes, 'storage_bytes_per_value': s, 'algorithmic_flops_per_step': tot_flops,
             'ms_per_step': tot_ms, 'frames_per_step': batch, 'layers': layers}
-
-
-def committed_traffic(det, batch):
-    """DRAM bytes per step of the sparse-conv launches from the committed ncu capture -- only for the exact configuration it was taken on"""
-    path = os.path.join(ROOT, 'profiles', 'r02_ncu_full_spconv_bf16x2_batch8.json')
-    try:
-        mode = det.model.backbone3d.model_cfg.get('COMPUTE_MODE')
-        if mode == 'bf16x2' and batch == 8 and type(det.model.backbone3d).__name__ == 'VoxelBackBone8x' and os.path.exists(path):
-            j = json.load(open(path))
-            return (j['dram_read_MB'] + j['dram_write_MB']) * 1e6
-    except Exception:
-        pass
-    return None
 
 
 SP_DTYPE = {'fp32': 'fp32 FMA', 'tf32x3': 'tf32x3 (3 TF32 passes, fp32-level)',
@@ -497,6 +508,8 @@ def run_config2(args):
     sampler.start()
     total_ms = env.timed(det.step_resident, args.steps, args.warmup)
     sampler.stop_flag = True
+    if env.rank == 0:
+        dump_outputs(args.dump_outputs, {k: det.last_out[k] for k in ('final_boxes_padded', 'final_boxes_count')})
     e2e_ms = env.timed(lambda i: det.step_e2e(i, out_host, state), args.steps, args.warmup)
     with torch.no_grad():                                   # overflow check of the resident-arm configuration (flag + counts)
         det.model.post_processing(det.step_resident(0))
@@ -592,6 +605,8 @@ def run_config3(args):
     sampler.start()
     total_ms = env.timed(det.step_resident, args.steps, args.warmup)
     sampler.stop_flag = True
+    if env.rank == 0:
+        dump_outputs(args.dump_outputs, {k: det.last_out[k] for k in ('final_boxes_padded', 'final_boxes_count')})
     e2e_ms = env.timed(lambda i: det.step_e2e(i, out_host, state), args.steps, args.warmup)
     frames = args.steps * env.world
     sb = 2 if sp_mode == 'bf16' else 4
@@ -674,7 +689,8 @@ class Refiner:
         return out, out2
 
     def step_resident(self, i):
-        return self.run(self.dev_in[i % 2])
+        self.last_out = self.run(self.dev_in[i % 2])
+        return self.last_out
 
     def step_e2e(self, i, host_out):
         d = {k: v.to(self.env.dev, non_blocking=True) for k, v in self.host[i % 2].items()}
@@ -704,6 +720,8 @@ def run_config4(args):
         sampler.start()
         ms = env.timed(rf.step_resident, args.steps, args.warmup)
         sampler.stop_flag = True
+        if env.rank == 0 and qpts == 1024:                  # the headline (BASELINE) crop size
+            dump_outputs(args.dump_outputs, {'prm_batch_box_preds': rf.last_out[0], 'grm_batch_box_preds': rf.last_out[1]})
         e2e_ms = env.timed(lambda i: rf.step_e2e(i, host_out), args.steps, args.warmup)
         tracks = args.steps * chunk * env.world
         tps = tracks / (ms / 1000.0)
@@ -779,10 +797,12 @@ def run_config5(args):
         if env.world > 1:
             dist.all_gather_into_tensor(refined_all, refined)            # the second gather: refined boxes per track
         e[3].record()
-        timing['ev'] = e
+        timing['ev'], timing['out'] = e, (boxes, counts, refined_all)
         return boxes, counts
 
     total_ms = env.timed(sequence, args.steps, max(1, args.warmup))
+    if env.rank == 0:
+        dump_outputs(args.dump_outputs, dict(zip(('sequence_boxes', 'sequence_box_counts', 'refined_boxes'), timing['out'])))
     ev = timing['ev']
     parts = {'detect_ms': ev[0].elapsed_time(ev[1]), 'box_gather_us': 1000 * ev[1].elapsed_time(ev[2]), 'refine_ms': ev[2].elapsed_time(ev[3])}
     sampler = ClockSampler(env.local)

@@ -1,4 +1,4 @@
-"""detzero_b200 -- Blackwell-native (sm_100a) implementation of the DetZero point-cloud hot path.
+"""detzero_b200 -- Hopper-native (sm_90a) implementation of the DetZero point-cloud hot path.
 
 csrc/            hand-written CUDA kernels + the C ABI (include/detzero_b200.h) -> libdetzero_b200.so
 _lib.py / ops.py ctypes binding and torch-tensor wrappers (torch = device memory + streams only)

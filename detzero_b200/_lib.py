@@ -80,7 +80,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 'detzero_b200: %s is missing. Build it with `python -c "import __graft_entry__ as g; g.build()"` '
-                '(nvcc, sm_100a). There is no CPU fallback.' % LIB_PATH)
+                '(nvcc, sm_90a). There is no CPU fallback.' % LIB_PATH)
         l = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in _SIGS.items():
             fn = getattr(l, name)            # AttributeError if the .so does not export a declared symbol

@@ -1,4 +1,4 @@
-"""In-tree build of libdetzero_b200.so (sm_100a) with nvcc.  No torch dependency in the library: it is a plain
+"""In-tree build of libdetzero_b200.so (sm_90a) with nvcc.  No torch dependency in the library: it is a plain
 C-ABI shared object (include/detzero_b200.h) loaded with ctypes."""
 import os
 import subprocess
@@ -10,7 +10,7 @@ CSRC = os.path.join(HERE, 'csrc')
 OBJ = os.path.join(CSRC, 'build')
 LIB = os.path.join(HERE, 'libdetzero_b200.so')
 
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr', '-Xptxas', '-v']
 # NOTE: no --use_fast_math: voxel indices need IEEE fp32 divide (SURVEY.md Appendix A.1)
 

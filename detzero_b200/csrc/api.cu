@@ -12,5 +12,5 @@ void dz_set_error(const char* fmt, ...) {
 }
 
 extern "C" int dz_version(void) { return 100; }                 // 0.1.0
-extern "C" int dz_sm_arch(void) { return 100; }
+extern "C" int dz_sm_arch(void) { return 90; }
 extern "C" const char* dz_last_error_string(void) { return g_err; }

@@ -1,23 +1,16 @@
-// attention_tc.cu -- multi-head attention core on the tensor cores (tcgen05, TF32 operands, fp32 TMEM accumulators), sm_100a.
+// attention_tc.cu -- multi-head attention core on the Hopper tensor cores (wgmma, TF32 operands, fp32 register accumulators).
 //
 // Replaces bmm(q,k^T) + key_padding masked_fill(-inf) + softmax + bmm(.,v) of multi_head_attention_forward
 // (refining/detzero_refine/models/modules/transformer/multi_head_attention.py:266-286), head_dim 32, without ever
-// materialising the (B*H, Pq, Pk) score tensor (15.7 GB at the BASELINE config-4 size).
+// materialising the (B*H, Pq, Pk) score tensor.
 //
-// One CTA = one (batch, head) x one tile of 128 queries.  Two kernels live here:
-//   * k_attention_tf32_v2 (default): SINGLE pass over the keys, online softmax with the block products P_j V_j folded into a register
-//     accumulator -- see the block comment above it (V as an MN-major TMA tile, score tiles two blocks ahead in three TMEM buffers,
-//     setmaxnreg).  291 us on the PRM cross-attention shape (16 tracks x 200 queries x 9600 keys x 8 heads).
-//   * k_attention_tf32 (DZ_ATTN_TWO_PASS=1, kept for A/B): TWO passes over the keys instead of the online-softmax rescaling: pass 1
-//     computes S = Q K^T block by block on the tensor cores and only tracks the row maxima; pass 2 recomputes S, forms
-//     P = exp(S - max) and accumulates O += P V in TMEM (528 us on the same shape).  Its roles:
-//   warps 16-19: loaders -- warp 16 lane 0: TMA for the Q tile and the K blocks (rows of 128 B = one head slice, SWIZZLE_128B =
-//             K-major UMMA operand); all four: register transpose of one 32-key k-block of V each into V^T
-//   warp 20 : single-thread MMA issuer (S = Q K^T : M128 N128 K32 ; O += P V^T : M128 N32 K128)
-//   warps 0-15: softmax.  Thread = (query row, 32-key column group): tcgen05.ld of its 32 scores, masking, max / exp / sum, P
-//             written to shared memory in the swizzled A-operand layout; the four column groups of a row combine their maxima
-//             after pass 1 and their sums at the end through shared memory.  (Round 1 used ONE thread per row, 128 scores each:
-//             the clock trace showed those 4 warps busy 817 K of the CTA's 870 K clocks while the MMA thread waited for P.)
+// One CTA = one (batch, head) x one tile of 128 queries, ONE pass over the keys in blocks of 128 (online softmax):
+//   warps 0-7  : two consumer warpgroups, 64 queries each.  Per key block: S = Q K^T (wgmma M64 N128 K8 x 4, registers), masked
+//                row maxima / exp2 in registers (a row's 128 scores live in the 4 threads of a lane quad), P to shared memory
+//                in the K-major SW128 A-operand layout, O = O * exp2(m_old - m_new) + P V (wgmma M64 N32 K8 x 16, registers).
+//   warps 8-11 : loaders.  Warp 8 lane 0 TMA-loads the Q tile once and the K blocks (rows of 128 B = one head slice,
+//                SWIZZLE_128B = K-major B operand); each warp transposes one 32-key k-block of V into V^T through registers
+//                (TF32 wgmma takes K-major operands only, and for P V the keys are the reduction dimension).
 #include <stdlib.h>
 #include "common.cuh"
 #include "tc.cuh"
@@ -26,45 +19,11 @@ static constexpr int AT_M = 128;            // queries per CTA
 static constexpr int AT_N = 128;            // keys per block
 static constexpr int AT_D = 32;             // head dim
 static constexpr int AT_TILE = AT_M * 128;  // 16 KB: 128 rows x 128 B
-static constexpr int AT_SM_WARPS = 16;          // softmax warps: 4 TMEM lane quarters x 4 column groups of 32 keys
-static constexpr int AT_THREADS = 32 * (AT_SM_WARPS + 5);   // warps 0-15 softmax, 16-19 loaders (V^T: one 32-key k-block each), 20 MMA
+static constexpr int AT_CONSUMERS = 8;
+static constexpr int AT_THREADS = 32 * (AT_CONSUMERS + 4);
 
-// validity of 32 consecutive keys as a bit mask (1 = masked); 4 mask bytes per load when the row is 4-byte aligned
-__device__ __forceinline__ uint32_t masked_bits32(const unsigned char* mrow, int key0, int Pk, bool fast) {
-    uint32_t bits = 0;
-    if (fast) {
-#pragma unroll
-        for (int w = 0; w < 8; ++w) {
-            const int key = key0 + 4 * w;
-            uint32_t m4 = key < Pk ? (mrow ? __ldg(reinterpret_cast<const uint32_t*>(mrow + key)) : 0u) : 0x01010101u;
-            bits |= ((m4 & 0xffu) ? 1u : 0u) << (4 * w);
-            bits |= ((m4 & 0xff00u) ? 1u : 0u) << (4 * w + 1);
-            bits |= ((m4 & 0xff0000u) ? 1u : 0u) << (4 * w + 2);
-            bits |= ((m4 & 0xff000000u) ? 1u : 0u) << (4 * w + 3);
-        }
-    } else {
-        for (int c = 0; c < 32; ++c) {
-            const int key = key0 + c;
-            if (key >= Pk || (mrow && mrow[key])) bits |= 1u << c;
-        }
-    }
-    return bits;
-}
-
-__device__ long long g_at_trace[64];         // clock accounting of CTA (0,0) (tools/trace_attention.py); written only when g_at_on != 0
-__device__ int g_at_on = 0;
-static int g_at_on_host = 0;               // host mirror: selects the traced instantiation of the single-pass kernel
-extern "C" int dz_debug_attention_trace(long long* host, int on) {
-    cudaDeviceSynchronize();
-    g_at_on_host = on;
-    if (cudaMemcpyToSymbol(g_at_on, &on, sizeof(int)) != cudaSuccess) return -1;
-    return host ? (cudaMemcpyFromSymbol(host, g_at_trace, sizeof(long long) * 64) == cudaSuccess ? 0 : -1) : 0;
-}
-#define AT2_T(slot, stmt) do { if (tr) { const unsigned c0__ = (unsigned)clock(); stmt; acc[slot] += (unsigned)clock() - c0__; } else { stmt; } } while (0)
-#define AT_T(slot, stmt) do { if (tr) { const long long c0__ = clock64(); stmt; acc[slot] += clock64() - c0__; } else { stmt; } } while (0)
-
-// 2^x on the MUFU pipe, one instruction (exp2f() is a ~6-instruction sequence; its arguments here are <= 0 and results land in
-// (0, 1], where ex2.approx is good to 2 ulp -- far inside the TF32 tolerance of this mode)
+// 2^x on the MUFU pipe, one instruction (its arguments here are <= 0 and results land in (0, 1], where ex2.approx is good
+// to 2 ulp -- far inside the TF32 tolerance of this mode)
 __device__ __forceinline__ float ex2_approx(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -75,16 +34,15 @@ struct AtSmem {
     static constexpr int Q = 0;
     static constexpr int K = AT_TILE;                    // 2 stages
     static constexpr int VT = K + 2 * AT_TILE;           // 2 stages of 4 k-blocks x (32 rows x 128 B) = 16 KB each
-    static constexpr int P = VT + 2 * AT_TILE;           // 2 buffers x 4 k-blocks x 16 KB: the softmax of block j+1 writes P while the
-    static constexpr int BARS = P + 8 * AT_TILE;         // tensor core still reads block j's (single-buffered they took turns)
-    static constexpr int RED = BARS + 256;               // [2][4][128] floats: row max / row sum partials of the column groups
-    static constexpr int TOTAL = RED + 2 * 4 * 128 * 4 + 1024;
+    static constexpr int P = VT + 2 * AT_TILE;           // per warpgroup: 4 k-blocks x (64 rows x 128 B) = 32 KB
+    static constexpr int MASK = P + 4 * AT_TILE;         // per warpgroup: 4 words = the 128 keys of the block (1 = masked)
+    static constexpr int BARS = MASK + 64;
+    static constexpr int TOTAL = BARS + 256 + 1024;
 };
 
 __global__ void __launch_bounds__(AT_THREADS, 1)
-k_attention_tf32(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, int q_col0, int k_col0,
-                 const float* __restrict__ v, int ldv, const unsigned char* __restrict__ kpm, int Pq, int Pk, int H,
-                 float* __restrict__ out, int ldo) {
+k_attention_tf32(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const float* __restrict__ v, int ldv,
+                 const unsigned char* __restrict__ kpm, int Pq, int Pk, int H, float* __restrict__ out, int ldo) {
     extern __shared__ unsigned char smem_raw[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + AtSmem::BARS);
@@ -93,17 +51,8 @@ k_attention_tf32(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     uint64_t* k_empty = bars + 3;     // [2]
     uint64_t* v_full = bars + 5;      // [2]
     uint64_t* v_empty = bars + 7;     // [2]
-    uint64_t* s_full = bars + 9;      // [2]
-    uint64_t* s_empty = bars + 11;    // [2]
-    uint64_t* p_full = bars + 13;     // [2]
-    uint64_t* p_empty = bars + 15;    // [2]
-    uint64_t* o_full = bars + 17;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 18);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const bool tr = g_at_on && blockIdx.x == 0 && blockIdx.y == 0;
-    long long acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    const long long t_start = tr ? clock64() : 0;
     const int bh = blockIdx.y, b = bh / H, h = bh % H;
     const int q0 = blockIdx.x * AT_M;
     const int nblk = (Pk + AT_N - 1) / AT_N;
@@ -113,513 +62,162 @@ k_attention_tf32(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
         tc::prefetch_tmap(&tmK);
         tc::mbar_init(q_full, 1);
         for (int i = 0; i < 2; ++i) {
-            tc::mbar_init(k_full + i, 1); tc::mbar_init(k_empty + i, 1);
-            tc::mbar_init(v_full + i, 4); tc::mbar_init(v_empty + i, 1);
-            tc::mbar_init(s_full + i, 1); tc::mbar_init(s_empty + i, AT_SM_WARPS);     // one arrival per WARP: 512 per-thread arrivals on one
-                                                                                        // mbarrier serialise in shared memory (~1.5 K clk per block)
+            tc::mbar_init(k_full + i, 1); tc::mbar_init(k_empty + i, AT_CONSUMERS);
+            tc::mbar_init(v_full + i, 4); tc::mbar_init(v_empty + i, AT_CONSUMERS);
         }
-        for (int i = 0; i < 2; ++i) { tc::mbar_init(p_full + i, AT_SM_WARPS); tc::mbar_init(p_empty + i, 1); }
-        tc::mbar_init(o_full, 1);
         tc::fence_barrier_init();
     }
-    if (warp == AT_SM_WARPS + 4) tc::tmem_alloc<512>(tmem_slot);
-    tc::tcgen05_fence_before();
     __syncthreads();
-    tc::tcgen05_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    const uint32_t tmem_s[2] = {tmem, tmem + 128};
-    const uint32_t tmem_o = tmem + 256;
 
-    if (warp >= AT_SM_WARPS && warp < AT_SM_WARPS + 4) {
+    if (warp >= AT_CONSUMERS) {
         // ============================== loaders ==============================
-        const int kk = warp - AT_SM_WARPS;                          // this warp's k-block (32 keys) of every V block
+        const int kk = warp - AT_CONSUMERS;                         // this warp's k-block (32 keys) of every V block
         if (kk == 0 && lane == 0) {
             tc::mbar_arrive_expect_tx(q_full, AT_TILE);
-            tc::tma_load_2d(smem + AtSmem::Q, &tmQ, q_full, q_col0 + h * AT_D, b * Pq + q0);
+            tc::tma_load_2d(smem + AtSmem::Q, &tmQ, q_full, h * AT_D, b * Pq + q0);
         }
-        for (int it = 0; it < 2 * nblk; ++it) {                     // K blocks: pass 1 then pass 2
-            const int j = it % nblk, st = it & 1;
+        for (int j = 0; j < nblk; ++j) {
+            const int st = j & 1;
             if (kk == 0 && lane == 0) {
-                AT_T(0, tc::mbar_wait(k_empty + st, ((it >> 1) & 1) ^ 1));
+                tc::mbar_wait(k_empty + st, ((j >> 1) & 1) ^ 1);
                 tc::mbar_arrive_expect_tx(k_full + st, AT_TILE);
-                tc::tma_load_2d(smem + AtSmem::K + st * AT_TILE, &tmK, k_full + st, k_col0 + h * AT_D, b * Pk + j * AT_N);
+                tc::tma_load_2d(smem + AtSmem::K + st * AT_TILE, &tmK, k_full + st, h * AT_D, b * Pk + j * AT_N);
             }
-            if (it >= nblk) {                                       // pass 2 also needs V_j^T
-                const int jv = it - nblk, sv = jv & 1;
-                AT_T(1, tc::mbar_wait(v_empty + sv, ((jv >> 1) & 1) ^ 1));
-                const long long tv0 = tr ? clock64() : 0;
-                unsigned char* vt = smem + AtSmem::VT + sv * AT_TILE;
-                // lane handles key kk*32 + lane ; 8 float4 per key ; writes V^T[d][key] swizzled
-                {
-                    const int key = kk * 32 + lane, kg = jv * AT_N + key;
-                    const float* vp = v + ((size_t)b * Pk + kg) * ldv + h * AT_D;
-                    float4 x[8];
+            tc::mbar_wait(v_empty + st, ((j >> 1) & 1) ^ 1);
+            unsigned char* vt = smem + AtSmem::VT + st * AT_TILE;
+            // lane handles key kk*32 + lane ; 8 float4 per key ; writes V^T[d][key] swizzled
+            const int key = kk * 32 + lane, kg = j * AT_N + key;
+            const float* vp = v + ((size_t)b * Pk + kg) * ldv + h * AT_D;
+            float4 x[8];
 #pragma unroll
-                    for (int d4 = 0; d4 < 8; ++d4) x[d4] = (kg < Pk) ? __ldg(reinterpret_cast<const float4*>(vp) + d4) : make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int d4 = 0; d4 < 8; ++d4) x[d4] = (kg < Pk) ? __ldg(reinterpret_cast<const float4*>(vp) + d4) : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
-                    for (int d4 = 0; d4 < 8; ++d4) {
-                        const float e[4] = {x[d4].x, x[d4].y, x[d4].z, x[d4].w};
+            for (int d4 = 0; d4 < 8; ++d4) {
+                const float e[4] = {x[d4].x, x[d4].y, x[d4].z, x[d4].w};
 #pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const int d = d4 * 4 + i;               // row of V^T
-                            // k-block kk (32 keys = 128 B), row d: (d>>3)*1024 + (d&7)*128, 16-byte chunk (lane>>2) ^ (d&7)
-                            const uint32_t off = (uint32_t)(kk * 4096 + (d >> 3) * 1024 + (d & 7) * 128 + (((lane >> 2) ^ (d & 7)) << 4) + (lane & 3) * 4);
-                            *reinterpret_cast<float*>(vt + off) = e[i];
-                        }
-                    }
+                for (int i = 0; i < 4; ++i) {
+                    const int d = d4 * 4 + i;                       // row of V^T
+                    // k-block kk (32 keys = 128 B), row d: (d>>3)*1024 + (d&7)*128, 16-byte chunk (lane>>2) ^ (d&7)
+                    const uint32_t off = (uint32_t)(kk * 4096 + (d >> 3) * 1024 + (d & 7) * 128 + (((lane >> 2) ^ (d & 7)) << 4) + (lane & 3) * 4);
+                    *reinterpret_cast<float*>(vt + off) = e[i];
                 }
-                tc::fence_proxy_async();
-                __syncwarp();
-                if (lane == 0) tc::mbar_arrive(v_full + sv);
-                if (tr) acc[2] += clock64() - tv0;
             }
-        }
-        if (tr && kk == 0 && lane == 0) { g_at_trace[0] = acc[0]; g_at_trace[1] = acc[1]; g_at_trace[2] = acc[2]; g_at_trace[3] = clock64() - t_start; }
-    } else if (warp == AT_SM_WARPS + 4) {
-        // ============================== MMA issuer ==============================
-        if (lane == 0) {
-            constexpr uint32_t idesc_s = tc::instr_desc(2, 128, AT_N);
-            constexpr uint32_t idesc_o = tc::instr_desc(2, 128, AT_D);
-            const uint64_t qdesc = tc::smem_desc_sw128(tc::smem_u32(smem + AtSmem::Q));
-            tc::mbar_wait(q_full, 0);
-            auto issue_s = [&](int it) {                            // S[it&1] = Q K_it^T
-                const int st = it & 1;
-                AT_T(0, tc::mbar_wait(k_full + st, (it >> 1) & 1));
-                AT_T(1, tc::mbar_wait(s_empty + st, ((it >> 1) & 1) ^ 1));
-                const long long ti0 = tr ? clock64() : 0;
-                tc::tcgen05_fence_after();
-                const uint64_t kdesc = tc::smem_desc_sw128(tc::smem_u32(smem + AtSmem::K + st * AT_TILE));
-#pragma unroll
-                for (int kk = 0; kk < 4; ++kk) tc::mma_tf32(tmem_s[st], qdesc + (uint64_t)(kk * 2), kdesc + (uint64_t)(kk * 2), idesc_s, kk ? 1u : 0u);
-                tc::mma_commit(k_empty + st);
-                tc::mma_commit(s_full + st);
-                if (tr) acc[4] += clock64() - ti0;
-            };
-            for (int it = 0; it < nblk; ++it) issue_s(it);          // pass 1: scores only
-            if (tr) g_at_trace[15] = clock64() - t_start;
-            issue_s(nblk);                                          // first block of pass 2
-            for (int j = 0; j < nblk; ++j) {
-                if (j + 1 < nblk) issue_s(nblk + j + 1);            // S of the next block overlaps this block's softmax
-                const int sv = j & 1;
-                AT_T(2, tc::mbar_wait(v_full + sv, (j >> 1) & 1));
-                AT_T(3, tc::mbar_wait(p_full + (j & 1), (j >> 1) & 1));
-                const long long tp0 = tr ? clock64() : 0;
-                tc::tcgen05_fence_after();
-                const uint32_t pa = tc::smem_u32(smem + AtSmem::P + (j & 1) * 4 * AT_TILE), va = tc::smem_u32(smem + AtSmem::VT + sv * AT_TILE);
-#pragma unroll
-                for (int kk = 0; kk < 16; ++kk) {
-                    const uint64_t pdesc = tc::smem_desc_sw128(pa + (kk >> 2) * AT_TILE) + (uint64_t)((kk & 3) * 2);
-                    const uint64_t vdesc = tc::smem_desc_sw128(va + (kk >> 2) * 4096) + (uint64_t)((kk & 3) * 2);
-                    tc::mma_tf32(tmem_o, pdesc, vdesc, idesc_o, (j | kk) ? 1u : 0u);
-                }
-                tc::mma_commit(v_empty + sv);
-                tc::mma_commit(p_empty + (j & 1));
-                if (tr) acc[5] += clock64() - tp0;
-            }
-            tc::mma_commit(o_full);
-            if (tr) { for (int i = 0; i < 6; ++i) g_at_trace[8 + i] = acc[i]; g_at_trace[14] = clock64() - t_start; }
+            tc::fence_proxy_async();
+            __syncwarp();
+            if (lane == 0) tc::mbar_arrive(v_full + st);
         }
     } else {
-        // ============================== softmax / epilogue: thread = (query row, 32-key column group) ==============================
-        const int qq = warp & 3, cg = warp >> 2;                    // TMEM lane quarter (== warp % 4), column group
-        const int row = qq * 32 + lane;
-        const int qi = q0 + row;
-        const uint32_t lane_base = (uint32_t)(qq * 32) << 16;
+        // ============================== consumers: warpgroup g = queries [64g, 64g+64) ==============================
+        const int g = warp >> 2, w = warp & 3, tid = threadIdx.x & 127;
+        const int rl = 16 * w + (lane >> 2);                        // this thread's rows: rl and rl + 8 of the warpgroup
         const unsigned char* mrow = kpm ? kpm + (size_t)b * Pk : nullptr;
-        const bool fast = (Pk & 3) == 0 && ((reinterpret_cast<uintptr_t>(mrow) & 3) == 0);
-        float* red = reinterpret_cast<float*>(smem + AtSmem::RED);
-        const int c0 = cg * 32;
-        float rmax = -INFINITY;
-        for (int it = 0; it < nblk; ++it) {                         // ---- pass 1: row maxima
-            const int st = it & 1;
-            AT_T(0, tc::mbar_wait(s_full + st, (it >> 1) & 1));
-            const long long tb0 = tr ? clock64() : 0;
-            tc::tcgen05_fence_after();
-            float sc[32];
-            tc::tmem_ld32(tmem_s[st] + lane_base + (uint32_t)c0, sc);
-            const uint32_t mb = masked_bits32(mrow, it * AT_N + c0, Pk, fast);
-            if (mb == 0u) {                                         // the mask depends on the key only: uniform over the CTA
-#pragma unroll
-                for (int c = 0; c < 32; ++c) rmax = fmaxf(rmax, sc[c]);
-            } else if (mb != 0xffffffffu) {
-#pragma unroll
-                for (int c = 0; c < 32; ++c)
-                    if (!((mb >> c) & 1u)) rmax = fmaxf(rmax, sc[c]);
-            }
-            tc::tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) tc::mbar_arrive(s_empty + st);
-            if (tr) acc[1] += clock64() - tb0;
-        }
-        red[cg * 128 + row] = rmax;                                 // combine the four column groups of the row
-        asm volatile("bar.sync 1, %0;" ::"n"(32 * AT_SM_WARPS) : "memory");
-        rmax = fmaxf(fmaxf(red[row], red[128 + row]), fmaxf(red[256 + row], red[384 + row]));
-        if (tr && threadIdx.x == 0) g_at_trace[23] = clock64() - t_start;
-        float lsum = 0.f;
+        uint32_t* mwords = reinterpret_cast<uint32_t*>(smem + AtSmem::MASK) + g * 4;
+        unsigned char* pg = smem + AtSmem::P + g * 2 * AT_TILE;
+        const uint64_t qdesc = tc::smem_desc_sw128(tc::smem_u32(smem + AtSmem::Q) + g * 64 * 128);
         const float LOG2E = 1.4426950408889634f;
-        const float mscaled = rmax * LOG2E;
-        unsigned char* pbase0 = smem + AtSmem::P + cg * AT_TILE + (row >> 3) * 1024 + (row & 7) * 128;     // k-block cg of P
-        for (int j = 0; j < nblk; ++j) {                            // ---- pass 2: P = exp(S - max), O += P V
-            const int it = nblk + j, st = it & 1;
-            AT_T(2, tc::mbar_wait(s_full + st, (it >> 1) & 1));
-            tc::tcgen05_fence_after();
-            AT_T(3, tc::mbar_wait(p_empty + (j & 1), ((j >> 1) & 1) ^ 1));   // the P buffer of block j-2 has been consumed by the tensor core
-            const long long tb0 = tr ? clock64() : 0;
-            unsigned char* pk = pbase0 + (j & 1) * 4 * AT_TILE;
-            float sc[32];
-            tc::tmem_ld32(tmem_s[st] + lane_base + (uint32_t)c0, sc);
-            const uint32_t mb = masked_bits32(mrow, j * AT_N + c0, Pk, fast);
-            if (mb == 0u) {
+        float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+        float o[AT_D / 2];
 #pragma unroll
-                for (int c = 0; c < 32; ++c) { sc[c] = ex2_approx(fmaf(sc[c], LOG2E, -mscaled)); lsum += sc[c]; }
-            } else if (mb == 0xffffffffu) {
-#pragma unroll
-                for (int c = 0; c < 32; ++c) sc[c] = 0.f;
-            } else {
-#pragma unroll
-                for (int c = 0; c < 32; ++c) {
-                    const float pv = ((mb >> c) & 1u) ? 0.f : ex2_approx(fmaf(sc[c], LOG2E, -mscaled));
-                    lsum += pv;
-                    sc[c] = pv;
-                }
+        for (int i = 0; i < AT_D / 2; ++i) o[i] = 0.f;
+        tc::mbar_wait(q_full, 0);
+        for (int j = 0; j < nblk; ++j) {
+            const int st = j & 1;
+            // key mask of the block: one key per thread, one ballot word per warp
+            {
+                const int key = j * AT_N + tid;
+                const bool mk = key >= Pk || (mrow && mrow[key]);
+                const uint32_t word = __ballot_sync(0xffffffffu, mk);
+                if (lane == 0) mwords[w] = word;
             }
+            // S = Q K_j^T
+            float s[AT_N / 2];
+            tc::mbar_wait(k_full + st, (j >> 1) & 1);
+            const uint64_t kdesc = tc::smem_desc_sw128(tc::smem_u32(smem + AtSmem::K + st * AT_TILE));
+            tc::wgmma_fence();
 #pragma unroll
-            for (int ch = 0; ch < 8; ++ch)
-                *reinterpret_cast<float4*>(pk + ((ch ^ (row & 7)) << 4)) = make_float4(sc[4 * ch], sc[4 * ch + 1], sc[4 * ch + 2], sc[4 * ch + 3]);
-            tc::fence_proxy_async();
-            tc::tcgen05_fence_before();
+            for (int kk = 0; kk < 4; ++kk) tc::wgmma<AT_N, tc::K_TF32>(s, qdesc + (uint64_t)(kk * 2), kdesc + (uint64_t)(kk * 2), kk ? 1u : 0u);
+            tc::wgmma_commit();
+            tc::wgmma_wait_all();
             __syncwarp();
-            if (lane == 0) { tc::mbar_arrive(p_full + (j & 1)); tc::mbar_arrive(s_empty + st); }
-            if (tr) acc[4] += clock64() - tb0;
+            if (lane == 0) tc::mbar_arrive(k_empty + st);
+            tc::named_sync(2 + g, 128);                             // mask words of this block are visible
+            uint32_t mw[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) mw[i] = mwords[i];
+            // masked row maxima (column of s[4c + 2r + e] = 8c + 2(lane%4) + e)
+            float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+            for (int c = 0; c < AT_N / 8; ++c)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int col = 8 * c + 2 * (lane & 3) + e;
+                    if ((mw[col >> 5] >> (col & 31)) & 1u) { s[4 * c + e] = -INFINITY; s[4 * c + 2 + e] = -INFINITY; }
+                    mx[0] = fmaxf(mx[0], s[4 * c + e]);
+                    mx[1] = fmaxf(mx[1], s[4 * c + 2 + e]);
+                }
+            float alpha[2], ms[2];
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+                mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+                const float m_new = fmaxf(m_run[r], mx[r]);
+                alpha[r] = (m_run[r] == -INFINITY) ? 0.f : ex2_approx((m_run[r] - m_new) * LOG2E);
+                ms[r] = m_new == -INFINITY ? 0.f : m_new * LOG2E;   // a row with every key so far masked keeps P = 0
+                m_run[r] = m_new;
+            }
+            // P = exp2(S - m) -> shared memory (k-block c/4, row rl + 8r, SW128)
+            float psum[2] = {0.f, 0.f};
+#pragma unroll
+            for (int c = 0; c < AT_N / 8; ++c)
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    const float p0 = ex2_approx(fmaf(s[4 * c + 2 * r], LOG2E, -ms[r]));
+                    const float p1 = ex2_approx(fmaf(s[4 * c + 2 * r + 1], LOG2E, -ms[r]));
+                    psum[r] += p0 + p1;
+                    const int row = rl + 8 * r, cc = (8 * c + 2 * (lane & 3)) & 31;
+                    const uint32_t off = (uint32_t)((c >> 2) * 8192 + (row >> 3) * 1024 + (row & 7) * 128 + (((cc >> 2) ^ (row & 7)) << 4) + (cc & 3) * 4);
+                    *reinterpret_cast<float2*>(pg + off) = make_float2(p0, p1);
+                }
+#pragma unroll
+            for (int r = 0; r < 2; ++r) l_run[r] = l_run[r] * alpha[r] + psum[r];
+#pragma unroll
+            for (int c = 0; c < AT_D / 8; ++c)
+#pragma unroll
+                for (int r = 0; r < 2; ++r) { o[4 * c + 2 * r] *= alpha[r]; o[4 * c + 2 * r + 1] *= alpha[r]; }
+            tc::fence_proxy_async();                                // P (generic-proxy writes) -> wgmma operand reads
+            tc::named_sync(2 + g, 128);
+            // O += P V_j
+            tc::mbar_wait(v_full + st, (j >> 1) & 1);
+            const uint32_t pa = tc::smem_u32(pg), va = tc::smem_u32(smem + AtSmem::VT + st * AT_TILE);
+            tc::wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < 16; ++kk) {
+                const uint64_t pdesc = tc::smem_desc_sw128(pa + (kk >> 2) * 8192) + (uint64_t)((kk & 3) * 2);
+                const uint64_t vdesc = tc::smem_desc_sw128(va + (kk >> 2) * 4096) + (uint64_t)((kk & 3) * 2);
+                tc::wgmma<AT_D, tc::K_TF32>(o, pdesc, vdesc, 1u);
+            }
+            tc::wgmma_commit();
+            tc::wgmma_wait_all();
+            __syncwarp();
+            if (lane == 0) tc::mbar_arrive(v_empty + st);
         }
-        if (tr && threadIdx.x == 0) { for (int i = 0; i < 5; ++i) g_at_trace[16 + i] = acc[i]; g_at_trace[22] = clock64() - t_start; g_at_trace[24] = nblk; }
-        red[512 + cg * 128 + row] = lsum;
-        asm volatile("bar.sync 1, %0;" ::"n"(32 * AT_SM_WARPS) : "memory");
-        if (cg == 0) {
-            lsum = (red[512 + row] + red[512 + 128 + row]) + (red[512 + 256 + row] + red[512 + 384 + row]);
-            tc::mbar_wait(o_full, 0);
-            tc::tcgen05_fence_after();
-            float o[32];
-            tc::tmem_ld32(tmem_o + lane_base, o);
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
+            l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
+            const int qi = q0 + g * 64 + rl + 8 * r;
             if (qi < Pq) {
                 float* op = out + ((size_t)b * Pq + qi) * ldo + h * AT_D;
-                const float inv = 1.f / lsum;                       // lsum == 0 (every key masked) -> NaN like softmax of all -inf
+                const float inv = 1.f / l_run[r];                   // l == 0 (every key masked): NaN, like softmax of all -inf
 #pragma unroll
-                for (int d = 0; d < AT_D; d += 4) {
-                    float4 r = make_float4(o[d] * inv, o[d + 1] * inv, o[d + 2] * inv, o[d + 3] * inv);
-                    if (lsum == 0.f) r = make_float4(NAN, NAN, NAN, NAN);
-                    *reinterpret_cast<float4*>(op + d) = r;
+                for (int c = 0; c < AT_D / 8; ++c) {
+                    float2 x = make_float2(o[4 * c + 2 * r] * inv, o[4 * c + 2 * r + 1] * inv);
+                    if (l_run[r] == 0.f) x = make_float2(NAN, NAN);
+                    *reinterpret_cast<float2*>(op + 8 * c + 2 * (lane & 3)) = x;
                 }
             }
         }
     }
-    tc::tcgen05_fence_before();
-    __syncthreads();
-    if (warp == AT_SM_WARPS + 4) tc::tmem_dealloc<512>(tmem);
-}
-
-// =====================================================================================================================
-// v2: SINGLE pass over the keys (online softmax).  The two-pass kernel above reads every 128 x 128 score tile from TMEM twice, and
-// tcgen05.ld moves 64 B/clk: 2 x 1024 clk per key block before any arithmetic (tools/trace_attention.py).  Here:
-//   * S_j is read once (half-by-half, issued under the exp2 phase of block j-1); the running row maximum is combined across a row's four
-//     column-group threads through shared memory + ONE 128-thread named barrier per row quarter and block;
-//   * P_j = exp2(S_j - m_j) goes to shared memory (SW128 A operand); the tensor core computes the BLOCK product Oblk_j = P_j V_j into a
-//     double-buffered 32-column TMEM tile (accumulate only inside the block) and each of the row's four threads folds its 8 output
-//     dims into a REGISTER accumulator one block later: O <- O * exp2(m_{j-2} - m_{j-1}) + Oblk_{j-1}.  No accumulator rescaling in
-//     TMEM, no tcgen05.st, no dependency of PV(j+1) on a correction of PV(j);
-//   * V_j is the TMA tile itself ([key][32 dims], rows of 128 B) used as an MN-major B operand -- no transposed copy (for tf32 that needs
-//     descriptor layout type 1 "128B swizzle, 32B atoms" and CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B);
-//   * the score tiles run TWO blocks ahead of the softmax in three 128-column TMEM buffers (the ncu source page showed 15 % of the stall
-//     samples on s_full when S(j+1) queued behind P(j-1) V(j-1)); K_t is requested before V_{t-1};
-//   * 20 warps: 16 softmax (setmaxnreg.inc 112), TMA producer, MMA issuer, 2 idle (the service warpgroup does setmaxnreg.dec 32).
-// =====================================================================================================================
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, float (&v)[8]) {
-    uint32_t r[8];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]) : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-constexpr int AT2_THREADS = 32 * (AT_SM_WARPS + 4);      // 16 softmax warps + one more warpgroup: TMA producer, MMA issuer, 2 idle warps (setmaxnreg works on whole warpgroups)
-struct At2Smem {
-    static constexpr int Q = 0;
-    static constexpr int K = AT_TILE;                    // 2 stages
-    static constexpr int VT = K + 2 * AT_TILE;           // 2 stages
-    static constexpr int P = VT + 2 * AT_TILE;           // 2 buffers x 4 k-blocks x 16 KB
-    static constexpr int BARS = P + 8 * AT_TILE;
-    static constexpr int RED = BARS + 256;               // [3][4][128] floats: block maxima (2 buffers) + final row sums
-    static constexpr int TOTAL = RED + 3 * 4 * 128 * 4 + 1024;
-};
-
-template <bool TRACE>
-__global__ void __launch_bounds__(AT2_THREADS, 1)
-k_attention_tf32_v2(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                    int q_col0, int k_col0, int v_col0, const unsigned char* __restrict__ kpm, int Pq, int Pk, int H,
-                    float* __restrict__ out, int ldo) {
-    extern __shared__ unsigned char smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + At2Smem::BARS);
-    uint64_t* q_full = bars + 0;
-    uint64_t* k_full = bars + 1;      // [2]
-    uint64_t* k_empty = bars + 3;     // [2]
-    uint64_t* v_full = bars + 5;      // [2]
-    uint64_t* v_empty = bars + 7;     // [2]
-    uint64_t* s_full = bars + 9;      // [3]: the score tiles run TWO key blocks ahead of the softmax (3 TMEM buffers), so S(j+1) never waits
-    uint64_t* s_empty = bars + 12;    // [3]  behind P(j-1) V(j-1) in the tensor pipe when the softmax asks for it
-    uint64_t* p_full = bars + 15;     // [2]
-    uint64_t* p_empty = bars + 17;    // [2]
-    uint64_t* o_full = bars + 19;     // [2]
-    uint64_t* o_empty = bars + 21;    // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 23);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const bool tr = TRACE && blockIdx.x == 0 && blockIdx.y == 0;
-    unsigned acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    const unsigned t_start = tr ? (unsigned)clock() : 0u;
-    const int bh = blockIdx.y, b = bh / H, h = bh % H;
-    const int q0 = blockIdx.x * AT_M;
-    const int nblk = (Pk + AT_N - 1) / AT_N;
-
-    if (threadIdx.x == 0) {
-        tc::prefetch_tmap(&tmQ);
-        tc::prefetch_tmap(&tmK);
-        tc::prefetch_tmap(&tmV);
-        tc::mbar_init(q_full, 1);
-        for (int i = 0; i < 2; ++i) {
-            tc::mbar_init(k_full + i, 1); tc::mbar_init(k_empty + i, 1);
-            tc::mbar_init(v_full + i, 1); tc::mbar_init(v_empty + i, 1);
-            tc::mbar_init(p_full + i, AT_SM_WARPS); tc::mbar_init(p_empty + i, 1);
-            tc::mbar_init(o_full + i, 1); tc::mbar_init(o_empty + i, AT_SM_WARPS);
-        }
-        for (int i = 0; i < 3; ++i) { tc::mbar_init(s_full + i, 1); tc::mbar_init(s_empty + i, AT_SM_WARPS); }
-        tc::fence_barrier_init();
-    }
-    if (warp == AT_SM_WARPS + 1) tc::tmem_alloc<512>(tmem_slot);
-    tc::tcgen05_fence_before();
-    __syncthreads();
-    tc::tcgen05_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    const uint32_t tmem_ob[2] = {tmem + 384, tmem + 416};       // score tiles: columns [0, 384), block products: [384, 448)
-
-    // register file: 640 threads x 96 at launch; the service warpgroup keeps 32 per thread and the softmax warpgroups take 112
-    // register file: 640 threads x 96 at launch; the service warpgroup (warps 16-19) keeps 32 per thread, the softmax warpgroups take 112
-    if (warp >= AT_SM_WARPS) asm volatile("setmaxnreg.dec.sync.aligned.u32 32;");
-    if (warp == AT_SM_WARPS) {
-        // ============================== TMA producer: Q once, then K_j and V_j tiles (both straight from global memory) ==============================
-        if (lane == 0) {
-            tc::mbar_arrive_expect_tx(q_full, AT_TILE);
-            tc::tma_load_2d(smem + At2Smem::Q, &tmQ, q_full, q_col0 + h * AT_D, b * Pq + q0);
-            for (int t = 0; t <= nblk; ++t) {                       // K_t is requested before V_{t-1}: the score tiles run ahead of the products
-                if (t < nblk) {
-                    const int st = t & 1;
-                    AT2_T(0, tc::mbar_wait(k_empty + st, ((t >> 1) & 1) ^ 1));
-                    tc::mbar_arrive_expect_tx(k_full + st, AT_TILE);
-                    tc::tma_load_2d(smem + At2Smem::K + st * AT_TILE, &tmK, k_full + st, k_col0 + h * AT_D, b * Pk + t * AT_N);
-                }
-                if (t >= 1) {
-                    const int j = t - 1, st = j & 1;
-                    AT2_T(1, tc::mbar_wait(v_empty + st, ((j >> 1) & 1) ^ 1));
-                    tc::mbar_arrive_expect_tx(v_full + st, AT_TILE);
-                    tc::tma_load_2d(smem + At2Smem::VT + st * AT_TILE, &tmV, v_full + st, v_col0 + h * AT_D, b * Pk + j * AT_N);
-                }
-            }
-            if (tr) { g_at_trace[0] = acc[0]; g_at_trace[1] = acc[1]; g_at_trace[2] = 0; g_at_trace[3] = (unsigned)clock() - t_start; }
-        }
-    } else if (warp == AT_SM_WARPS + 1) {
-        // ============================== MMA issuer ==============================
-        if (lane == 0) {
-            constexpr uint32_t idesc_s = tc::instr_desc(2, 128, AT_N);
-            constexpr uint32_t idesc_o = tc::instr_desc(2, 128, AT_D) | (1u << 16);      // B (= V tile, [key][dim] rows of 128 B) is MN-major: no transposed copy of V
-            const uint64_t qdesc = tc::smem_desc_sw128(tc::smem_u32(smem + At2Smem::Q));
-            tc::mbar_wait(q_full, 0);
-            auto issue_s = [&](int it) {                            // S[it&1] = Q K_it^T
-                const int st = it & 1, s3 = it % 3;
-                AT2_T(0, tc::mbar_wait(k_full + st, (it >> 1) & 1));
-                AT2_T(1, tc::mbar_wait(s_empty + s3, ((it / 3) & 1) ^ 1));
-                tc::tcgen05_fence_after();
-                const uint64_t kdesc = tc::smem_desc_sw128(tc::smem_u32(smem + At2Smem::K + st * AT_TILE));
-#pragma unroll
-                for (int kk = 0; kk < 4; ++kk) tc::mma_tf32(tmem + (uint32_t)(s3 * 128), qdesc + (uint64_t)(kk * 2), kdesc + (uint64_t)(kk * 2), idesc_s, kk ? 1u : 0u);
-                tc::mma_commit(k_empty + st);
-                tc::mma_commit(s_full + s3);
-            };
-            issue_s(0);
-            if (nblk > 1) issue_s(1);
-            for (int j = 0; j < nblk; ++j) {
-                if (j + 2 < nblk) issue_s(j + 2);                   // two blocks ahead: queued in front of P_j V_j, ready long before the softmax wants it
-                const int st = j & 1;
-                AT2_T(2, tc::mbar_wait(v_full + st, (j >> 1) & 1));
-                AT2_T(3, tc::mbar_wait(p_full + st, (j >> 1) & 1));
-                AT2_T(4, tc::mbar_wait(o_empty + st, ((j >> 1) & 1) ^ 1));    // the owners have folded Oblk_{j-2} into their registers
-                tc::tcgen05_fence_after();
-                const uint32_t pa = tc::smem_u32(smem + At2Smem::P + st * 4 * AT_TILE), va = tc::smem_u32(smem + At2Smem::VT + st * AT_TILE);
-#pragma unroll
-                for (int kk = 0; kk < 16; ++kk) {
-                    const uint64_t pdesc = tc::smem_desc_sw128(pa + (kk >> 2) * AT_TILE) + (uint64_t)((kk & 3) * 2);
-                    // V tile as TMA wrote it: [key][32 dims] rows of 128 B = an MN-major B operand.  For tf32 the only MN-major layout is
-                    // "128-byte swizzle, 32-byte atoms" (descriptor layout type 1; TMA SWIZZLE_128B_ATOM_32B): 4-key groups 512 B apart
-                    // (SBO), one 128-byte chunk along N (LBO unused but must be a multiple of 32 B: 0), 8 keys = 1024 B per K step
-                    const uint64_t vdesc = (uint64_t)(((va + kk * 1024) >> 4) & 0x3FFF) | ((uint64_t)(512 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)1 << 61);
-                    tc::mma_tf32(tmem_ob[st], pdesc, vdesc, idesc_o, kk ? 1u : 0u);       // block product only: no cross-block accumulation
-                }
-                tc::mma_commit(v_empty + st);
-                tc::mma_commit(p_empty + st);
-                tc::mma_commit(o_full + st);
-            }
-            if (tr) { for (int i = 0; i < 6; ++i) g_at_trace[8 + i] = acc[i]; g_at_trace[14] = (unsigned)clock() - t_start; }
-        }
-    } else if (warp < AT_SM_WARPS) {
-        // ============================== softmax / accumulate: thread = (query row, 32-key column group) ==============================
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 112;");
-        const int qq = warp & 3, cg = warp >> 2;
-        const int row = qq * 32 + lane;
-        const int qi = q0 + row;
-        const uint32_t lane_base = (uint32_t)(qq * 32) << 16;
-        const unsigned char* mrow = kpm ? kpm + (size_t)b * Pk : nullptr;
-        float* red = reinterpret_cast<float*>(smem + At2Smem::RED);
-        const int c0 = cg * 32;
-        const float LOG2E = 1.4426950408889634f;
-        float m_run = -INFINITY, lpart = 0.f, alpha_prev = 0.f;
-        float o[8];                                                 // this thread's 8 of the row's 32 output dims: [cg*8, cg*8+8)
-#pragma unroll
-        for (int d = 0; d < 8; ++d) o[d] = 0.f;
-        unsigned char* pbase0 = smem + At2Smem::P + cg * AT_TILE + (row >> 3) * 1024 + (row & 7) * 128;
-        // Software pipeline inside the thread: the TMEM read of S_{j+1} is issued BEFORE the exp2 phase of block j and completes under it
-        // (the four warps of an SM sub-partition are the four column groups of one row quarter and run in lockstep through the row-max
-        // exchange, so nothing else would hide that latency there).  sa / sb alternate as "this block" / "next block".
-        auto issue_half = [&](int jn, int half, float (&dst)[32]) {     // 16 of the thread's 32 score columns of block jn: TMEM -> registers, not waited for
-            const int sn = jn % 3;
-            if (half == 0) { AT2_T(0, tc::mbar_wait(s_full + sn, (jn / 3) & 1)); }
-            tc::tcgen05_fence_after();
-            uint32_t* r = reinterpret_cast<uint32_t*>(dst) + half * 16;
-            asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                         : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-                           "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                         : "r"(tmem + (uint32_t)(sn * 128) + lane_base + (uint32_t)(c0 + half * 16)));
-        };
-        auto mask_byte = [&](int jn) -> unsigned {                   // lane-parallel mask read: one byte per lane, 32 keys per warp; the RAW byte is kept
-            const int mkey = jn * AT_N + c0 + lane;                 // in a register and only tested at the ballot one block later (load latency hidden)
-            return mkey >= Pk ? 1u : (mrow ? (unsigned)__ldg(mrow + mkey) : 0u);
-        };
-        unsigned mk_next = mask_byte(0);
-        auto block = [&](int j, float (&sc)[32], float (&scn)[32]) {
-            const int st = j & 1;
-            const unsigned tb0 = tr ? (unsigned)clock() : 0u;
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");          // S_j (issued one block ago) is in sc
-            tc::tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) tc::mbar_arrive(s_empty + j % 3);        // the scores are in registers: the tensor core may overwrite this S buffer
-            const uint32_t mb = __ballot_sync(0xffffffffu, mk_next != 0u); // bit c = key c of this thread's 32-key column group is masked
-            float lm = -INFINITY;
-            if (mb == 0u) {
-#pragma unroll
-                for (int c = 0; c < 32; ++c) lm = fmaxf(lm, sc[c]);
-            } else if (mb != 0xffffffffu) {
-#pragma unroll
-                for (int c = 0; c < 32; ++c)
-                    if (!((mb >> c) & 1u)) lm = fmaxf(lm, sc[c]);
-            }
-            float* rb = red + st * 512;
-            rb[cg * 128 + row] = lm;
-            if (tr) acc[1] += (unsigned)clock() - tb0;
-            AT2_T(2, asm volatile("bar.sync %0, 128;" ::"r"(1 + qq) : "memory"));      // only the row's 4 column-group warps
-            const bool more = j + 1 < nblk;
-            if (more) mk_next = mask_byte(j + 1);
-            const unsigned te0 = tr ? (unsigned)clock() : 0u;
-            const float bm = fmaxf(fmaxf(rb[row], rb[128 + row]), fmaxf(rb[256 + row], rb[384 + row]));
-            const float m_new = fmaxf(m_run, bm);
-            const float alpha = (m_run == -INFINITY) ? 0.f : ex2_approx((m_run - m_new) * LOG2E);
-            const float ms = m_new * LOG2E;
-            float psum = 0.f;
-            tc::mbar_wait(p_empty + st, ((j >> 1) & 1) ^ 1);        // the tensor core has consumed P_{j-2} (long ago)
-            unsigned char* pk = pbase0 + st * 4 * AT_TILE;
-            // two halves of 16 columns: exp2 -> st.shared; the registers of a finished half are reused for the same half of S_{j+1}, whose
-            // TMEM read then runs under the rest of this block (the sub-partition's four warps are in lockstep: nothing else hides it)
-#pragma unroll
-            for (int half = 0; half < 2; ++half) {
-                if (mb == 0u) {
-#pragma unroll
-                    for (int c = half * 16; c < half * 16 + 16; ++c) { sc[c] = ex2_approx(fmaf(sc[c], LOG2E, -ms)); psum += sc[c]; }
-                } else if (mb == 0xffffffffu) {
-#pragma unroll
-                    for (int c = half * 16; c < half * 16 + 16; ++c) sc[c] = 0.f;
-                } else {
-#pragma unroll
-                    for (int c = half * 16; c < half * 16 + 16; ++c) {
-                        const float pv = ((mb >> c) & 1u) ? 0.f : ex2_approx(fmaf(sc[c], LOG2E, -ms));
-                        psum += pv;
-                        sc[c] = pv;
-                    }
-                }
-#pragma unroll
-                for (int ch = half * 4; ch < half * 4 + 4; ++ch)
-                    *reinterpret_cast<float4*>(pk + ((ch ^ (row & 7)) << 4)) = make_float4(sc[4 * ch], sc[4 * ch + 1], sc[4 * ch + 2], sc[4 * ch + 3]);
-                if (more) issue_half(j + 1, half, scn);
-            }
-            lpart = lpart * alpha + psum;
-            m_run = m_new;
-            if (tr) acc[3] += (unsigned)clock() - te0;
-            uint32_t obr[8];
-            const unsigned tw0 = tr ? (unsigned)clock() : 0u;
-            if (j >= 1) {                                           // the PREVIOUS block's product: start its TMEM read, fold it in below
-                const int so = (j - 1) & 1;
-                AT2_T(6, tc::mbar_wait(o_full + so, ((j - 1) >> 1) & 1));
-                tc::tcgen05_fence_after();
-                asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                             : "=r"(obr[0]), "=r"(obr[1]), "=r"(obr[2]), "=r"(obr[3]), "=r"(obr[4]), "=r"(obr[5]), "=r"(obr[6]), "=r"(obr[7])
-                             : "r"(tmem_ob[so] + lane_base + (uint32_t)(cg * 8)));
-            }
-            tc::fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) tc::mbar_arrive(p_full + st);
-            if (tr) acc[5] += (unsigned)clock() - tw0;
-            if (j >= 1) {
-                const unsigned tf0 = tr ? (unsigned)clock() : 0u;
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");      // Oblk_{j-1} (and S_{j+1}, long since) have landed
-                tc::tcgen05_fence_before();
-                __syncwarp();
-                if (lane == 0) tc::mbar_arrive(o_empty + ((j - 1) & 1));
-#pragma unroll
-                for (int d = 0; d < 8; ++d) o[d] = fmaf(o[d], alpha_prev, __uint_as_float(obr[d]));      // O scaled to m_{j-1}
-                if (tr) acc[7] += (unsigned)clock() - tf0;
-            }
-            alpha_prev = alpha;                                      // = exp2(m_{j-1} - m_j): applied when Oblk_j is folded in
-        };
-        float sa[32], sb[32];
-        issue_half(0, 0, sa);
-        issue_half(0, 1, sa);
-        for (int j = 0; j < nblk; j += 2) {
-            block(j, sa, sb);
-            if (j + 1 < nblk) block(j + 1, sb, sa);
-        }
-        if (tr && threadIdx.x == 0) { for (int i = 0; i < 8; ++i) g_at_trace[16 + i] = acc[i]; g_at_trace[24] = nblk; g_at_trace[25] = (unsigned)clock() - t_start; }
-        red[1024 + cg * 128 + row] = lpart;
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + qq) : "memory");
-        {
-            const int so = (nblk - 1) & 1;
-            tc::mbar_wait(o_full + so, ((nblk - 1) >> 1) & 1);
-            tc::tcgen05_fence_after();
-            float ob[8];
-            tmem_ld8(tmem_ob[so] + lane_base + (uint32_t)(cg * 8), ob);
-            const float lsum = (red[1024 + row] + red[1024 + 128 + row]) + (red[1024 + 256 + row] + red[1024 + 384 + row]);
-            if (qi < Pq) {
-                float* op = out + ((size_t)b * Pq + qi) * ldo + h * AT_D + cg * 8;
-                const float inv = 1.f / lsum;                       // lsum == 0 (every key masked): NaN, like softmax of all -inf
-#pragma unroll
-                for (int d = 0; d < 8; d += 4) {
-                    float4 r = make_float4(fmaf(o[d], alpha_prev, ob[d]) * inv, fmaf(o[d + 1], alpha_prev, ob[d + 1]) * inv,
-                                           fmaf(o[d + 2], alpha_prev, ob[d + 2]) * inv, fmaf(o[d + 3], alpha_prev, ob[d + 3]) * inv);
-                    if (lsum == 0.f) r = make_float4(NAN, NAN, NAN, NAN);
-                    *reinterpret_cast<float4*>(op + d) = r;
-                }
-            }
-        }
-    }
-    tc::tcgen05_fence_before();
-    __syncthreads();
-    if (warp == AT_SM_WARPS + 1) tc::tmem_dealloc<512>(tmem);
 }
 
 int dz_attention_fwd_tc(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, const unsigned char* kpm, int B,
@@ -631,33 +229,28 @@ int dz_attention_fwd_tc(const float* q, int ldq, const float* k, int ldk, const 
     }
     tc::EncodeTiledFn enc = tc::get_encode_tiled();
     if (!enc) { dz_set_error("cuTensorMapEncodeTiled unavailable"); return DZ_ERR_CUDA; }
-    CUtensorMap tmQ, tmK, tmV;
-    const float* ptrs[3] = {q, k, v};
-    const int lds[3] = {ldq, ldk, ldv};
-    const long long rows[3] = {(long long)B * Pq, (long long)B * Pk, (long long)B * Pk};
-    CUtensorMap* maps[3] = {&tmQ, &tmK, &tmV};
-    for (int i = 0; i < 3; ++i) {
+    CUtensorMap tmQ, tmK;
+    const float* ptrs[2] = {q, k};
+    const int lds[2] = {ldq, ldk};
+    const long long rows[2] = {(long long)B * Pq, (long long)B * Pk};
+    CUtensorMap* maps[2] = {&tmQ, &tmK};
+    for (int i = 0; i < 2; ++i) {
         // the head slice starts at column h*32 of a row of ld floats; the map covers the H*32 columns reachable from the base pointer
         cuuint64_t dims[2] = {(cuuint64_t)(H * AT_D), (cuuint64_t)rows[i]};
         cuuint64_t strides[1] = {(cuuint64_t)lds[i] * 4};
         cuuint32_t box[2] = {AT_D, AT_M};
         cuuint32_t estr[2] = {1, 1};
         CUresult r = enc(maps[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)ptrs[i], dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         (i == 2) ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { dz_set_error("cuTensorMapEncodeTiled(attention %d) failed: %d", i, (int)r); return DZ_ERR_CUDA; }
     }
     static bool configured = false;
     if (!configured) {
         DZ_CUDA(cudaFuncSetAttribute(k_attention_tf32, cudaFuncAttributeMaxDynamicSharedMemorySize, AtSmem::TOTAL));
-        DZ_CUDA(cudaFuncSetAttribute(k_attention_tf32_v2<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, At2Smem::TOTAL));
-        DZ_CUDA(cudaFuncSetAttribute(k_attention_tf32_v2<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, At2Smem::TOTAL));
         configured = true;
     }
     dim3 grid(dz_cdiv(Pq, AT_M), B * H);
-    static const int two_pass = getenv("DZ_ATTN_TWO_PASS") ? atoi(getenv("DZ_ATTN_TWO_PASS")) : 0;      // the round-1/2 two-pass kernel, kept for A/B
-    if (two_pass) k_attention_tf32<<<grid, AT_THREADS, AtSmem::TOTAL, st>>>(tmQ, tmK, 0, 0, v, ldv, kpm, Pq, Pk, H, out, ldo);
-    else if (g_at_on_host) k_attention_tf32_v2<true><<<grid, AT2_THREADS, At2Smem::TOTAL, st>>>(tmQ, tmK, tmV, 0, 0, 0, kpm, Pq, Pk, H, out, ldo);
-    else k_attention_tf32_v2<false><<<grid, AT2_THREADS, At2Smem::TOTAL, st>>>(tmQ, tmK, tmV, 0, 0, 0, kpm, Pq, Pk, H, out, ldo);
+    k_attention_tf32<<<grid, AT_THREADS, AtSmem::TOTAL, st>>>(tmQ, tmK, v, ldv, kpm, Pq, Pk, H, out, ldo);
     DZ_LAUNCH_CHECK();
     return DZ_OK;
 }

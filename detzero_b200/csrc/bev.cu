@@ -1,4 +1,4 @@
-// bev.cu -- sparse->dense BEV scatter and NHWC conv2d / deconv2d (exact-fp32 SIMT path), sm_100a.
+// bev.cu -- sparse->dense BEV scatter and NHWC conv2d / deconv2d (exact-fp32 SIMT path), sm_90a.
 //
 // Replaces HeightCompression.forward (height_compression.py:20-25: SparseConvTensor.dense() + reshape), the
 // ZeroPad2d+Conv2d+BatchNorm2d+ReLU stacks and ConvTranspose2d deblocks of BaseBEVBackbone
@@ -7,7 +7,7 @@
 // Layout: dense maps are NHWC so that a pixel's channel vector is one contiguous 128-bit-loadable run and the
 // implicit-GEMM K dimension (tap, cin) is contiguous; BatchNorm (eval) + bias + ReLU are folded into the epilogue
 // and torch.cat of the deblock outputs (backbone2d.py:107-108) is fused as a channel-offset write.
-// DZ_F32 here is the exact-fp32 path; the tcgen05 tensor-core path lives in conv2d_tc.cu.
+// DZ_F32 here is the exact-fp32 path; the wgmma tensor-core path lives in conv2d_tc.cu.
 #include <stdlib.h>
 #include "common.cuh"
 #include "conv2d.cuh"

@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for libdetzero_b200 (sm_100a).
+// common.cuh -- shared helpers for libdetzero_b200 (sm_90a).
 #pragma once
 #include <stdlib.h>
 #include <cuda_runtime.h>
@@ -6,7 +6,7 @@
 #include <stdio.h>
 #include "../../include/detzero_b200.h"
 
-#define DZ_NUM_SMS 148
+#define DZ_NUM_SMS 132
 
 void dz_set_error(const char* fmt, ...);
 

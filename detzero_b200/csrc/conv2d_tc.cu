@@ -1,16 +1,17 @@
-// conv2d_tc.cu -- NHWC conv2d as a tcgen05 implicit GEMM (TF32 inputs, fp32 accumulation in TMEM), sm_100a.
+// conv2d_tc.cu -- NHWC conv2d as a wgmma implicit GEMM (TF32 inputs, fp32 register accumulation), sm_90a.
 //
 // Replaces the cuDNN convolutions of BaseBEVBackbone / CenterHead (backbone2d.py:34-81, center_head.py:25-31,81-88);
 // the reference runs them with TF32 tensor cores too (torch.backends.cudnn.allow_tf32 defaults to True, SURVEY A.6).
 //
 // Design: output tile = 8 x 16 pixel patch (M = 128) x BN output channels.  For every filter tap (r,s) and every
 // 32-channel slice of Cin, ONE 4-D TMA box load of the shifted input patch lands in shared memory already in the
-// canonical K-major 128B-swizzled UMMA layout (row = pixel, 128 B = 32 fp32 channels); out-of-image pixels are
+// canonical K-major 128B-swizzled layout (row = pixel, 128 B = 32 fp32 channels); out-of-image pixels are
 // zero-filled by the TMA unit, which implements the conv padding (and ZeroPad2d) for free.  Weights are a 2-D TMA
-// load of W[cout][(r,s,cin)].  One elected thread issues tcgen05.mma (M=128, N=BN, K=8) into a TMEM accumulator;
-// a ring of mbarrier-guarded stages overlaps TMA with MMA; 4 epilogue warps read TMEM (tcgen05.ld), apply the
-// folded BatchNorm / bias / ReLU and write NHWC rows (optionally into a channel slice / strided pixels: fused
-// torch.cat and ConvTranspose2d with kernel == stride).
+// load of W[cout][(r,s,cin)].  Two consumer warpgroups (64 pixels each) issue wgmma (M=64, N=BN, K=8) into register
+// accumulators; a ring of mbarrier-guarded stages overlaps TMA with MMA.  After the main loop the accumulators go to a
+// shared-memory tile and the same 8 warps run the epilogue (each one quarter of the pixels and half of the channels):
+// folded BatchNorm / bias / ReLU, NHWC rows written through TMA stores (optionally into a channel slice / strided pixels:
+// fused torch.cat and ConvTranspose2d with kernel == stride), or a fused max over row groups.
 #include <stdlib.h>
 #include "common.cuh"
 #include "conv2d.cuh"
@@ -31,101 +32,65 @@ EncodeTiledFn get_encode_tiled() {
 
 static constexpr int CT_TH = 8, CT_TW = 16, CT_BK = 32;       // pixel patch, channels per k-step group (128 B)
 static constexpr int CT_A_BYTES = CT_TH * CT_TW * CT_BK * 4;  // 16 KB
-static constexpr int CT_THREADS = 320;                        // warp0 TMA, warp1 MMA+TMEM, warps 2-5 and 6-9 epilogue (one half of the
-                                                              // accumulator columns each: the epilogue of a single-tile CTA is not overlapped
-                                                              // with anything, so it is spread over 8 warps)
+static constexpr int CT_CONSUMERS = 8;                        // warps 0-7: two wgmma warpgroups, then the epilogue
+static constexpr int CT_THREADS = 32 * (CT_CONSUMERS + 1);    // warp 8: TMA producer
 
-// OCC = CTAs per SM the shared-memory budget is cut for: with many tiles per SM (batched frames) two co-resident
-// single-patch CTAs overlap one CTA's epilogue / set-up with the other's main loop
-template <int BN, int MT, int OCC = 1>
+// HALO variant (3x3 stride-1 convolutions, 16 of the 22 dense convs of the BEV backbone + head).  The generic kernel re-reads its
+// 128-pixel activation patch from L2 once per filter tap: 9 x 16 KB per 32-channel slice.  The halo kernel loads the (16+2) x (8+2)
+// pixel HALO of a 16 x 8 output patch ONCE per 32-channel slice (23 KB) and the nine taps are nine A descriptors into that one tile:
+// a K-major SW128 descriptor may start at any 128-byte pixel row, its 8-row core groups are the 8-pixel rows of the patch, and the
+// stride between groups (SBO) is the halo's row pitch, 10 pixels = 1280 B.  The 128-byte swizzle is a function of the absolute
+// shared-memory address for the TMA unit and for wgmma alike, so a window shifted by (r, s) reads exactly the bytes the TMA unit wrote
+// for pixel (y + r, x + s) with the descriptor's base-offset field left at 0 (measured: the field set to (start >> 7) & 7 gives
+// wrong results; the conv2d tests cover every tile width).
+static constexpr int HL_TH = 16, HL_TW = 8, HL_PITCH = HL_TW + 2, HL_ROWS = HL_TH + 2;
+static constexpr int HL_A_BYTES = HL_ROWS * HL_PITCH * 128;          // 23040 B delivered by the TMA unit
+static constexpr int HL_A_SLOT = (HL_A_BYTES + 1023) / 1024 * 1024;  // 23552: slots stay 1024-byte aligned (swizzle phase)
+static constexpr int HL_A_STAGES = 2;
+
+template <int BN, bool HALO>
 struct CtCfg {
+    static constexpr int TH = HALO ? HL_TH : CT_TH, TW = HALO ? HL_TW : CT_TW;        // output patch (TH x TW = 128 pixels)
     static constexpr int B_BYTES = BN * CT_BK * 4;
-    static constexpr int STAGE_BYTES = MT * CT_A_BYTES + B_BYTES;
-    static constexpr int BUDGET = OCC == 1 ? 200 * 1024 : 104 * 1024;
-    static constexpr int STAGES = BUDGET / STAGE_BYTES > 8 ? 8 : BUDGET / STAGE_BYTES;
-    static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-    static constexpr int TMEM_COLS = (MT * BN) < 32 ? 32 : MT * BN;      // MT accumulators side by side
+    static constexpr int ACC_LD = BN + 4;                               // row pitch of the staged accumulator tile
+    static constexpr int ACC_BYTES = CT_TH * CT_TW * ACC_LD * 4;
+    static constexpr int BUDGET = 227 * 1024 - 1024 - 256 - ACC_BYTES;  // H100: 227 KB of shared memory per block
+    // generic: STAGES x (A patch + B tile); halo: HL_A_STAGES halo slots + STAGES B tiles
+    static constexpr int STAGE_BYTES = HALO ? B_BYTES : CT_A_BYTES + B_BYTES;
+    static constexpr int A_REGION = HALO ? HL_A_STAGES * HL_A_SLOT : 0;
+    static constexpr int FIT = (BUDGET - A_REGION) / STAGE_BYTES;
+    static constexpr int STAGES = FIT > (HALO ? 9 : 8) ? (HALO ? 9 : 8) : FIT;
+    static constexpr int BUF = A_REGION + STAGES * STAGE_BYTES;         // pipeline buffers (epilogue staging slots afterwards)
+    static constexpr int SMEM = BUF + ACC_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 };
 
-// MT = output patches per CTA (stacked in y): the weight tile of every k-step is shared by MT accumulators, which cuts the
-// L2->SM bytes per MMA (the kernel is bound by the ~34 B/clk/SM an SM can pull from L2, not by the tensor pipe)
-__device__ long long g_ct_trace[64];          // DZ_CONV2D_DBG & 4: clock stamps of CTA 0 (tools/bench_conv2d.py)
+__device__ long long g_ct_trace[64];          // DZ_CONV2D_DBG & 4: clock stamps of CTA 0 (dz_debug_conv2d_trace)
 extern "C" int dz_debug_conv2d_trace(long long* host) {
     cudaDeviceSynchronize();
     return cudaMemcpyFromSymbol(host, g_ct_trace, sizeof(long long) * 64) == cudaSuccess ? 0 : -1;
 }
 
-// ---- CTA-pair variant (TWO = 1): a cluster of 2 CTAs (the two SMs of a TPC) owns two M tiles and ONE BN-wide weight tile.  Each CTA loads
-// its own activation patch and HALF of the weight rows (TMA .cta_group::2: the bytes of both CTAs complete on the leader's mbarrier);
-// the leader's MMA thread issues tcgen05.mma.cta_group::2 (M = 256 = 128 rows per CTA, N = BN) and its commits are multicast to both
-// CTAs' barriers.  Per SM and MMA the shared-memory port then moves A 4 KB + B BN/2 x 32 B (written once, read once) instead of
-// A 4 KB + B BN x 32 B: with TF32 operands the single-CTA kernel spends 128 clk of port time per 64 clk of tensor-pipe time at BN = 128
-// (profiles/r02_ncu_full_conv2d_batch8.json: 50-57 % tensor pipe); the pair needs 96, and at BN = 256 (Cout = 256 layers) 128 per 128.
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-template <int NCOLS> __device__ __forceinline__ void tmem_alloc2(uint32_t* smem_dst) {          // one full warp in EACH CTA of the pair
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tc::smem_u32(smem_dst)), "n"(NCOLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int NCOLS> __device__ __forceinline__ void tmem_dealloc2(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-__device__ __forceinline__ void mma2_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void mma2_commit_multicast(uint64_t* bar, uint16_t cta_mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(tc::smem_u32(bar)), "h"(cta_mask) : "memory");
-}
-// TMA loads of a CTA pair: the transaction bytes go to the mbarrier of the pair's LEADER (bit 24 of the shared::cluster address
-// selects the CTA inside the pair; same trick as CUTLASS' SM100_TMA_2SM_LOAD)
-__device__ __forceinline__ void tma2_load_2d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(tc::smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(tc::smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tma2_load_4d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(tc::smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(tc::smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-
-template <int BN, int MT, int OCC, int TWO>
-struct CtKCfg {
-    static constexpr int B_ROWS = TWO ? BN / 2 : BN;                     // weight rows this CTA holds
-    static constexpr int B_BYTES = B_ROWS * CT_BK * 4;
-    static constexpr int STAGE_BYTES = MT * CT_A_BYTES + B_BYTES;
-    static constexpr int BUDGET = OCC == 1 ? 200 * 1024 : 104 * 1024;
-    static constexpr int STAGES = BUDGET / STAGE_BYTES > 8 ? 8 : BUDGET / STAGE_BYTES;
-    static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-    static constexpr int TMEM_COLS = (MT * BN) < 32 ? 32 : MT * BN;
-};
-
-template <int BN, int MT, int OCC, int TWO>
-__device__ __forceinline__ void conv2d_tf32_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO,
-                                                 const Conv2dParams& p, int tiles_x, int tiles_y, int tiles_total) {
-    using Cfg = CtKCfg<BN, MT, OCC, TWO>;
+template <int BN, bool HALO>
+__global__ void __launch_bounds__(CT_THREADS, 1)
+k_conv2d_tf32(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
+              Conv2dParams p, int tiles_x, int tiles_y) {
+    using Cfg = CtCfg<BN, HALO>;
+    constexpr int TH = Cfg::TH, TW = Cfg::TW;
     extern __shared__ unsigned char smem_raw[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
+    unsigned char* smB = smem + Cfg::A_REGION;                              // halo: the B ring follows the halo slots
+    float* acc_stg = reinterpret_cast<float*>(smem + Cfg::BUF);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::BUF + Cfg::ACC_BYTES);
     uint64_t* empty = full + Cfg::STAGES;
-    uint64_t* tmem_full = empty + Cfg::STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);
+    uint64_t* a_full = empty + Cfg::STAGES;                                 // halo slots
+    uint64_t* a_empty = a_full + HL_A_STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const bool tr = (p.dbg & 4) && blockIdx.x == 0 && blockIdx.y == 0;
     if (tr && threadIdx.x == 0) g_ct_trace[0] = clock64();
-    int mt = min((int)blockIdx.x, tiles_total - 1);         // pair kernel: an odd tile count is padded with a duplicate of the last tile
-    const uint32_t rank = TWO ? cluster_ctarank() : 0u;     // (it recomputes and re-stores identical values)
-    const int tx0 = (mt % tiles_x) * CT_TW; mt /= tiles_x;
-    const int ty0 = (mt % tiles_y) * (CT_TH * MT);
+    int mt = blockIdx.x;
+    const int tx0 = (mt % tiles_x) * TW; mt /= tiles_x;
+    const int ty0 = (mt % tiles_y) * TH;
     const int b = mt / tiles_y;
     const int n0 = blockIdx.y * BN;
     const int cchunks = p.cin / CT_BK;
@@ -135,116 +100,120 @@ __device__ __forceinline__ void conv2d_tf32_body(const CUtensorMap& tmA, const C
         tc::prefetch_tmap(&tmA);
         tc::prefetch_tmap(&tmB);
         if (p.tma_store) tc::prefetch_tmap(&tmO);
-        for (int s = 0; s < Cfg::STAGES; ++s) { tc::mbar_init(full + s, 1); tc::mbar_init(empty + s, 1); }
-        tc::mbar_init(tmem_full, 1);
+        for (int s = 0; s < Cfg::STAGES; ++s) { tc::mbar_init(full + s, 1); tc::mbar_init(empty + s, CT_CONSUMERS); }
+        if (HALO) for (int s = 0; s < HL_A_STAGES; ++s) { tc::mbar_init(a_full + s, 1); tc::mbar_init(a_empty + s, CT_CONSUMERS); }
         tc::fence_barrier_init();
     }
-    if (TWO) { __syncthreads(); cluster_sync_all(); }       // both CTAs' barriers exist before anything cluster-scoped touches them
-    if (warp == 1) { if (TWO) tmem_alloc2<Cfg::TMEM_COLS>(tmem_slot); else tc::tmem_alloc<Cfg::TMEM_COLS>(tmem_slot); }
-    tc::tcgen05_fence_before();
     __syncthreads();
-    tc::tcgen05_fence_after();
-    if (TWO) cluster_sync_all();
-    const uint32_t tmem_base = *tmem_slot;
     if (tr && threadIdx.x == 0) g_ct_trace[1] = clock64();
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp == CT_CONSUMERS) {
+        if (HALO && lane == 0) {
+            int bit = 0;
+            for (int cc = 0; cc < cchunks; ++cc) {
+                const int a = cc % HL_A_STAGES;
+                tc::mbar_wait(a_empty + a, ((cc / HL_A_STAGES) & 1) ^ 1);
+                tc::mbar_arrive_expect_tx(a_full + a, HL_A_BYTES);
+                tc::tma_load_4d(smem + a * HL_A_SLOT, &tmA, a_full + a, cc * CT_BK, tx0 - p.pad, ty0 - p.pad, b);
+                for (int tap = 0; tap < 9; ++tap, ++bit) {
+                    const int s = bit % Cfg::STAGES;
+                    tc::mbar_wait(empty + s, ((bit / Cfg::STAGES) & 1) ^ 1);
+                    tc::mbar_arrive_expect_tx(full + s, Cfg::B_BYTES);
+                    tc::tma_load_2d(smB + s * Cfg::B_BYTES, &tmB, full + s, tap * p.cin + cc * CT_BK, n0);
+                }
+            }
+        } else if (lane == 0) {
             for (int it = 0; it < iters; ++it) {
                 const int s = it % Cfg::STAGES;
                 tc::mbar_wait(empty + s, ((it / Cfg::STAGES) & 1) ^ 1);
                 unsigned char* sa = smem + s * Cfg::STAGE_BYTES;
-                unsigned char* sb = sa + MT * CT_A_BYTES;
+                unsigned char* sb = sa + CT_A_BYTES;
                 const int tap = it / cchunks, cc = it - tap * cchunks;
                 const int r = tap / p.KW, sx = tap - r * p.KW;
                 const bool ldA = !(p.dbg & 2) || it < Cfg::STAGES, ldB = !(p.dbg & 1) || it < Cfg::STAGES;
-                if (TWO) {
-                    // the leader's barrier collects the bytes of BOTH CTAs (each: its patch + its half of the weight rows)
-                    if (rank == 0) tc::mbar_arrive_expect_tx(full + s, 2 * (MT * CT_A_BYTES + Cfg::B_BYTES));
-#pragma unroll
-                    for (int m = 0; m < MT; ++m)
-                        tma2_load_4d(sa + m * CT_A_BYTES, &tmA, full + s, cc * CT_BK, tx0 * p.stride + sx - p.pad,
-                                     (ty0 + m * CT_TH) * p.stride + r - p.pad, b);
-                    tma2_load_2d(sb, &tmB, full + s, tap * p.cin + cc * CT_BK, n0 + (int)rank * Cfg::B_ROWS);
-                    continue;
-                }
-                tc::mbar_arrive_expect_tx(full + s, (ldA ? MT * CT_A_BYTES : 0) + (ldB ? Cfg::B_BYTES : 0));
-                if (ldA) {
-#pragma unroll
-                    for (int m = 0; m < MT; ++m)
-                        tc::tma_load_4d(sa + m * CT_A_BYTES, &tmA, full + s, cc * CT_BK, tx0 * p.stride + sx - p.pad,
-                                        (ty0 + m * CT_TH) * p.stride + r - p.pad, b);
-                }
+                tc::mbar_arrive_expect_tx(full + s, (ldA ? CT_A_BYTES : 0) + (ldB ? Cfg::B_BYTES : 0));
+                if (ldA) tc::tma_load_4d(sa, &tmA, full + s, cc * CT_BK, tx0 * p.stride + sx - p.pad, ty0 * p.stride + r - p.pad, b);
                 if (ldB) tc::tma_load_2d(sb, &tmB, full + s, tap * p.cin + cc * CT_BK, n0);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0 && TWO) {
-            if (rank == 0) {                                // the pair's leader issues every MMA; its commits reach both CTAs
-                constexpr uint32_t idesc2 = tc::instr_desc(2, 256, BN);
-                for (int it = 0; it < iters; ++it) {
-                    const int s = it % Cfg::STAGES;
-                    tc::mbar_wait(full + s, (it / Cfg::STAGES) & 1);
-                    tc::tcgen05_fence_after();
-                    const uint32_t sa = tc::smem_u32(smem + s * Cfg::STAGE_BYTES);
-                    const uint64_t bdesc = tc::smem_desc_sw128(sa + MT * CT_A_BYTES);
+    } else {
+        // ---- main loop: warpgroup g accumulates pixels [64g, 64g+64) of the patch
+        const int g = warp >> 2;
+        float acc[BN / 2];
 #pragma unroll
-                    for (int m = 0; m < MT; ++m) {
-                        const uint64_t adesc = tc::smem_desc_sw128(sa + m * CT_A_BYTES);
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        if (HALO) {
+            int bit = 0;
+            for (int cc = 0; cc < cchunks; ++cc) {
+                const int a = cc % HL_A_STAGES;
+                tc::mbar_wait(a_full + a, (cc / HL_A_STAGES) & 1);
+                const uint32_t ha = tc::smem_u32(smem + a * HL_A_SLOT);
+                for (int tap = 0; tap < 9; ++tap, ++bit) {
+                    const int s = bit % Cfg::STAGES;
+                    tc::mbar_wait(full + s, (bit / Cfg::STAGES) & 1);
+                    const int r = tap / 3, sx = tap - r * 3;
+                    // window (r, sx) of the halo for pixel rows [64g, 64g+64) = patch rows [8g, 8g+8): 8-pixel rows HL_PITCH pixels apart
+                    const uint32_t a0 = ha + (uint32_t)(((r + 8 * g) * HL_PITCH + sx) * 128);
+                    const uint64_t adesc = tc::smem_desc_sw128(a0, HL_PITCH * 128);
+                    const uint64_t bdesc = tc::smem_desc_sw128(tc::smem_u32(smB + s * Cfg::B_BYTES));
+                    tc::wgmma_fence();
 #pragma unroll
-                        for (int k = 0; k < CT_BK / 8; ++k)
-                            mma2_tf32(tmem_base + (uint32_t)(m * BN), adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc2, (it | k) ? 1u : 0u);
-                    }
-                    mma2_commit_multicast(empty + s, 0b11);
+                    for (int k = 0; k < CT_BK / 8; ++k)
+                        tc::wgmma<BN, tc::K_TF32>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), 1u);
+                    tc::wgmma_commit();
+                    tc::wgmma_wait_one();               // this tap's MMAs stay in flight; the previous tap's weight tile is free
+                    __syncwarp();
+                    if (lane == 0 && bit > 0) tc::mbar_arrive(empty + (bit - 1) % Cfg::STAGES);
+                    // every MMA of the previous slice has completed: its halo slot is free
+                    if (lane == 0 && tap == 0 && cc > 0) tc::mbar_arrive(a_empty + (cc - 1) % HL_A_STAGES);
                 }
-                mma2_commit_multicast(tmem_full, 0b11);
             }
-        } else if (lane == 0) {
-            constexpr uint32_t idesc = tc::instr_desc(2, 128, BN < 16 ? 16 : BN);
+            tc::wgmma_wait_all();
+        } else {
             for (int it = 0; it < iters; ++it) {
                 const int s = it % Cfg::STAGES;
-                if (tr && it < 20) g_ct_trace[8 + it * 2] = clock64();
+                if (tr && threadIdx.x == 0 && it < 20) g_ct_trace[8 + it * 2] = clock64();
                 tc::mbar_wait(full + s, (it / Cfg::STAGES) & 1);
-                if (tr && it < 20) g_ct_trace[9 + it * 2] = clock64();
-                tc::tcgen05_fence_after();
+                if (tr && threadIdx.x == 0 && it < 20) g_ct_trace[9 + it * 2] = clock64();
                 const uint32_t sa = tc::smem_u32(smem + s * Cfg::STAGE_BYTES);
-                const uint64_t bdesc = tc::smem_desc_sw128(sa + MT * CT_A_BYTES);
+                const uint64_t adesc = tc::smem_desc_sw128(sa + g * 64 * 128), bdesc = tc::smem_desc_sw128(sa + CT_A_BYTES);
+                tc::wgmma_fence();
 #pragma unroll
-                for (int m = 0; m < MT; ++m) {
-                    const uint64_t adesc = tc::smem_desc_sw128(sa + m * CT_A_BYTES);
-#pragma unroll
-                    for (int k = 0; k < CT_BK / 8; ++k)        // K = 8 tf32 = 32 bytes per instruction
-                        tc::mma_tf32(tmem_base + (uint32_t)(m * BN), adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc,
-                                     (it | k) ? 1u : 0u);
-                }
-                tc::mma_commit(empty + s);                      // frees the stage once these MMAs have read it
+                for (int k = 0; k < CT_BK / 8; ++k)        // K = 8 tf32 = 32 bytes per instruction
+                    tc::wgmma<BN, tc::K_TF32>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), 1u);
+                tc::wgmma_commit();
+                tc::wgmma_wait_one();                   // this step's MMAs stay in flight; the previous step's stage is free
+                __syncwarp();
+                if (lane == 0 && it > 0) tc::mbar_arrive(empty + (it - 1) % Cfg::STAGES);
             }
-            tc::mma_commit(tmem_full);
-            if (tr) g_ct_trace[2] = clock64();
+            tc::wgmma_wait_all();
         }
-    } else {
-        // epilogue: warp w may only touch TMEM lanes [32*(w%4), 32*(w%4)+32)
+        // (no stage is released after the last step: the producer has nothing left to load)
+        if (tr && threadIdx.x == 0) g_ct_trace[2] = clock64();
+        tc::acc_to_smem<BN>(acc, acc_stg, Cfg::ACC_LD, g * 64);
+        // the pipeline buffers are idle from here on: the epilogue stages its output tiles there
+        tc::named_sync(1, 32 * CT_CONSUMERS);
+        if (tr && threadIdx.x == 0) g_ct_trace[3] = clock64();
+
+        // ---- epilogue: warp w handles pixels [32*(w%4), +32) and channel half w/4 of the accumulator
         const int q = warp & 3;
-        const int row = q * 32 + lane;                          // pixel index inside the 8x16 patch
-        tc::mbar_wait(tmem_full, 0);
-        tc::tcgen05_fence_after();
-        if (tr && threadIdx.x == 64) g_ct_trace[3] = clock64();
-        constexpr int COLS = MT * BN, PER = COLS >= 64 ? COLS / 2 : COLS;
-        const int half = (warp - 2) >> 2;
-        if (half == 1 && COLS < 64) { /* nothing left for the second warp group */ } else
+        const int row = q * 32 + lane;                          // pixel index inside the TH x TW patch
+        constexpr int PER = BN >= 64 ? BN / 2 : BN;
+        const int half = warp >> 2;
+        const int y = ty0 + row / TW, x = tx0 + row % TW;
+        const bool valid = (y < p.Ho) && (x < p.Wo);
+        if (half == 1 && BN < 64) { /* nothing left for the second warp group */ } else
 #pragma unroll 1
         for (int mc = half * PER; mc < half * PER + PER; mc += 32) {
-            const int m = mc / BN, c0 = mc % BN;
-            const int y = ty0 + m * CT_TH + row / CT_TW, x = tx0 + row % CT_TW;
-            const bool valid = (y < p.Ho) && (x < p.Wo);
+            const int c0 = mc;
             float* orow = p.out + (((size_t)b * p.OH + (y * p.os + p.oy0)) * p.OW + (x * p.os + p.ox0)) * p.out_cstride + p.out_coff;
             float v[32];
-            tc::tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)mc, v);
+            tc::smem_row32(acc_stg, Cfg::ACC_LD, row, mc, v);
             if (p.gmax) {
                 // fused max-pool over the points of a crop (torch.max(dim=points), position_transformer.py:109,118): the 128 rows of this
                 // tile belong to ONE group (gmax_rows % 128 == 0); warp-shuffle max over its 32 rows per column, one atomic per warp and
                 // column.  The (rows, cout) activation is never written to HBM, the group_max pass never reads it back.
-                const int grp = (p.grow0 + (ty0 + m * CT_TH) * p.Wo + tx0) / p.gmax_rows;
+                const int grp = (p.grow0 + ty0 * p.Wo + tx0) / p.gmax_rows;
                 // transpose through the (idle) pipeline buffers: row stride 33 floats => conflict-free scalar stores and column reads
                 float* stg = reinterpret_cast<float*>(smem + ((mc / 32) * 4 + q) * 4352);
 #pragma unroll
@@ -270,13 +239,12 @@ __device__ __forceinline__ void conv2d_tf32_body(const CUtensorMap& tmA, const C
                 }
                 __syncwarp();
             } else if (p.tma_store) {
-                // The strided per-pixel stores of the direct path (32 lanes -> 32 different lines per instruction) made the
-                // epilogue as long as the main loop.  Here the warp's 32 pixels x 32 channels go to the (now idle) pipeline
-                // buffers in the 128B-swizzled box layout and ONE TMA store per warp writes them (edge tiles clipped by the
-                // tensor map, channel range clipped at out_coff + cout).
-                // staging slots (16 KB each, 4 KB per warp) are carved from the pipeline buffers; each warp group owns half of them and a
-                // warp re-uses its 4 KB only after its own earlier TMA store has read it (BN = 256 pair kernel: 4 chunks, 3 slots per group)
-                constexpr int SLOTS_H = (Cfg::STAGES * Cfg::STAGE_BYTES / CT_A_BYTES) / 2;
+                // Per-pixel strided stores (32 lanes -> 32 different lines per instruction) would make the epilogue as long as the
+                // main loop.  Here the warp's 32 pixels x 32 channels go to the (now idle) pipeline buffers in the 128B-swizzled box
+                // layout and ONE TMA store per warp writes them (edge tiles clipped by the tensor map, channel range clipped at
+                // out_coff + cout).  Staging slots (16 KB each, 4 KB per warp) are carved from the pipeline buffers; each warp group
+                // owns half of them and a warp re-uses its 4 KB only after its own earlier TMA store has read it.
+                constexpr int SLOTS_H = (Cfg::BUF / CT_A_BYTES) / 2;
                 const int cj = (mc - half * PER) / 32;
                 if (cj >= SLOTS_H) { if (lane == 0) tc::tma_store_wait_read(); __syncwarp(); }
                 unsigned char* stg = smem + (half * SLOTS_H + cj % SLOTS_H) * CT_A_BYTES + q * 4096;        // 32 rows x 128 B
@@ -303,7 +271,7 @@ __device__ __forceinline__ void conv2d_tf32_body(const CUtensorMap& tmA, const C
                 tc::fence_proxy_async();                 // generic-proxy smem writes -> visible to the TMA (async proxy)
                 __syncwarp();
                 if (lane == 0 && n0 + c0 < p.cout) {
-                    const int row0 = ty0 + m * CT_TH + q * 2;
+                    const int row0 = ty0 + q * (32 / TW);      // the warp's 32 pixels = 32/TW patch rows
                     if (p.tma_store == 2) {
                         // ConvTranspose2d with kernel == stride: output pixel (y*os + oy0, x*os + ox0) through the 5-D view
                         // [C][dx][x][dy][b*Ho + y] of the NHWC tensor.  The merged (batch, y) axis cannot clip rows past Ho: skip them
@@ -332,518 +300,25 @@ __device__ __forceinline__ void conv2d_tf32_body(const CUtensorMap& tmA, const C
                 }
             }
         }
+        if (p.tma_store && lane == 0) tc::tma_store_wait_read();      // the stores must have read the staging buffers
     }
-    if (p.tma_store && warp >= 2 && lane == 0) tc::tma_store_wait_read();      // the stores must have read the staging buffers
-    if (tr && threadIdx.x == 64) g_ct_trace[5] = clock64();
-    tc::tcgen05_fence_before();
-    __syncthreads();
     if (tr && threadIdx.x == 0) g_ct_trace[4] = clock64();
-    if (TWO) cluster_sync_all();                            // the peer's shared memory / TMEM stay alive until the pair is done
-    if (warp == 1) { if (TWO) tmem_dealloc2<Cfg::TMEM_COLS>(tmem_base); else tc::tmem_dealloc<Cfg::TMEM_COLS>(tmem_base); }
 }
 
-template <int BN, int MT, int OCC>
-__global__ void __launch_bounds__(CT_THREADS, OCC)
-k_conv2d_tf32(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
-              Conv2dParams p, int tiles_x, int tiles_y) {
-    conv2d_tf32_body<BN, MT, OCC, 0>(tmA, tmB, tmO, p, tiles_x, tiles_y, 0x7fffffff);
-}
-
-template <int BN, int OCC>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(CT_THREADS, OCC)
-k_conv2d_tf32_pair(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
-                   Conv2dParams p, int tiles_x, int tiles_y, int tiles_total) {
-    conv2d_tf32_body<BN, 1, OCC, 1>(tmA, tmB, tmO, p, tiles_x, tiles_y, tiles_total);
-}
-
-template <int BN, int OCC>
-static int launch_tf32_pair(const Conv2dParams& p, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, cudaStream_t st) {
-    using Cfg = CtKCfg<BN, 1, OCC, 1>;
-    static bool configured = false;
-    if (!configured) {
-        DZ_CUDA(cudaFuncSetAttribute(k_conv2d_tf32_pair<BN, OCC>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM));
-        configured = true;
-    }
-    const int tiles_x = dz_cdiv(p.Wo, CT_TW), tiles_y = dz_cdiv(p.Ho, CT_TH);
-    const int tiles = tiles_x * tiles_y * p.B;
-    dim3 grid((tiles + 1) / 2 * 2, dz_cdiv(p.cout, BN));
-    static_assert(Cfg::STAGES * Cfg::STAGE_BYTES / CT_A_BYTES >= 2, "epilogue staging needs at least one slot per warp group");
-    k_conv2d_tf32_pair<BN, OCC><<<grid, CT_THREADS, Cfg::SMEM, st>>>(tmA, tmB, tmO, p, tiles_x, tiles_y, tiles);
-    DZ_LAUNCH_CHECK();
-    return DZ_OK;
-}
-
-template <int BN, int MT, int OCC = 1>
+template <int BN, bool HALO>
 static int launch_tf32(const Conv2dParams& p, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, cudaStream_t st) {
-    using Cfg = CtKCfg<BN, MT, OCC, 0>;
+    using Cfg = CtCfg<BN, HALO>;
     static bool configured = false;
     if (!configured) {
-        DZ_CUDA(cudaFuncSetAttribute(k_conv2d_tf32<BN, MT, OCC>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM));
+        DZ_CUDA(cudaFuncSetAttribute(k_conv2d_tf32<BN, HALO>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM));
         configured = true;
     }
-    int tiles_x = dz_cdiv(p.Wo, CT_TW), tiles_y = dz_cdiv(p.Ho, CT_TH * MT);
+    int tiles_x = dz_cdiv(p.Wo, Cfg::TW), tiles_y = dz_cdiv(p.Ho, Cfg::TH);
     dim3 grid(tiles_x * tiles_y * p.B, dz_cdiv(p.cout, BN));
-    static_assert((MT * BN / 32) * CT_A_BYTES <= Cfg::STAGES * Cfg::STAGE_BYTES || MT * BN < 32, "epilogue staging must fit in the pipeline buffers");
-    // (programmatic dependent launch was tried for this kernel and the sparse conv: no measurable gain in the graph replay)
-    k_conv2d_tf32<BN, MT, OCC><<<grid, CT_THREADS, Cfg::SMEM, st>>>(tmA, tmB, tmO, p, tiles_x, tiles_y);
+    static_assert((BN / 32) * CT_A_BYTES <= Cfg::BUF, "epilogue staging must fit in the pipeline buffers");
+    k_conv2d_tf32<BN, HALO><<<grid, CT_THREADS, Cfg::SMEM, st>>>(tmA, tmB, tmO, p, tiles_x, tiles_y);
     DZ_LAUNCH_CHECK();
     return DZ_OK;
-}
-
-// =====================================================================================================================
-// HALO kernel: 3x3 stride-1 convolutions (16 of the 22 dense convs of the BEV backbone + head).
-//
-// The generic kernel above re-reads its 128-pixel activation patch from L2 once per filter tap: 9 x 16 KB per 32-channel slice, and with
-// three 32 KB stages per CTA the SM cannot keep enough bytes in flight to cover the L2 latency at the tensor pipe's rate (50-57 % tensor
-// pipe in profiles/r02_ncu_full_conv2d_batch8.json, nothing else saturated).  Here the CTA loads the (16+2) x (8+2) pixel HALO of its
-// 16 x 8 output patch ONCE per 32-channel slice (23 KB) and the nine taps are nine A descriptors into that one tile: the UMMA
-// shared-memory descriptor may start at any 128-byte pixel row, its 8-row core groups are the 8-pixel rows of the patch, and the stride
-// between groups (SBO) is the halo's row pitch, 10 pixels = 1280 B -- the 128-byte swizzle is a function of the absolute shared-memory
-// address, so a window shifted by (r, s) reads exactly the bytes the TMA unit wrote for pixel (y + r, x + s) (tools/ubench_halo.cu checks
-// all nine taps).  Per slice the SM now pulls 23 KB + 9 weight tiles instead of 9 x (16 KB + weight tile).
-// TWO = 1: CTA pair as above (each CTA its own halo, half of the weight rows, tcgen05.mma.cta_group::2).
-// =====================================================================================================================
-static constexpr int HL_TH = 16, HL_TW = 8, HL_PITCH = HL_TW + 2, HL_ROWS = HL_TH + 2;
-static constexpr int HL_A_BYTES = HL_ROWS * HL_PITCH * 128;          // 23040 B delivered by the TMA unit
-static constexpr int HL_A_SLOT = (HL_A_BYTES + 1023) / 1024 * 1024;  // 23552: slots stay 1024-byte aligned (swizzle phase)
-static constexpr int HL_A_STAGES = 2;
-
-template <int BN, int TWO>
-struct HlCfg {
-    static constexpr int B_ROWS = TWO ? BN / 2 : BN;
-    static constexpr int B_BYTES = B_ROWS * 128;
-    static constexpr int BUDGET = 104 * 1024;                         // two CTAs per SM
-    static constexpr int B_STAGES = (BUDGET - HL_A_STAGES * HL_A_SLOT) / B_BYTES > 9 ? 9 : (BUDGET - HL_A_STAGES * HL_A_SLOT) / B_BYTES;
-    static constexpr int BUF = HL_A_STAGES * HL_A_SLOT + B_STAGES * B_BYTES;
-    static constexpr int SMEM = BUF + 1024 + 256;
-    static constexpr int TMEM_COLS = BN < 32 ? 32 : BN;
-};
-
-template <int BN, int TWO>
-__device__ __forceinline__ void conv2d_halo_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, const Conv2dParams& p,
-                                                 int tiles_x, int tiles_y, int tiles_total) {
-    using Cfg = HlCfg<BN, TWO>;
-    extern __shared__ unsigned char smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    unsigned char* smB = smem + HL_A_STAGES * HL_A_SLOT;
-    uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + Cfg::BUF);
-    uint64_t* a_empty = a_full + HL_A_STAGES;
-    uint64_t* b_full = a_empty + HL_A_STAGES;
-    uint64_t* b_empty = b_full + Cfg::B_STAGES;
-    uint64_t* tmem_full = b_empty + Cfg::B_STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    int mt = min((int)blockIdx.x, tiles_total - 1);         // pair kernel: an odd tile count is padded with a duplicate of the last tile
-    const uint32_t rank = TWO ? cluster_ctarank() : 0u;
-    const int tx0 = (mt % tiles_x) * HL_TW; mt /= tiles_x;
-    const int ty0 = (mt % tiles_y) * HL_TH;
-    const int b = mt / tiles_y;
-    const int n0 = blockIdx.y * BN;
-    const int cchunks = p.cin / CT_BK;
-
-    if (threadIdx.x == 0) {
-        tc::prefetch_tmap(&tmA);
-        tc::prefetch_tmap(&tmB);
-        tc::prefetch_tmap(&tmO);
-        for (int s = 0; s < HL_A_STAGES; ++s) { tc::mbar_init(a_full + s, 1); tc::mbar_init(a_empty + s, 1); }
-        for (int s = 0; s < Cfg::B_STAGES; ++s) { tc::mbar_init(b_full + s, 1); tc::mbar_init(b_empty + s, 1); }
-        tc::mbar_init(tmem_full, 1);
-        tc::fence_barrier_init();
-    }
-    if (TWO) { __syncthreads(); cluster_sync_all(); }
-    if (warp == 1) { if (TWO) tmem_alloc2<Cfg::TMEM_COLS>(tmem_slot); else tc::tmem_alloc<Cfg::TMEM_COLS>(tmem_slot); }
-    tc::tcgen05_fence_before();
-    __syncthreads();
-    tc::tcgen05_fence_after();
-    if (TWO) cluster_sync_all();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            int bit = 0;
-            for (int cc = 0; cc < cchunks; ++cc) {
-                const int a = cc % HL_A_STAGES;
-                tc::mbar_wait(a_empty + a, ((cc / HL_A_STAGES) & 1) ^ 1);
-                if (TWO) {
-                    if (rank == 0) tc::mbar_arrive_expect_tx(a_full + a, 2 * HL_A_BYTES);
-                    tma2_load_4d(smem + a * HL_A_SLOT, &tmA, a_full + a, cc * CT_BK, tx0 - p.pad, ty0 - p.pad, b);
-                } else {
-                    tc::mbar_arrive_expect_tx(a_full + a, HL_A_BYTES);
-                    tc::tma_load_4d(smem + a * HL_A_SLOT, &tmA, a_full + a, cc * CT_BK, tx0 - p.pad, ty0 - p.pad, b);
-                }
-                for (int tap = 0; tap < 9; ++tap, ++bit) {
-                    const int s = bit % Cfg::B_STAGES;
-                    tc::mbar_wait(b_empty + s, ((bit / Cfg::B_STAGES) & 1) ^ 1);
-                    if (TWO) {
-                        if (rank == 0) tc::mbar_arrive_expect_tx(b_full + s, 2 * Cfg::B_BYTES);
-                        tma2_load_2d(smB + s * Cfg::B_BYTES, &tmB, b_full + s, tap * p.cin + cc * CT_BK, n0 + (int)rank * Cfg::B_ROWS);
-                    } else {
-                        tc::mbar_arrive_expect_tx(b_full + s, Cfg::B_BYTES);
-                        tc::tma_load_2d(smB + s * Cfg::B_BYTES, &tmB, b_full + s, tap * p.cin + cc * CT_BK, n0);
-                    }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0 && (!TWO || rank == 0)) {                 // pair: the leader issues every MMA; its commits reach both CTAs
-            constexpr uint32_t idesc = tc::instr_desc(2, TWO ? 256 : 128, BN);
-            int bit = 0;
-            for (int cc = 0; cc < cchunks; ++cc) {
-                const int a = cc % HL_A_STAGES;
-                tc::mbar_wait(a_full + a, (cc / HL_A_STAGES) & 1);
-                const uint32_t ha = tc::smem_u32(smem + a * HL_A_SLOT);
-                for (int tap = 0; tap < 9; ++tap, ++bit) {
-                    const int s = bit % Cfg::B_STAGES;
-                    tc::mbar_wait(b_full + s, (bit / Cfg::B_STAGES) & 1);
-                    tc::tcgen05_fence_after();
-                    const int r = tap / 3, sx = tap - r * 3;
-                    // window (r, sx) of the halo: start at pixel (r, sx), 8-pixel rows HL_PITCH pixels apart
-                    const uint32_t a0 = ha + (uint32_t)((r * HL_PITCH + sx) * 128);
-                    const uint64_t adesc = (uint64_t)((a0 >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)((HL_PITCH * 128) >> 4) << 32) |
-                                           ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-                    const uint64_t bdesc = tc::smem_desc_sw128(tc::smem_u32(smB + s * Cfg::B_BYTES));
-#pragma unroll
-                    for (int k = 0; k < CT_BK / 8; ++k) {
-                        if (TWO) mma2_tf32(tmem_base, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, (bit | k) ? 1u : 0u);
-                        else tc::mma_tf32(tmem_base, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, (bit | k) ? 1u : 0u);
-                    }
-                    if (TWO) mma2_commit_multicast(b_empty + s, 0b11); else tc::mma_commit(b_empty + s);
-                }
-                if (TWO) mma2_commit_multicast(a_empty + a, 0b11); else tc::mma_commit(a_empty + a);
-            }
-            if (TWO) mma2_commit_multicast(tmem_full, 0b11); else tc::mma_commit(tmem_full);
-        }
-    } else {
-        // epilogue: folded BN / bias / ReLU, staged through the (idle) pipeline buffers, one TMA store of 4 patch rows x 8 pixels x 32
-        // channels per warp and 32-column chunk
-        const int q = warp & 3;
-        const int half = (warp - 2) >> 2;
-        tc::mbar_wait(tmem_full, 0);
-        tc::tcgen05_fence_after();
-        constexpr int PER = BN >= 64 ? BN / 2 : BN;             // BN = 32: one 32-column chunk, the second warp group has nothing to do
-        constexpr int SLOTS_H = (Cfg::BUF / CT_A_BYTES) / 2;
-        static_assert(SLOTS_H >= 1, "epilogue staging needs one 16 KB slot per warp group");
-        if (half == 1 && BN < 64) { /* nothing */ } else
-#pragma unroll 1
-        for (int mc = half * PER; mc < half * PER + PER; mc += 32) {
-            float v[32];
-            tc::tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)mc, v);
-            const int cj = (mc - half * PER) / 32;
-            if (cj >= SLOTS_H) { if (lane == 0) tc::tma_store_wait_read(); __syncwarp(); }
-            unsigned char* stg = smem + (half * SLOTS_H + cj % SLOTS_H) * CT_A_BYTES + q * 4096;        // 32 rows x 128 B
-            const uint32_t stg_u = tc::smem_u32(stg) + (uint32_t)((lane >> 3) * 1024 + (lane & 7) * 128);
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-                const int n = n0 + mc + j;
-                float4 o = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-                if (n < p.cout) {
-                    if (p.scale) { float4 sc = __ldg(reinterpret_cast<const float4*>(p.scale + n)); o.x *= sc.x; o.y *= sc.y; o.z *= sc.z; o.w *= sc.w; }
-                    if (p.shift) { float4 sh = __ldg(reinterpret_cast<const float4*>(p.shift + n)); o.x += sh.x; o.y += sh.y; o.z += sh.z; o.w += sh.w; }
-                }
-                if (p.relu) {
-                    o.x = tc::rna_tf32(fmaxf(o.x, 0.f)); o.y = tc::rna_tf32(fmaxf(o.y, 0.f));
-                    o.z = tc::rna_tf32(fmaxf(o.z, 0.f)); o.w = tc::rna_tf32(fmaxf(o.w, 0.f));
-                }
-                asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(stg_u + (uint32_t)((((j >> 2) ^ (lane & 7))) << 4)),
-                             "f"(o.x), "f"(o.y), "f"(o.z), "f"(o.w) : "memory");
-            }
-            tc::fence_proxy_async();
-            __syncwarp();
-            if (lane == 0 && n0 + mc < p.cout) {
-                tc::tma_store_4d(&tmO, stg, p.out_coff + n0 + mc, tx0, ty0 + q * 4, b);      // rows q*4 .. q*4+3 of the 16 x 8 patch
-                tc::tma_store_commit();
-            }
-        }
-    }
-    if (warp >= 2 && lane == 0) tc::tma_store_wait_read();
-    tc::tcgen05_fence_before();
-    __syncthreads();
-    if (TWO) cluster_sync_all();
-    if (warp == 1) { if (TWO) tmem_dealloc2<Cfg::TMEM_COLS>(tmem_base); else tc::tmem_dealloc<Cfg::TMEM_COLS>(tmem_base); }
-}
-
-template <int BN>
-__global__ void __launch_bounds__(CT_THREADS, 2)
-k_conv2d_tf32_halo(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
-                   Conv2dParams p, int tiles_x, int tiles_y) {
-    conv2d_halo_body<BN, 0>(tmA, tmB, tmO, p, tiles_x, tiles_y, 0x7fffffff);
-}
-template <int BN>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(CT_THREADS, 2)
-k_conv2d_tf32_halo_pair(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
-                        Conv2dParams p, int tiles_x, int tiles_y, int tiles_total) {
-    conv2d_halo_body<BN, 1>(tmA, tmB, tmO, p, tiles_x, tiles_y, tiles_total);
-}
-
-// ---- persistent halo kernel: ONE CTA per SM walks the (patch, Cout block) list.  The non-persistent kernel above spends ~40 % of a CTA's
-// life outside the main loop on the short layers (128 -> 128: 144 MMAs = 9.2 K clk per patch; fused head stage 1, 64 -> 384: 72 MMAs):
-// barrier set-up, TMEM allocation, the first halo's L2 latency, the epilogue.  Here the TMEM accumulator is double-buffered (2 x BN columns):
-// the epilogue warps drain patch i while the MMA thread is already on patch i+1, the TMA producer runs ahead across patch boundaries, and
-// set-up is paid once per SM.  Epilogue staging has its own 4 KB per warp (the pipeline buffers never go idle).
-template <int BN>
-struct HpCfg {
-    static constexpr int B_BYTES = BN * 128;
-    static constexpr int STG_BYTES = 8 * 4096;                                   // 8 epilogue warps x (32 rows x 128 B)
-    static constexpr int BUDGET = 200 * 1024;
-    static constexpr int B_STAGES = (BUDGET - HL_A_STAGES * HL_A_SLOT - STG_BYTES) / B_BYTES > 9 ? 9 : (BUDGET - HL_A_STAGES * HL_A_SLOT - STG_BYTES) / B_BYTES;
-    static constexpr int BUF = HL_A_STAGES * HL_A_SLOT + B_STAGES * B_BYTES + STG_BYTES;
-    static constexpr int SMEM = BUF + 1024 + 256;
-    static constexpr int TMEM_COLS = 2 * BN < 32 ? 32 : 2 * BN;
-    static constexpr int EPI_WARPS = BN >= 64 ? 8 : 4;                           // warps that read the accumulator (BN = 32: one 32-column chunk)
-};
-
-template <int BN>
-__global__ void __launch_bounds__(CT_THREADS, 1)
-k_conv2d_tf32_halo_persist(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
-                           Conv2dParams p, int tiles_x, int tiles_y, int nblocks, int items) {
-    using Cfg = HpCfg<BN>;
-    extern __shared__ unsigned char smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    unsigned char* smB = smem + HL_A_STAGES * HL_A_SLOT;
-    unsigned char* smS = smB + Cfg::B_STAGES * Cfg::B_BYTES;
-    uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + Cfg::BUF);
-    uint64_t* a_empty = a_full + HL_A_STAGES;
-    uint64_t* b_full = a_empty + HL_A_STAGES;
-    uint64_t* b_empty = b_full + Cfg::B_STAGES;
-    uint64_t* acc_full = b_empty + Cfg::B_STAGES;      // [2]
-    uint64_t* acc_empty = acc_full + 2;                // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int cchunks = p.cin / CT_BK;
-    const int G = gridDim.x;
-
-    if (threadIdx.x == 0) {
-        tc::prefetch_tmap(&tmA);
-        tc::prefetch_tmap(&tmB);
-        tc::prefetch_tmap(&tmO);
-        for (int s = 0; s < HL_A_STAGES; ++s) { tc::mbar_init(a_full + s, 1); tc::mbar_init(a_empty + s, 1); }
-        for (int s = 0; s < Cfg::B_STAGES; ++s) { tc::mbar_init(b_full + s, 1); tc::mbar_init(b_empty + s, 1); }
-        for (int s = 0; s < 2; ++s) { tc::mbar_init(acc_full + s, 1); tc::mbar_init(acc_empty + s, Cfg::EPI_WARPS); }
-        tc::fence_barrier_init();
-    }
-    if (warp == 1) tc::tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-    tc::tcgen05_fence_before();
-    __syncthreads();
-    tc::tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    // work item w -> (patch, Cout block): the Cout blocks of one patch are consecutive items, i.e. run at the same time on neighbouring
-    // SMs and share the patch's halo through L2
-    auto decode = [&](int w, int& tx0, int& ty0, int& b, int& n0) {
-        const int nb = w % nblocks;
-        int mt = w / nblocks;
-        tx0 = (mt % tiles_x) * HL_TW; mt /= tiles_x;
-        ty0 = (mt % tiles_y) * HL_TH;
-        b = mt / tiles_y;
-        n0 = nb * BN;
-    };
-
-    if (warp == 0) {
-        if (lane == 0) {
-            int ait = 0, bit = 0;
-            for (int w = blockIdx.x; w < items; w += G) {
-                int tx0, ty0, b, n0;
-                decode(w, tx0, ty0, b, n0);
-                for (int cc = 0; cc < cchunks; ++cc, ++ait) {
-                    const int a = ait % HL_A_STAGES;
-                    tc::mbar_wait(a_empty + a, ((ait / HL_A_STAGES) & 1) ^ 1);
-                    tc::mbar_arrive_expect_tx(a_full + a, HL_A_BYTES);
-                    tc::tma_load_4d(smem + a * HL_A_SLOT, &tmA, a_full + a, cc * CT_BK, tx0 - p.pad, ty0 - p.pad, b);
-                    for (int tap = 0; tap < 9; ++tap, ++bit) {
-                        const int s = bit % Cfg::B_STAGES;
-                        tc::mbar_wait(b_empty + s, ((bit / Cfg::B_STAGES) & 1) ^ 1);
-                        tc::mbar_arrive_expect_tx(b_full + s, Cfg::B_BYTES);
-                        tc::tma_load_2d(smB + s * Cfg::B_BYTES, &tmB, b_full + s, tap * p.cin + cc * CT_BK, n0);
-                    }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = tc::instr_desc(2, 128, BN);
-            int ait = 0, bit = 0, i = 0;
-            for (int w = blockIdx.x; w < items; w += G, ++i) {
-                const int buf = i & 1;
-                tc::mbar_wait(acc_empty + buf, ((i >> 1) & 1) ^ 1);          // the epilogue has drained this accumulator (item i-2)
-                tc::tcgen05_fence_after();
-                const uint32_t acc = tmem_base + (uint32_t)(buf * BN);
-                for (int cc = 0; cc < cchunks; ++cc, ++ait) {
-                    const int a = ait % HL_A_STAGES;
-                    tc::mbar_wait(a_full + a, (ait / HL_A_STAGES) & 1);
-                    const uint32_t ha = tc::smem_u32(smem + a * HL_A_SLOT);
-                    for (int tap = 0; tap < 9; ++tap, ++bit) {
-                        const int s = bit % Cfg::B_STAGES;
-                        tc::mbar_wait(b_full + s, (bit / Cfg::B_STAGES) & 1);
-                        tc::tcgen05_fence_after();
-                        const int r = tap / 3, sx = tap - r * 3;
-                        const uint32_t a0 = ha + (uint32_t)((r * HL_PITCH + sx) * 128);
-                        const uint64_t adesc = (uint64_t)((a0 >> 4) & 0x3FFF) | ((uint64_t)1 << 16) | ((uint64_t)((HL_PITCH * 128) >> 4) << 32) |
-                                               ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-                        const uint64_t bdesc = tc::smem_desc_sw128(tc::smem_u32(smB + s * Cfg::B_BYTES));
-#pragma unroll
-                        for (int k = 0; k < CT_BK / 8; ++k)
-                            tc::mma_tf32(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, (cc | tap | k) ? 1u : 0u);
-                        tc::mma_commit(b_empty + s);
-                    }
-                    tc::mma_commit(a_empty + a);
-                }
-                tc::mma_commit(acc_full + buf);
-            }
-        }
-    } else {
-        const int q = warp & 3;
-        const int half = (warp - 2) >> 2;
-        constexpr int PER = BN >= 64 ? BN / 2 : BN;
-        if (!(half == 1 && BN < 64)) {
-            unsigned char* stg = smS + (warp - 2) * 4096;                          // this warp's own 32 rows x 128 B
-            const uint32_t stg_u = tc::smem_u32(stg) + (uint32_t)((lane >> 3) * 1024 + (lane & 7) * 128);
-            int i = 0;
-            for (int w = blockIdx.x; w < items; w += G, ++i) {
-                int tx0, ty0, b, n0;
-                decode(w, tx0, ty0, b, n0);
-                const int buf = i & 1;
-                tc::mbar_wait(acc_full + buf, (i >> 1) & 1);
-                tc::tcgen05_fence_after();
-#pragma unroll 1
-                for (int mc = half * PER; mc < half * PER + PER; mc += 32) {
-                    float v[32];
-                    tc::tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * BN + mc), v);
-                    if (mc + 32 >= half * PER + PER) {                             // last read of this accumulator by this warp: hand it back
-                        tc::tcgen05_fence_before();
-                        __syncwarp();
-                        if (lane == 0) tc::mbar_arrive(acc_empty + buf);
-                    }
-                    if (lane == 0) tc::tma_store_wait_read();                      // the previous store has read the staging rows
-                    __syncwarp();
-#pragma unroll
-                    for (int j = 0; j < 32; j += 4) {
-                        const int n = n0 + mc + j;
-                        float4 o = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-                        if (n < p.cout) {
-                            if (p.scale) { float4 sc = __ldg(reinterpret_cast<const float4*>(p.scale + n)); o.x *= sc.x; o.y *= sc.y; o.z *= sc.z; o.w *= sc.w; }
-                            if (p.shift) { float4 sh = __ldg(reinterpret_cast<const float4*>(p.shift + n)); o.x += sh.x; o.y += sh.y; o.z += sh.z; o.w += sh.w; }
-                        }
-                        if (p.relu) {
-                            o.x = tc::rna_tf32(fmaxf(o.x, 0.f)); o.y = tc::rna_tf32(fmaxf(o.y, 0.f));
-                            o.z = tc::rna_tf32(fmaxf(o.z, 0.f)); o.w = tc::rna_tf32(fmaxf(o.w, 0.f));
-                        }
-                        asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(stg_u + (uint32_t)((((j >> 2) ^ (lane & 7))) << 4)),
-                                     "f"(o.x), "f"(o.y), "f"(o.z), "f"(o.w) : "memory");
-                    }
-                    tc::fence_proxy_async();
-                    __syncwarp();
-                    if (lane == 0 && n0 + mc < p.cout) {
-                        tc::tma_store_4d(&tmO, stg, p.out_coff + n0 + mc, tx0, ty0 + q * 4, b);
-                        tc::tma_store_commit();
-                    }
-                }
-            }
-            if (lane == 0) tc::tma_store_wait_read();
-        }
-    }
-    tc::tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) tc::tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-}
-
-template <int BN>
-static int launch_halo_persist(const Conv2dParams& p, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, int tiles_x, int tiles_y,
-                               cudaStream_t st) {
-    static bool configured = false;
-    if (!configured) {
-        DZ_CUDA(cudaFuncSetAttribute(k_conv2d_tf32_halo_persist<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, HpCfg<BN>::SMEM));
-        configured = true;
-    }
-    const int nblocks = dz_cdiv(p.cout, BN), items = tiles_x * tiles_y * p.B * nblocks;
-    const int grid = items < DZ_NUM_SMS ? items : DZ_NUM_SMS;
-    k_conv2d_tf32_halo_persist<BN><<<grid, CT_THREADS, HpCfg<BN>::SMEM, st>>>(tmA, tmB, tmO, p, tiles_x, tiles_y, nblocks, items);
-    DZ_LAUNCH_CHECK();
-    return DZ_OK;
-}
-
-template <int BN>
-static int launch_halo_single(const Conv2dParams& p, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, int tiles_x, int tiles_y,
-                              cudaStream_t st) {
-    static bool configured = false;
-    if (!configured) {
-        DZ_CUDA(cudaFuncSetAttribute(k_conv2d_tf32_halo<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, HlCfg<BN, 0>::SMEM));
-        configured = true;
-    }
-    dim3 grid(tiles_x * tiles_y * p.B, dz_cdiv(p.cout, BN));
-    k_conv2d_tf32_halo<BN><<<grid, CT_THREADS, HlCfg<BN, 0>::SMEM, st>>>(tmA, tmB, tmO, p, tiles_x, tiles_y);
-    DZ_LAUNCH_CHECK();
-    return DZ_OK;
-}
-template <int BN>
-static int launch_halo_pair(const Conv2dParams& p, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, int tiles_x, int tiles_y,
-                            cudaStream_t st) {
-    static bool configured = false;
-    if (!configured) {
-        DZ_CUDA(cudaFuncSetAttribute(k_conv2d_tf32_halo_pair<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, HlCfg<BN, 1>::SMEM));
-        configured = true;
-    }
-    const int tiles = tiles_x * tiles_y * p.B;
-    dim3 grid((tiles + 1) / 2 * 2, dz_cdiv(p.cout, BN));
-    k_conv2d_tf32_halo_pair<BN><<<grid, CT_THREADS, HlCfg<BN, 1>::SMEM, st>>>(tmA, tmB, tmO, p, tiles_x, tiles_y, tiles);
-    DZ_LAUNCH_CHECK();
-    return DZ_OK;
-}
-
-// mode (DZ_CONV2D_HALO): 1 = automatic -- CTA pair with a 256-wide weight tile when Cout % 256 == 0 (256 -> 256 @94^2, 8 frames: 114 -> 103 us),
-// otherwise one CTA per patch (128 -> 128 @188^2: 177 -> 138 us; the BN = 128 pair is slower, 152 us); 2 = pair whenever Cout % 128 == 0;
-// 3 = never pair
-static int launch_halo(const Conv2dParams& p, int mode, cudaStream_t st) {
-    tc::EncodeTiledFn enc = tc::get_encode_tiled();
-    CUtensorMap tmA, tmB, tmO;
-    const bool pair = mode != 3 && ((p.cout % 256 == 0) || (mode == 2 && (p.cout % 128 == 0 || p.cout == 64)));
-    const int bn = pair ? (p.cout % 256 == 0 ? 256 : (p.cout == 64 ? 64 : 128)) : (p.cout > 64 ? 128 : (p.cout > 32 ? 64 : 32));
-    {
-        cuuint64_t dims[4] = {(cuuint64_t)p.in_cstride, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.B};
-        cuuint64_t strides[3] = {(cuuint64_t)p.in_cstride * 4, (cuuint64_t)p.W * p.in_cstride * 4, (cuuint64_t)p.H * p.W * p.in_cstride * 4};
-        cuuint32_t box[4] = {(cuuint32_t)CT_BK, (cuuint32_t)HL_PITCH, (cuuint32_t)HL_ROWS, 1};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        CUresult r = enc(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)p.in, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { dz_set_error("cuTensorMapEncodeTiled(halo A) failed: %d", (int)r); return DZ_ERR_CUDA; }
-    }
-    {
-        cuuint64_t ktot = (cuuint64_t)9 * p.cin;
-        cuuint64_t dims[2] = {ktot, (cuuint64_t)p.cout};
-        cuuint64_t strides[1] = {ktot * 4};
-        cuuint32_t box[2] = {(cuuint32_t)CT_BK, (cuuint32_t)(pair ? bn / 2 : bn)};
-        cuuint32_t estr[2] = {1, 1};
-        CUresult r = enc(&tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)p.w, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { dz_set_error("cuTensorMapEncodeTiled(halo B) failed: %d", (int)r); return DZ_ERR_CUDA; }
-    }
-    {
-        cuuint64_t dims[4] = {(cuuint64_t)(p.out_coff + p.cout), (cuuint64_t)p.OW, (cuuint64_t)p.OH, (cuuint64_t)p.B};
-        cuuint64_t strides[3] = {(cuuint64_t)p.out_cstride * 4, (cuuint64_t)p.OW * p.out_cstride * 4, (cuuint64_t)p.OH * p.OW * p.out_cstride * 4};
-        cuuint32_t box[4] = {32, (cuuint32_t)HL_TW, 4, 1};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        CUresult r = enc(&tmO, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)p.out, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { dz_set_error("cuTensorMapEncodeTiled(halo out) failed: %d", (int)r); return DZ_ERR_CUDA; }
-    }
-    const int tiles_x = dz_cdiv(p.Wo, HL_TW), tiles_y = dz_cdiv(p.Ho, HL_TH);
-    if (pair) return bn == 256 ? launch_halo_pair<256>(p, tmA, tmB, tmO, tiles_x, tiles_y, st)
-                     : (bn == 64 ? launch_halo_pair<64>(p, tmA, tmB, tmO, tiles_x, tiles_y, st) : launch_halo_pair<128>(p, tmA, tmB, tmO, tiles_x, tiles_y, st));
-    // DZ_CONV2D_PERSIST: 1 = persistent kernel (double-buffered TMEM accumulator) for the single-CTA shapes, 0 = one CTA per patch
-    static const int persist = getenv("DZ_CONV2D_PERSIST") ? atoi(getenv("DZ_CONV2D_PERSIST")) : 0;
-    if (persist) {
-        switch (bn) {
-            case 128: return launch_halo_persist<128>(p, tmA, tmB, tmO, tiles_x, tiles_y, st);
-            case 64: return launch_halo_persist<64>(p, tmA, tmB, tmO, tiles_x, tiles_y, st);
-            default: return launch_halo_persist<32>(p, tmA, tmB, tmO, tiles_x, tiles_y, st);
-        }
-    }
-    switch (bn) {
-        case 128: return launch_halo_single<128>(p, tmA, tmB, tmO, tiles_x, tiles_y, st);
-        case 64: return launch_halo_single<64>(p, tmA, tmB, tmO, tiles_x, tiles_y, st);
-        default: return launch_halo_single<32>(p, tmA, tmB, tmO, tiles_x, tiles_y, st);
-    }
 }
 
 // p.w must be in (cout, KH, KW, cin) layout for this path
@@ -856,45 +331,44 @@ int dz_conv2d_fwd_tc(const Conv2dParams& p_in, int mode, cudaStream_t st) {
     }
     tc::EncodeTiledFn enc = tc::get_encode_tiled();
     if (!enc) { dz_set_error("cuTensorMapEncodeTiled unavailable"); return DZ_ERR_CUDA; }
+    static const int no_tma_store = getenv("DZ_CONV2D_NO_TMA_STORE") ? 1 : 0;
+    p.tma_store = (!p.gmax && !no_tma_store && p.os == 1 && p.oy0 == 0 && p.ox0 == 0 && p.OH == p.Ho && p.OW == p.Wo &&
+                   (reinterpret_cast<uintptr_t>(p.out) & 15) == 0) ? 1 : 0;
+    // 3x3 stride-1 convolutions with at least two patches per SM and 128-channel slice: the halo variant (DZ_CONV2D_HALO=0 switches it off)
+    static const int use_halo = getenv("DZ_CONV2D_HALO") ? atoi(getenv("DZ_CONV2D_HALO")) : 1;
+    const long long tiles_m = (long long)dz_cdiv(p.Wo, CT_TW) * dz_cdiv(p.Ho, CT_TH) * p.B;
+    const bool halo = use_halo && p.KH == 3 && p.KW == 3 && p.stride == 1 && p.tma_store == 1 && !p.gshift && !(p.dbg & 3) &&
+                      tiles_m * dz_cdiv(p.cout, 128) >= 2 * DZ_NUM_SMS;
+    const int TW = halo ? HL_TW : CT_TW;
     CUtensorMap tmA, tmB;
     {
         cuuint64_t dims[4] = {(cuuint64_t)p.in_cstride, (cuuint64_t)p.W, (cuuint64_t)p.H, (cuuint64_t)p.B};
         cuuint64_t strides[3] = {(cuuint64_t)p.in_cstride * 4, (cuuint64_t)p.W * p.in_cstride * 4, (cuuint64_t)p.H * p.W * p.in_cstride * 4};
-        // with a traversal stride s the box spans (n-1)*s+1 input elements and delivers n of them
+        // with a traversal stride s the box spans (n-1)*s+1 input elements and delivers n of them; the halo box is the patch + 1 pixel
+        // on each side
         cuuint32_t box[4] = {(cuuint32_t)CT_BK, (cuuint32_t)((CT_TW - 1) * p.stride + 1), (cuuint32_t)((CT_TH - 1) * p.stride + 1), 1};
+        if (halo) { box[1] = HL_PITCH; box[2] = HL_ROWS; }
         cuuint32_t estr[4] = {1, (cuuint32_t)p.stride, (cuuint32_t)p.stride, 1};
         CUresult r = enc(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)p.in, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { dz_set_error("cuTensorMapEncodeTiled(A) failed: %d", (int)r); return DZ_ERR_CUDA; }
     }
-    int bn = p.cout > 128 ? 128 : (p.cout > 64 ? 128 : (p.cout > 32 ? 64 : 32));
-    // CTA-pair kernel (tcgen05 cta_group::2): real convolutions with Cout a multiple of 128 and at least one tile pair per SM pair
-    static const int use_pair = getenv("DZ_CONV2D_2SM") ? atoi(getenv("DZ_CONV2D_2SM")) : 1;
-    const long long tiles_m = (long long)dz_cdiv(p.Wo, CT_TW) * dz_cdiv(p.Ho, CT_TH) * p.B;
-    // Measured (profiles/r02_spconv_notes.md): the pair pays off where it makes a 256-wide tile possible (256 -> 256 @94^2: 158 -> 120 us,
-    // 1x1 128 -> 256: 110 -> 80 us); with BN = 128 it is no faster than two co-resident single CTAs (128 -> 128 @188^2: 177 vs 182 us),
-    // so Cout % 256 != 0 keeps the single-CTA kernel.  DZ_CONV2D_2SM=0 switches the pair kernel off, =128 forces it for Cout % 128 == 0.
-    const bool pair = use_pair && !p.gmax && !p.gshift && tiles_m * (p.cout / 128) >= 2 * DZ_NUM_SMS &&
-                      (use_pair == 128 ? p.cout % 128 == 0 : p.cout % 256 == 0);
-    const int bn_pair = (p.cout % 256 == 0 && use_pair != 128) ? 256 : 128;
+    const int bn = p.cout > 64 ? 128 : (p.cout > 32 ? 64 : 32);
     {
         cuuint64_t ktot = (cuuint64_t)p.KH * p.KW * p.cin;
         cuuint64_t dims[2] = {ktot, (cuuint64_t)p.cout};
         cuuint64_t strides[1] = {ktot * 4};
-        cuuint32_t box[2] = {(cuuint32_t)CT_BK, (cuuint32_t)(pair ? bn_pair / 2 : bn)};
+        cuuint32_t box[2] = {(cuuint32_t)CT_BK, (cuuint32_t)bn};
         cuuint32_t estr[2] = {1, 1};
         CUresult r = enc(&tmB, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)p.w, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { dz_set_error("cuTensorMapEncodeTiled(B) failed: %d", (int)r); return DZ_ERR_CUDA; }
     }
     CUtensorMap tmO = tmB;
-    static const int no_tma_store = getenv("DZ_CONV2D_NO_TMA_STORE") ? 1 : 0;
-    p.tma_store = (!p.gmax && !no_tma_store && p.os == 1 && p.oy0 == 0 && p.ox0 == 0 && p.OH == p.Ho && p.OW == p.Wo && bn >= 32 &&
-                   (reinterpret_cast<uintptr_t>(p.out) & 15) == 0) ? 1 : 0;
-    if (!p.tma_store && !p.gmax && !no_tma_store && p.os >= 2 && p.OH == p.Ho * p.os && p.OW == p.Wo * p.os && p.Ho % 2 == 0 && bn >= 32 &&
+    if (!p.tma_store && !p.gmax && !no_tma_store && p.os >= 2 && p.OH == p.Ho * p.os && p.OW == p.Wo * p.os && p.Ho % 2 == 0 &&
         p.oy0 < p.os && p.ox0 < p.os && (reinterpret_cast<uintptr_t>(p.out) & 15) == 0) {
         // strided output (ConvTranspose2d as os*os 1x1 convs): 5-D view [C][dx][x][dy][b*Ho + y], one TMA store per warp as above instead of
-        // per-thread strided stores (256 -> 256 @94^2, 8 frames: 70 us per (dy, dx) with 14 % tensor pipe before)
+        // per-thread strided stores
         p.tma_store = 2;
         cuuint64_t dims[5] = {(cuuint64_t)(p.out_coff + p.cout), (cuuint64_t)p.os, (cuuint64_t)p.Wo, (cuuint64_t)p.os, (cuuint64_t)p.Ho * p.B};
         cuuint64_t strides[4] = {(cuuint64_t)p.out_cstride * 4, (cuuint64_t)p.os * p.out_cstride * 4, (cuuint64_t)p.OW * p.out_cstride * 4,
@@ -908,32 +382,21 @@ int dz_conv2d_fwd_tc(const Conv2dParams& p_in, int mode, cudaStream_t st) {
         // channels [0, out_coff + cout) of the (possibly wider, concatenated) output tensor: stores past cout are clipped
         cuuint64_t dims[4] = {(cuuint64_t)(p.out_coff + p.cout), (cuuint64_t)p.OW, (cuuint64_t)p.OH, (cuuint64_t)p.B};
         cuuint64_t strides[3] = {(cuuint64_t)p.out_cstride * 4, (cuuint64_t)p.OW * p.out_cstride * 4, (cuuint64_t)p.OH * p.OW * p.out_cstride * 4};
-        cuuint32_t box[4] = {32, (cuuint32_t)CT_TW, 2, 1};
+        cuuint32_t box[4] = {32, (cuuint32_t)TW, (cuuint32_t)(32 / TW), 1};      // one warp's 32 pixels
         cuuint32_t estr[4] = {1, 1, 1, 1};
         CUresult r = enc(&tmO, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)p.out, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { dz_set_error("cuTensorMapEncodeTiled(out) failed: %d", (int)r); return DZ_ERR_CUDA; }
     }
-    // 3x3 stride-1 convolutions: the halo kernel (DZ_CONV2D_HALO: 0 = off, 1 = single CTA, 2 = CTA pair)
-    static const int halo = getenv("DZ_CONV2D_HALO") ? atoi(getenv("DZ_CONV2D_HALO")) : 1;
-    if (halo && p.KH == 3 && p.KW == 3 && p.stride == 1 && p.tma_store == 1 && !p.gshift && !(p.dbg & 3) &&
-        tiles_m * dz_cdiv(p.cout, 128) >= 2 * DZ_NUM_SMS)
-        return launch_halo(p, halo, st);
-    if (pair) return bn_pair == 256 ? launch_tf32_pair<256, 2>(p, tmA, tmB, tmO, st) : launch_tf32_pair<128, 2>(p, tmA, tmB, tmO, st);
-    // two stacked patches per CTA when there are enough tiles to still fill the GPU (the weight tile is then loaded once
-    // for 256 output pixels)
-    const long long tiles1 = (long long)dz_cdiv(p.Wo, CT_TW) * dz_cdiv(p.Ho, CT_TH) * p.B * dz_cdiv(p.cout, bn);
-    const bool two = tiles1 >= 2 * DZ_NUM_SMS - 16;
-    // >= 1 single-patch tile per SM: two co-resident single-patch CTAs per SM instead of one double-patch CTA, so that one
-    // CTA's epilogue and set-up overlap the other's main loop (batch 8: +2.5 % frames/s, batch 1: +1.9 %).
-    // DZ_CONV2D_OCC2=0 switches it off, =n sets the threshold to n tiles per SM.
-    static const int occ2 = getenv("DZ_CONV2D_OCC2") ? atoi(getenv("DZ_CONV2D_OCC2")) : 1;
-    if (occ2 && tiles1 >= occ2 * DZ_NUM_SMS && bn == 128) return launch_tf32<128, 1, 2>(p, tmA, tmB, tmO, st);
-    if (occ2 && tiles1 >= occ2 * DZ_NUM_SMS && bn == 64) return launch_tf32<64, 1, 2>(p, tmA, tmB, tmO, st);
+    if (halo) switch (bn) {
+        case 128: return launch_tf32<128, true>(p, tmA, tmB, tmO, st);
+        case 64: return launch_tf32<64, true>(p, tmA, tmB, tmO, st);
+        default: return launch_tf32<32, true>(p, tmA, tmB, tmO, st);
+    }
     switch (bn) {
-        case 128: return two ? launch_tf32<128, 2>(p, tmA, tmB, tmO, st) : launch_tf32<128, 1>(p, tmA, tmB, tmO, st);
-        case 64: return two ? launch_tf32<64, 2>(p, tmA, tmB, tmO, st) : launch_tf32<64, 1>(p, tmA, tmB, tmO, st);
-        default: return two ? launch_tf32<32, 2>(p, tmA, tmB, tmO, st) : launch_tf32<32, 1>(p, tmA, tmB, tmO, st);
+        case 128: return launch_tf32<128, false>(p, tmA, tmB, tmO, st);
+        case 64: return launch_tf32<64, false>(p, tmA, tmB, tmO, st);
+        default: return launch_tf32<32, false>(p, tmA, tmB, tmO, st);
     }
 }
 

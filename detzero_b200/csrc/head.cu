@@ -1,4 +1,4 @@
-// head.cu -- CenterHead heat-map decode (top-K + box decode) and device-resident rotated-BEV NMS, sm_100a.
+// head.cu -- CenterHead heat-map decode (top-K + box decode) and device-resident rotated-BEV NMS, sm_90a.
 //
 // Replaces centernet_utils._topk / decode_bbox_from_heatmap (detection/detzero_det/utils/centernet_utils.py:138-230),
 // CenterHead.generate_predicted_boxes (center_head.py:315-368), model_nms_utils.class_agnostic_nms

@@ -1,4 +1,4 @@
-// refine.cu -- refiner (GRM / PRM / CRM) building blocks, exact-fp32 SIMT path, sm_100a.
+// refine.cu -- refiner (GRM / PRM / CRM) building blocks, exact-fp32 SIMT path, sm_90a.
 //
 // Replaces, for refining/detzero_refine/models/modules/transformer/multi_head_attention.py:90-295
 // (multi_head_attention_forward), decoder.py:48-92 (TransformerDecoderLayer.forward), position_encoding.py,

@@ -1,4 +1,4 @@
-// rulebook.cu -- rulebook (neighbour-table) build for submanifold and strided sparse convolution, sm_100a.
+// rulebook.cu -- rulebook (neighbour-table) build for submanifold and strided sparse convolution, sm_90a.
 //
 // Replaces spconv's generate_subm_conv_inds / generate_conv_inds_stage{1,2} (GPU hash table) used through
 // SubMConv3d / SparseConv3d at detection/detzero_det/models/centerpoint_modules/backbone3d.py:68-71,93-100.
@@ -309,7 +309,7 @@ extern "C" int dz_rulebook_conv(const int32_t* in_coords, const int* d_n_in, int
 // The conv kernel owns 128 output rows per CTA and skips a kernel offset k when NONE of its rows has a neighbour through
 // k.  In coordinate order a tile touches ~21-23 of the 27 offsets although each row only has 4.6 (0.1 m level) to 14.7
 // (0.8 m level) neighbours; after grouping rows by mask a tile touches 7-17 offsets, i.e. the gather and the MMA work
-// drop 1.3-3x (synthetic Waymo frame, profiles/r01_spconv_notes.md).  spconv's implicit-GEMM path sorts by the full mask
+// drop 1.3-3x (synthetic Waymo frame).  spconv's implicit-GEMM path sorts by the full mask
 // for the same reason; here a single-pass counting sort on a 12-bit digest of the mask is enough: the digest keeps the
 // five "line present" bits of the z+-1 planes, the six x+-1 bits of the centre plane and one more (order found by greedy
 // search on the frame statistics), most significant first.  The digest and its histogram are produced by the rulebook

@@ -1,4 +1,4 @@
-// spconv.cu -- sparse convolution forward (output-stationary implicit GEMM over the neighbour table), sm_100a.
+// spconv.cu -- sparse convolution forward (output-stationary implicit GEMM over the neighbour table), sm_90a.
 //
 // Replaces spconv SubMConv3d / SparseConv3d forward + BatchNorm1d(eval) + bias + residual + ReLU as composed at
 // detection/detzero_det/models/centerpoint_modules/backbone3d.py:64-83 (post_act_block) and :105-121

@@ -1,4 +1,4 @@
-// spconv_bf16.cu -- persistent, warp-specialised sparse convolution forward on tcgen05 with bf16 operand PLANES (sm_100a).
+// spconv_bf16.cu -- persistent, warp-specialised sparse convolution forward on wgmma with bf16 operand PLANES (sm_90a).
 //
 // Same contract as spconv.cu / spconv_tc.cu (SubMConv3d / SparseConv3d + folded BatchNorm1d + bias + residual + ReLU,
 // detection/detzero_det/models/centerpoint_modules/backbone3d.py:64-83,105-121) for the modes DZ_BF16 and DZ_BF16X2.
@@ -6,26 +6,26 @@
 // Feature storage ("planes"): a row holds PLANES x C bf16 values, [plane 0 | plane 1].
 //   PLANES = 1 (DZ_BF16)   : x ~ p0                     = RN_bf16(x)                       2 bytes / value
 //   PLANES = 2 (DZ_BF16X2) : x ~ p0 + p1, p1 = RN_bf16(x - p0)  (16 significand bits)      4 bytes / value (= fp32 storage)
-// Weights are split the same way (w = w0 + w1).  The products are accumulated in fp32 TMEM as
+// Weights are split the same way (w = w0 + w1).  The products are accumulated in fp32 registers as
 //   PLANES = 1:  p0 * w0
-//   PLANES = 2:  p0 * [w0 | w1]  (ONE MMA, N = 2*Cout: the two halves are summed in the epilogue)  +  p1 * w0
+//   PLANES = 2:  p0 * w0 + p0 * w1 + p1 * w0
 // i.e. x*w up to the dropped p1*w1 term and the 2^-18 representation error of each operand: per-layer error ~1e-6..1e-5
 // relative to fp32 FMA (tests: <= 2e-5 per layer, <= 2e-4 through a whole backbone) at the MMA and gather cost of ONE
-// TF32 pass (kind::f16 has K = 16 per instruction, a 128-byte smem row holds 64 channels).
+// TF32 pass (bf16 wgmma has K = 16 per instruction, a 128-byte smem row holds 64 channels).
 //
 // Kernel structure (one CTA per SM, persistent over the tile list; roles by warp):
-//   warps 0-3      epilogue: tcgen05.ld of accumulator buffer t&1 -> scale/shift (+residual) -> ReLU -> plane split -> stores
-//   warps 4-11     producers (all of them fill one pipeline stage at a time): cp.async zero-fill gather of the neighbour rows of a 64-element block of
+//   warps 0-7      two consumer warpgroups (64 rows each): wgmma bf16 (M64 x Cout x K16) into register accumulators; after the
+//                  tile's last block the accumulators pass through a shared-memory staging tile 32 columns at a time and
+//                  warps 0-3 run the epilogue: scale/shift (+residual) -> ReLU -> plane split -> stores
+//   warps 8-15     producers (all of them fill one pipeline stage at a time): cp.async zero-fill gather of the neighbour rows of a 64-element block of
 //                  the (offset, channel) reduction dimension into K-major SW128 smem; one lane TMA-loads the weight tile
-//   MMA warp       one thread issues tcgen05.mma kind::f16 (M128 x N x K16) into TMEM accumulator buffer t&1
 //   fence warp     one thread turns "the cp.async data of stage s has landed" (async mbarrier arrival of the producers) into "stage s
-//                  is visible to the tensor core": fence.proxy.async, then arrives on the barrier the MMA thread waits on.  The
-//                  fence costs ~200 clk per step: in the MMA thread it was on the critical path, in the producers it would block
-//                  them for the landing latency (both measured, profiles/r02_spconv_notes.md)
+//                  is visible to the tensor core": fence.proxy.async, then arrives on the barrier the consumers wait on, so
+//                  neither the producers nor the consumers wait for the landing latency themselves
 //   tile warp      walks the CTA's tiles (heaviest-first tile order of the rulebook schedule, serpentine over the CTAs), loads
 //                  the 128 x 27 neighbour rows of tile t+1/t+2 into the double-buffered table while tile t is computed
-// so a tile's prologue (table load) and epilogue hide under the neighbouring tiles' main loops, the smem ring never drains
-// between tiles, and the TMEM accumulator is double-buffered.  No atomics: deterministic; a row's accumulation order over
+// so a tile's prologue (table load) hides under the neighbouring tile's main loop and the producers run ahead into the next
+// tile while the consumers run the epilogue.  No atomics: deterministic; a row's accumulation order over
 // the reduction blocks never depends on the schedule, so results are bit-identical with or without it.
 #include <stdlib.h>
 #include <cuda_bf16.h>
@@ -49,18 +49,21 @@ struct SbCfg {
     static constexpr int STAGE_BYTES = PLANES * SB_A_BYTES + W_BYTES;
     static constexpr int NBR_BYTES = 2 * SB_NPLANES * SB_ROWS * 4;   // double-buffered tile block: K neighbour planes + the row plane
     static constexpr int MISC_BYTES = 2 * 64 * 4 + 2 * COUT * 4 + 512;                     // block lists | scale,shift | barriers
-    static constexpr int STAGES_FIT = (232448 - NBR_BYTES - MISC_BYTES - 1024) / STAGE_BYTES;
-    static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;   // as deep as shared memory allows: 3 .. 8
+    static constexpr int CW = COUT < 32 ? COUT : 32;                                         // accumulator columns per epilogue pass
+    static constexpr int STG_LD = CW + 4;
+    static constexpr int STG_BYTES = SB_ROWS * STG_LD * 4;                                   // epilogue staging tile
+    static constexpr int STAGES_FIT = (232448 - NBR_BYTES - MISC_BYTES - STG_BYTES - 1024) / STAGE_BYTES;
+    static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;   // as deep as shared memory allows: 2 (bf16x2, Cout = 128) .. 8
     // ALL producer warps fill ONE stage at a time (16 rows each): a stage is complete after 1/NPROD of the LSU time a
     // warp-per-stage split needs, so the oldest stage lands early and the ring covers the MMA -> commit -> refill latency
-    static constexpr int NPROD = 8;
-    static constexpr int WARP_MMA = 4 + NPROD;
-    static constexpr int WARP_TILE = WARP_MMA + 1;
+    // with the two consumer warpgroups holding Cout/2 accumulator registers each, 8 producer warps leave too few registers for
+    // Cout >= 64 (spills): 4 there
+    static constexpr int NPROD = COUT >= 64 ? 4 : 8;
+    static constexpr int CONSUMERS = 8;
+    static constexpr int WARP_TILE = CONSUMERS + NPROD;
     static constexpr int WARP_FENCE = WARP_TILE + 1;
     static constexpr int THREADS = 32 * (WARP_FENCE + 1);
-    static constexpr int ACC_COLS = WROWS < 32 ? 32 : WROWS;         // TMEM columns of one accumulator buffer
-    static constexpr int TMEM_COLS = 2 * ACC_COLS;                   // 64 .. 512 (power of two)
-    static constexpr int SMEM = STAGES * STAGE_BYTES + NBR_BYTES + MISC_BYTES + 1024;
+    static constexpr int SMEM = STAGES * STAGE_BYTES + NBR_BYTES + MISC_BYTES + STG_BYTES + 1024;
 };
 
 __device__ __forceinline__ void cp_async16_zfill(uint32_t dst, const void* src, bool valid) {
@@ -74,27 +77,14 @@ __device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t* bar) {
 __device__ __forceinline__ void mbar_wait_bounded(uint64_t* bar, uint32_t parity) {
     uint32_t spins = 0;
     while (!tc::mbar_try_wait(bar, parity)) {
-        if (++spins > (1u << 24)) { printf("spconv_bf16: mbarrier timeout (block %d thread %d)\n", (int)blockIdx.x, (int)threadIdx.x); __trap(); }
+        if (++spins > (1u << 24)) __trap();          // (no printf: a call anywhere in the kernel serialises its wgmma pipeline)
     }
-}
-// 32 lanes x 32 columns, no wait (the caller waits once for several loads)
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
 }
 // bulk copy global -> shared, completion counted in bytes on an mbarrier
 __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* src, uint32_t bytes, uint64_t* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(tc::smem_u32(smem_dst)), "l"(src), "r"(bytes), "r"(tc::smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
     __nv_bfloat162 v = __floats2bfloat162_rn(a, b);
@@ -122,17 +112,15 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
     int* s_blk = s_nbr + 2 * SB_NPLANES * SB_ROWS;                                // [2][64]  live reduction blocks; [63] = count, [62] = tile (-1: end)
     float* s_scale = reinterpret_cast<float*>(s_blk + 2 * 64);
     float* s_shift = s_scale + COUT;
-    uint64_t* full = reinterpret_cast<uint64_t*>(s_shift + COUT);
+    float* s_stg = s_shift + COUT;                                                 // [128][STG_LD] epilogue staging
+    uint64_t* full = reinterpret_cast<uint64_t*>(s_stg + SB_ROWS * Cfg::STG_LD);
     uint64_t* empty = full + S;
     uint64_t* landed = empty + S;                  // producers' cp.async data + weight TMA of a stage have landed (generic proxy)
     uint64_t* nbr_full = landed + S;
     uint64_t* nbr_empty = nbr_full + 2;
-    uint64_t* acc_full = nbr_empty + 2;
-    uint64_t* acc_empty = acc_full + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const bool tr = dbg && blockIdx.x == 0;                            // clock trace of CTA 0 (tools/trace_spconv_bf16.py)
+    const bool tr = dbg && blockIdx.x == 0;                            // clock trace of CTA 0 (dz_debug_trace)
     long long tr_a = 0, tr_b = 0, tr_c = 0, tr_n = 0;                  // per-role wait / work accumulators
     const long long tr_t0 = tr ? clock64() : 0;
 #define TR_WAIT(acc, stmt) do { if (tr) { const long long c0__ = clock64(); stmt; acc += clock64() - c0__; } else { stmt; } } while (0)
@@ -141,12 +129,10 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
 
     if (threadIdx.x == 0) {
         tc::prefetch_tmap(&tmW);
-        for (int s = 0; s < S; ++s) { tc::mbar_init(landed + s, 32 * Cfg::NPROD + 1); tc::mbar_init(full + s, 1); tc::mbar_init(empty + s, 1); }
+        for (int s = 0; s < S; ++s) { tc::mbar_init(landed + s, 32 * Cfg::NPROD + 1); tc::mbar_init(full + s, 1); tc::mbar_init(empty + s, Cfg::CONSUMERS); }
         for (int b = 0; b < 2; ++b) {
             tc::mbar_init(nbr_full + b, 1);
-            tc::mbar_init(nbr_empty + b, Cfg::NPROD + 2 + 4);
-            tc::mbar_init(acc_full + b, 1);
-            tc::mbar_init(acc_empty + b, 4);
+            tc::mbar_init(nbr_empty + b, Cfg::NPROD + 1 + Cfg::CONSUMERS);
         }
         tc::fence_barrier_init();
     }
@@ -154,11 +140,7 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
         s_scale[c] = scale ? __ldg(scale + c) : 1.f;
         s_shift[c] = shift ? __ldg(shift + c) : 0.f;
     }
-    if (warp == Cfg::WARP_MMA) tc::tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-    tc::tcgen05_fence_before();
     __syncthreads();
-    tc::tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     if (warp == Cfg::WARP_TILE) {
         // ================= tile warp: neighbour rows + live block list of the CTA's next tile ===================================
@@ -234,11 +216,11 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
             }
             ++t;
         }
-    } else if (warp >= 4 && warp < 4 + Cfg::NPROD) {
+    } else if (warp >= Cfg::CONSUMERS && warp < Cfg::CONSUMERS + Cfg::NPROD) {
         // ================= producers ============================================================================================
-        const int pw = warp - 4;
-        constexpr int RPW = SB_ROWS / Cfg::NPROD;    // rows per producer warp (16)
-        constexpr int RPL = RPW / 4;                 // rows per lane (8 lanes cover the 8 chunks of a row): 4 = one int4 of the table
+        const int pw = warp - Cfg::CONSUMERS;
+        constexpr int RPW = SB_ROWS / Cfg::NPROD;    // rows per producer warp (16 or 32)
+        constexpr int RPL = RPW / 4;                 // rows per lane (8 lanes cover the 8 chunks of a row): 4 or 8 = one or two int4 of the table
         const int j = lane & 7, rg = lane >> 3;
         const int rbase = pw * RPW + rg * RPL;
         const uint32_t smem_u = tc::smem_u32(smem);
@@ -310,52 +292,12 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
                 }
             }
         }
-    } else if (warp == Cfg::WARP_MMA) {
-        // ================= MMA issuer ==========================================================================================
-        if (lane == 0) {
-            constexpr uint32_t idesc0 = tc::instr_desc(1, 128, Cfg::WROWS);        // bf16 x bf16 -> fp32, N = PLANES * COUT
-            constexpr uint32_t idesc1 = tc::instr_desc(1, 128, COUT);
-            const uint32_t smem_u = tc::smem_u32(smem);
-            int g = 0;
-            for (int t = 0;; ++t) {
-                const int b = t & 1;
-                TR_WAIT(tr_a, mbar_wait_bounded(nbr_full + b, (t >> 1) & 1));
-                if (s_blk[b * 64 + 62] < 0) {
-                    if (tr) { dbg[2048 + 16] = tr_a; dbg[2048 + 17] = tr_b; dbg[2048 + 18] = tr_c; dbg[2048 + 19] = tr_n; dbg[2048 + 20] = clock64() - tr_t0; }
-                    break;
-                }
-                const int nb = s_blk[b * 64 + 63];
-                tc::mbar_arrive(nbr_empty + b);                         // only `nb` was needed
-                TR_WAIT(tr_a, mbar_wait_bounded(acc_empty + b, ((t >> 1) & 1) ^ 1));   // epilogue of tile t-2 has drained this accumulator
-                tc::tcgen05_fence_after();
-                const uint32_t acc = tmem_base + (uint32_t)(b * Cfg::ACC_COLS);
-                for (int i = 0; i < nb; ++i, ++g) {
-                    const int s = g % S;
-                    TR_WAIT(tr_b, mbar_wait_bounded(full + s, (g / S) & 1));
-                    const long long tr_i0 = tr ? clock64() : 0;
-                    tc::tcgen05_fence_after();          // (the generic->async proxy fence is executed by the producers before they arrive)
-                    const uint32_t sa = smem_u + (uint32_t)(s * Cfg::STAGE_BYTES);
-                    const uint64_t a0 = tc::smem_desc_sw128(sa), wd = tc::smem_desc_sw128(sa + PLANES * SB_A_BYTES);
-#pragma unroll
-                    for (int kk = 0; kk < 4; ++kk)
-                        tc::mma_f16(acc, a0 + (uint64_t)(kk * 2), wd + (uint64_t)(kk * 2), idesc0, (i | kk) ? 1u : 0u);
-                    if (PLANES == 2) {
-                        const uint64_t a1 = tc::smem_desc_sw128(sa + SB_A_BYTES);
-#pragma unroll
-                        for (int kk = 0; kk < 4; ++kk)
-                            tc::mma_f16(acc, a1 + (uint64_t)(kk * 2), wd + (uint64_t)(kk * 2), idesc1, 1u);
-                    }
-                    tc::mma_commit(empty + s);
-                    if (tr) { tr_c += clock64() - tr_i0; ++tr_n; }
-                }
-                tc::mma_commit(acc_full + b);
-            }
-        }
     } else {
-        // ================= epilogue (warps 0-3 <-> TMEM lane quarters) ========================================================
-        const int q = warp;
-        const int trow = q * 32 + lane;
-        constexpr int CW = COUT < 32 ? COUT : 32;         // channels per pass
+        // ================= consumers: warpgroup cg accumulates rows [64cg, 64cg+64) of each tile; warps 0-3 run the epilogue ======
+        const int cg = warp >> 2;
+        const uint32_t smem_u = tc::smem_u32(smem);
+        constexpr int CW = Cfg::CW;
+        int g = 0;
         for (int t = 0;; ++t) {
             const int b = t & 1;
             TR_WAIT(tr_a, mbar_wait_bounded(nbr_full + b, (t >> 1) & 1));
@@ -364,31 +306,49 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
                 break;
             }
             const int nb = s_blk[b * 64 + 63];
-            const int r = s_nbr[b * SB_NPLANES * SB_ROWS + K * SB_ROWS + trow];
+            const int r = warp < 4 ? s_nbr[b * SB_NPLANES * SB_ROWS + K * SB_ROWS + threadIdx.x] : -1;
             __syncwarp();
             if (lane == 0) tc::mbar_arrive(nbr_empty + b);
-            TR_WAIT(tr_b, mbar_wait_bounded(acc_full + b, (t >> 1) & 1));
-            const long long tr_e0 = tr ? clock64() : 0;
-            tc::tcgen05_fence_after();
-            const uint32_t acc = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(b * Cfg::ACC_COLS);
-#pragma unroll 1
-            for (int c0 = 0; c0 < COUT; c0 += CW) {
-                uint32_t v0[32], v1[32];
-                tmem_ld32_nowait(acc + (uint32_t)c0, v0);
-                if (PLANES == 2 && COUT >= 32) tmem_ld32_nowait(acc + (uint32_t)(COUT + c0), v1);
-                tmem_ld_wait();
-                if (c0 + CW >= COUT) {                    // last TMEM read of this tile: hand the accumulator back to the MMA warp
-                    tc::tcgen05_fence_before();
-                    __syncwarp();
-                    if (lane == 0) tc::mbar_arrive(acc_empty + b);
+            float acc[COUT / 2];
+#pragma unroll
+            for (int i = 0; i < COUT / 2; ++i) acc[i] = 0.f;
+            for (int i = 0; i < nb; ++i, ++g) {
+                const int s = g % S;
+                TR_WAIT(tr_b, mbar_wait_bounded(full + s, (g / S) & 1));
+                // (the generic->async proxy fence is executed by the fence warp before it arrives)
+                const uint32_t sa = smem_u + (uint32_t)(s * Cfg::STAGE_BYTES) + cg * 64 * 128;
+                const uint32_t sw = smem_u + (uint32_t)(s * Cfg::STAGE_BYTES + PLANES * SB_A_BYTES);
+                const uint64_t a0 = tc::smem_desc_sw128(sa), w0 = tc::smem_desc_sw128(sw);
+                tc::wgmma_fence();
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk) tc::wgmma<COUT, tc::K_BF16>(acc, a0 + (uint64_t)(kk * 2), w0 + (uint64_t)(kk * 2), 1u);
+                if (PLANES == 2) {
+                    const uint64_t a1 = tc::smem_desc_sw128(sa + SB_A_BYTES), w1 = tc::smem_desc_sw128(sw + COUT * 128);
+#pragma unroll
+                    for (int kk = 0; kk < 4; ++kk) {
+                        tc::wgmma<COUT, tc::K_BF16>(acc, a0 + (uint64_t)(kk * 2), w1 + (uint64_t)(kk * 2), 1u);
+                        tc::wgmma<COUT, tc::K_BF16>(acc, a1 + (uint64_t)(kk * 2), w0 + (uint64_t)(kk * 2), 1u);
+                    }
                 }
-                if (r >= 0) {
+                tc::wgmma_commit();
+                tc::wgmma_wait_one();                   // this step's MMAs stay in flight; the previous step's stage is free
+                __syncwarp();
+                if (lane == 0 && i > 0) tc::mbar_arrive(empty + (g - 1) % S);
+            }
+            tc::wgmma_wait_all();
+            __syncwarp();
+            if (lane == 0 && nb > 0) tc::mbar_arrive(empty + (g - 1) % S);
+            const long long tr_e0 = tr ? clock64() : 0;
+#pragma unroll
+            for (int c0 = 0; c0 < COUT; c0 += CW) {
+                tc::named_sync(1, 32 * Cfg::CONSUMERS);             // the previous pass has read the staging tile
+                tc::acc_cols_to_smem<COUT>(acc, s_stg, Cfg::STG_LD, cg * 64, c0, CW);
+                tc::named_sync(1, 32 * Cfg::CONSUMERS);
+                if (warp < 4 && r >= 0) {
                     float o[CW];
 #pragma unroll
                     for (int jj = 0; jj < CW; ++jj) {
-                        float a = __uint_as_float(v0[jj]);
-                        if (PLANES == 2) a += (COUT >= 32) ? __uint_as_float(v1[jj]) : __uint_as_float(v0[COUT + jj]);
-                        if (nb == 0) a = 0.f;
+                        const float a = nb == 0 ? 0.f : s_stg[threadIdx.x * Cfg::STG_LD + jj];
                         o[jj] = fmaf(a, s_scale[c0 + jj], s_shift[c0 + jj]);
                     }
                     if (residual) {
@@ -428,9 +388,6 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
         }
     }
 #undef TR_WAIT
-    tc::tcgen05_fence_before();
-    __syncthreads();
-    if (warp == Cfg::WARP_MMA) tc::tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
 }
 
 // ---- tensor-map cache: the weight matrix of a layer never moves, encode its map once ---------------------------------------

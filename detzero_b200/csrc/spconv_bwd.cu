@@ -1,4 +1,4 @@
-// spconv_bwd.cu -- backward of the sparse convolution on the same neighbour tables (SURVEY.md §8f row 1), exact fp32, sm_100a.
+// spconv_bwd.cu -- backward of the sparse convolution on the same neighbour tables (SURVEY.md §8f row 1), exact fp32, sm_90a.
 //
 // The reference trains through spconv's autograd (detection/tools/train_utils.py:59-68: loss.backward() over SubMConv3d /
 // SparseConv3d, backbone3d.py:64-121).  With out[o] = sum_k W[k] in[nbr[k][o]]:

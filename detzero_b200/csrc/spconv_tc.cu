@@ -1,4 +1,4 @@
-// spconv_tc.cu -- sparse convolution forward on the 5th-gen tensor cores (tcgen05, TF32 operands, fp32 TMEM accumulators).
+// spconv_tc.cu -- sparse convolution forward on the Hopper tensor cores (wgmma, TF32 operands, fp32 register accumulators).
 //
 // Same contract as the exact-fp32 kernel in spconv.cu (SubMConv3d / SparseConv3d + folded BatchNorm1d + bias + residual
 // + ReLU, backbone3d.py:64-83,105-121) for DZ_TF32.  spconv's own default keeps TF32 off (SURVEY A.4), so this mode
@@ -11,10 +11,11 @@
 // two offsets, for Cin = 64 an offset spans two blocks -- so narrow layers still fill the MMA K dimension.  Blocks whose
 // offsets no row of the tile uses are skipped (that is what the schedule maximises).  Per block, the producer warps (PW
 // per pipeline stage) gather the neighbour rows straight from global/L2 into shared memory with cp.async (zero-fill for
-// missing neighbours) in the canonical K-major 128B-swizzled UMMA layout, one thread TMA-loads the matching
-// W[cout][k-block] tile, and one thread issues tcgen05.mma (M=128, N=Cout, K=8) into TMEM.  Warps 0-3 then run the
-// epilogue: tcgen05.ld -> scale/shift (+residual) -> ReLU -> 128-bit stores to row order[p].  No atomics: deterministic,
-// and bit-identical with or without a schedule (a row's accumulation order over k never changes).
+// missing neighbours) in the canonical K-major 128B-swizzled layout, one thread TMA-loads the matching W[cout][k-block]
+// tile, and two consumer warpgroups (64 rows each) issue wgmma (M=64, N=Cout, K=8) into register accumulators.  After the
+// last block the accumulators go through the (then idle) pipeline buffers and warps 0-3 run the epilogue, one row per
+// thread: scale/shift (+residual) -> ReLU -> 128-bit stores to row order[p].  No atomics: deterministic, and bit-identical
+// with or without a schedule (a row's accumulation order over k never changes).
 #include <stdlib.h>
 #include "common.cuh"
 #include "tc.cuh"
@@ -27,17 +28,17 @@ template <int COUT, int PW>
 struct StCfg {
     static constexpr int W_BYTES = COUT * 128;
     static constexpr int STAGE_BYTES = ST_A_BYTES + W_BYTES;
-    // 2 CTAs/SM (the other CTA's prologue/epilogue overlaps this one's main loop)
-    // Cout = 128 only occurs with K = 3 (conv_out): few k-steps, so 2 CTAs/SM beat depth.  (3 stages / 3 CTAs per SM for
-    // Cout <= 32 was measured: no gain.)
+    // Cout = 128 only occurs with K = 3 (conv_out): few k-steps, so a shallow ring suffices
     static constexpr int STAGES = COUT >= 128 ? 3 : 4;
-    // PW producer warps per stage: warp w gathers its 128/PW rows of the steps it = s, s+STAGES, ... into stage s = w % STAGES
-    // (a single warp sustains only one LDGSTS per ~70-130 cycles, tools/ubench_gather.cu; the SM's LSU takes one per ~8.5);
-    // warp STAGES*PW issues the MMAs and owns TMEM; warps 0-3 double as the epilogue
+    // PW producer warps per stage: warp w gathers its 128/PW rows of the steps it = s, s+STAGES, ... into stage s = (w-8) % STAGES
+    // (one warp alone cannot keep enough cp.async gathers in flight); warps 0-7 are the two consumer
+    // warpgroups, warps 0-3 double as the epilogue
     static constexpr int PRODUCERS = STAGES * PW;
-    static constexpr int THREADS = 32 * (PRODUCERS + 1);
+    static constexpr int CONSUMERS = 8;
+    static constexpr int THREADS = 32 * (CONSUMERS + PRODUCERS);
+    static constexpr int ACC_LD = COUT + 4;                    // row pitch of the accumulator tile staged for the epilogue
     static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 + ST_KMAX * ST_ROWS * 4 + 128 * 4 + 256;
-    static constexpr int TMEM_COLS = COUT < 32 ? 32 : COUT;
+    static_assert(ST_ROWS * ACC_LD * 4 <= STAGES * STAGE_BYTES, "accumulator staging must fit in the pipeline buffers");
 };
 
 __device__ __forceinline__ void cp_async16_zfill(uint32_t dst, const void* src, bool valid) {
@@ -58,7 +59,7 @@ k_spconv_tf32(const __grid_constant__ CUtensorMap tmW, const float* __restrict__
               int nbr_cap, const int32_t* __restrict__ order, const int* __restrict__ d_n_out, int out_cap, const float* __restrict__ scale,
               const float* __restrict__ shift, const float* __restrict__ residual, int relu, float* __restrict__ out, long long* __restrict__ dbgbuf) {
     using Cfg = StCfg<COUT, PW>;
-    const bool tr = dbgbuf && blockIdx.x == 1;      // clock trace of CTA 1 (tools/trace_spconv.py); dbgbuf is NULL in normal runs
+    const bool tr = dbgbuf && blockIdx.x == 1;      // clock trace of CTA 1 (dz_debug_trace); dbgbuf is NULL in normal runs
     if (tr && threadIdx.x == 0) dbgbuf[0] = clock64();
     const int n = min(*d_n_out, out_cap);
     // under a tile schedule CTAs take the tiles heaviest-first (launch order ~ blockIdx order): order[nbr_cap + i]
@@ -71,9 +72,7 @@ k_spconv_tf32(const __grid_constant__ CUtensorMap tmW, const float* __restrict__
     int* s_blocks = s_nbr + ST_KMAX * ST_ROWS;                                            // active block list (<= 108)
     uint64_t* full = reinterpret_cast<uint64_t*>(s_blocks + 124);
     uint64_t* empty = full + Cfg::STAGES;
-    uint64_t* tmem_full = empty + Cfg::STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);
-    int* s_nb = reinterpret_cast<int*>(tmem_slot + 1);
+    int* s_nb = reinterpret_cast<int*>(empty + Cfg::STAGES);
     unsigned* s_mask = reinterpret_cast<unsigned*>(s_nb + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -82,12 +81,10 @@ k_spconv_tf32(const __grid_constant__ CUtensorMap tmW, const float* __restrict__
 
     if (threadIdx.x == 0) {
         tc::prefetch_tmap(&tmW);
-        for (int s = 0; s < Cfg::STAGES; ++s) { tc::mbar_init(full + s, 32 * PW + 1); tc::mbar_init(empty + s, 1); }
-        tc::mbar_init(tmem_full, 1);
+        for (int s = 0; s < Cfg::STAGES; ++s) { tc::mbar_init(full + s, 32 * PW + 1); tc::mbar_init(empty + s, Cfg::CONSUMERS); }
         tc::fence_barrier_init();
         *s_mask = 0u;
     }
-    if (warp == Cfg::PRODUCERS) tc::tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
     __syncthreads();
     // ---- neighbour rows of this tile + which offsets are populated
     if (warp < 4) {
@@ -115,9 +112,7 @@ k_spconv_tf32(const __grid_constant__ CUtensorMap tmW, const float* __restrict__
         mine = __reduce_or_sync(0xffffffffu, mine);
         if (lane == 0 && mine) atomicOr(s_mask, mine);
     }
-    tc::tcgen05_fence_before();
     __syncthreads();
-    tc::tcgen05_fence_after();
     if (threadIdx.x == 0) {
         const unsigned mask = *s_mask;
         int nb = 0;
@@ -131,16 +126,15 @@ k_spconv_tf32(const __grid_constant__ CUtensorMap tmW, const float* __restrict__
     }
     __syncthreads();
     const int nb = *s_nb;
-    const uint32_t tmem_base = *tmem_slot;
     if (tr && threadIdx.x == 0) { dbgbuf[1] = clock64(); dbgbuf[2] = nb; }
 
-    if (warp < Cfg::PRODUCERS) {
+    if (warp >= Cfg::CONSUMERS) {
         // ================= producers: warp w fills rows [part*RPW, (part+1)*RPW) of stage s for the steps s, s+STAGES, ... ===
         constexpr int RPW = ST_ROWS / PW;           // rows per producer warp
         constexpr int RPL = RPW / 4;                // rows per 8-lane group
         const int j = lane & 7;                     // 16-byte chunk inside the 128-byte row
         const int rg = lane >> 3;                   // lane covers chunk j of rows rbase .. rbase+RPL-1
-        const int s = warp % Cfg::STAGES, part = warp / Cfg::STAGES;
+        const int s = (warp - Cfg::CONSUMERS) % Cfg::STAGES, part = (warp - Cfg::CONSUMERS) / Cfg::STAGES;
         const int rbase = part * RPW + rg * RPL;
         unsigned char* sa = smem + s * Cfg::STAGE_BYTES;
         const uint32_t sa_u = tc::smem_u32(sa);
@@ -184,70 +178,74 @@ k_spconv_tf32(const __grid_constant__ CUtensorMap tmW, const float* __restrict__
             cp_async_mbar_arrive_noinc(full + s);
             if (tr && lane == 0 && part == 0 && it < 120) dbgbuf[8 + it * 8 + 2] = clock64();
         }
-    }
-    if (warp < 4) {
-        // ================= epilogue =================
-        const int q = warp;                         // TMEM lane quarter == warp id for warps 0..3
-        const int pos = row0 + q * 32 + lane;       // tile position; the output row is order[pos] under a tile schedule
-        const int r = pos < n ? (order ? __ldg(order + pos) : pos) : n;
-        tc::mbar_wait(tmem_full, 0);
-        tc::tcgen05_fence_after();
-        if (tr && threadIdx.x == 0) dbgbuf[3] = clock64();
-#pragma unroll 1
-        for (int c0 = 0; c0 < COUT; c0 += 32) {
-            float v[32];
-            tc::tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-            if (r < n) {
+    } else {
+        // ================= consumers: warpgroup g accumulates rows [64g, 64g+64) of the tile =================
+        const int g = warp >> 2;
+        float acc[COUT / 2];
 #pragma unroll
-                for (int jj = 0; jj < 32; jj += 4) {
-                    const int ch = c0 + jj;
-                    if (ch >= COUT) break;
-                    float4 o = nb > 0 ? make_float4(v[jj], v[jj + 1], v[jj + 2], v[jj + 3]) : make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (scale) { float4 sc = __ldg(reinterpret_cast<const float4*>(scale + ch)); o.x *= sc.x; o.y *= sc.y; o.z *= sc.z; o.w *= sc.w; }
-                    if (shift) { float4 sh = __ldg(reinterpret_cast<const float4*>(shift + ch)); o.x += sh.x; o.y += sh.y; o.z += sh.z; o.w += sh.w; }
-                    if (residual) {
-                        float4 rr = __ldg(reinterpret_cast<const float4*>(residual + (size_t)r * COUT + ch));
-                        o.x += rr.x; o.y += rr.y; o.z += rr.z; o.w += rr.w;
+        for (int i = 0; i < COUT / 2; ++i) acc[i] = 0.f;
+        for (int it = 0; it < nb; ++it) {
+            const int s = it % Cfg::STAGES;
+            if (tr && threadIdx.x == 0 && it < 120) dbgbuf[8 + it * 8 + 3] = clock64();
+            tc::mbar_wait(full + s, (it / Cfg::STAGES) & 1);
+            if (tr && threadIdx.x == 0 && it < 120) dbgbuf[8 + it * 8 + 4] = clock64();
+            tc::fence_proxy_async();                // cp.async (generic proxy) writes -> tensor-core (async proxy) reads
+            const uint32_t sa = tc::smem_u32(smem + s * Cfg::STAGE_BYTES);
+            const uint64_t adesc = tc::smem_desc_sw128(sa + g * 64 * 128), bdesc = tc::smem_desc_sw128(sa + ST_A_BYTES);
+            tc::wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) tc::wgmma<COUT, tc::K_TF32>(acc, adesc + (uint64_t)(kk * 2), bdesc + (uint64_t)(kk * 2), 1u);
+            tc::wgmma_commit();
+            tc::wgmma_wait_one();                       // this step's MMAs stay in flight; the previous step's stage is free
+            __syncwarp();
+            if (lane == 0 && it > 0) tc::mbar_arrive(empty + (it - 1) % Cfg::STAGES);
+            if (tr && threadIdx.x == 0 && it < 120) dbgbuf[8 + it * 8 + 5] = clock64();
+        }
+        tc::wgmma_wait_all();
+        __syncwarp();
+        if (lane == 0 && nb > 0) tc::mbar_arrive(empty + (nb - 1) % Cfg::STAGES);
+        // every stage has been consumed: the pipeline buffers hold the accumulator tile for the epilogue
+        float* stg = reinterpret_cast<float*>(smem);
+        tc::named_sync(1, 32 * Cfg::CONSUMERS);
+        tc::acc_to_smem<COUT>(acc, stg, Cfg::ACC_LD, g * 64);
+        tc::named_sync(1, 32 * Cfg::CONSUMERS);
+        if (warp < 4) {
+            // ================= epilogue: thread = tile row =================
+            const int pos = row0 + threadIdx.x;     // tile position; the output row is order[pos] under a tile schedule
+            const int r = pos < n ? (order ? __ldg(order + pos) : pos) : n;
+            if (tr && threadIdx.x == 0) dbgbuf[3] = clock64();
+#pragma unroll 1
+            for (int c0 = 0; c0 < COUT; c0 += 32) {
+                float v[32];
+                if (c0 + 32 <= COUT) tc::smem_row32(stg, Cfg::ACC_LD, threadIdx.x, c0, v);
+                else { for (int i = 0; i < 16; ++i) v[i] = stg[threadIdx.x * Cfg::ACC_LD + c0 + i]; }
+                if (r < n) {
+#pragma unroll
+                    for (int jj = 0; jj < 32; jj += 4) {
+                        const int ch = c0 + jj;
+                        if (ch >= COUT) break;
+                        float4 o = nb > 0 ? make_float4(v[jj], v[jj + 1], v[jj + 2], v[jj + 3]) : make_float4(0.f, 0.f, 0.f, 0.f);
+                        if (scale) { float4 sc = __ldg(reinterpret_cast<const float4*>(scale + ch)); o.x *= sc.x; o.y *= sc.y; o.z *= sc.z; o.w *= sc.w; }
+                        if (shift) { float4 sh = __ldg(reinterpret_cast<const float4*>(shift + ch)); o.x += sh.x; o.y += sh.y; o.z += sh.z; o.w += sh.w; }
+                        if (residual) {
+                            float4 rr = __ldg(reinterpret_cast<const float4*>(residual + (size_t)r * COUT + ch));
+                            o.x += rr.x; o.y += rr.y; o.z += rr.z; o.w += rr.w;
+                        }
+                        if (relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
+                        // round-to-nearest to TF32: the next layer's truncating tensor-core read is then exact (no toward-zero bias)
+                        o.x = tc::rna_tf32(o.x); o.y = tc::rna_tf32(o.y); o.z = tc::rna_tf32(o.z); o.w = tc::rna_tf32(o.w);
+                        *reinterpret_cast<float4*>(out + (size_t)r * COUT + ch) = o;
                     }
-                    if (relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-                    // round-to-nearest to TF32: the next layer's truncating tensor-core read is then exact (no toward-zero bias)
-                    o.x = tc::rna_tf32(o.x); o.y = tc::rna_tf32(o.y); o.z = tc::rna_tf32(o.z); o.w = tc::rna_tf32(o.w);
-                    *reinterpret_cast<float4*>(out + (size_t)r * COUT + ch) = o;
                 }
             }
         }
     }
-    if (warp == Cfg::PRODUCERS) {
-        // ================= MMA issuer =================
-        if (lane == 0) {
-            constexpr uint32_t idesc = tc::instr_desc(2, 128, COUT);
-            for (int it = 0; it < nb; ++it) {
-                const int s = it % Cfg::STAGES;
-                if (tr && it < 120) dbgbuf[8 + it * 8 + 3] = clock64();
-                tc::mbar_wait(full + s, (it / Cfg::STAGES) & 1);
-                if (tr && it < 120) dbgbuf[8 + it * 8 + 4] = clock64();
-                tc::fence_proxy_async();            // cp.async (generic proxy) writes -> tensor-core (async proxy) reads
-                tc::tcgen05_fence_after();
-                const uint32_t sa = tc::smem_u32(smem + s * Cfg::STAGE_BYTES);
-                const uint64_t adesc = tc::smem_desc_sw128(sa), bdesc = tc::smem_desc_sw128(sa + ST_A_BYTES);
-#pragma unroll
-                for (int kk = 0; kk < 4; ++kk)
-                    tc::mma_tf32(tmem_base, adesc + (uint64_t)(kk * 2), bdesc + (uint64_t)(kk * 2), idesc, (it | kk) ? 1u : 0u);
-                tc::mma_commit(empty + s);
-                if (tr && it < 120) dbgbuf[8 + it * 8 + 5] = clock64();
-            }
-            tc::mma_commit(tmem_full);
-        }
-    }
-    tc::tcgen05_fence_before();
-    __syncthreads();
     if (tr && threadIdx.x == 0) dbgbuf[4] = clock64();
-    if (warp == Cfg::PRODUCERS) tc::tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
 }
 
-long long* g_dbgbuf = nullptr;          // shared with spconv_bf16.cu (clock traces, tools/trace_*.py)
+long long* g_dbgbuf = nullptr;          // shared with spconv_bf16.cu (clock traces, dz_debug_trace)
 bool g_trace_on = false;
-extern "C" int dz_debug_trace(long long* host, int n) {      // clock-trace helper for tools/trace_spconv.py (not part of the public header)
+extern "C" int dz_debug_trace(long long* host, int n) {      // clock-trace helper (not part of the public header)
     if (!g_dbgbuf) { if (cudaMalloc(&g_dbgbuf, 4096 * 8) != cudaSuccess) return -1; cudaMemset(g_dbgbuf, 0, 4096 * 8); g_trace_on = true; return 1; }
     cudaDeviceSynchronize();
     return cudaMemcpy(host, g_dbgbuf, (size_t)n * 8, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -1;
@@ -279,7 +277,7 @@ static int launch(const CUtensorMap& tmW, const float* in, int cin, int in_rows,
 
 // weight layout for this path: (cout, K * cin_pad) row-major, cin_pad = 8 for cin <= 8 else cin.
 // (A TMA tile::gather4 producer was built and measured 1.6x slower than the cp.async gather for 128-byte rows -- the TMA unit
-// has a per-row cost -- and a hybrid LSU+TMA split gave no gain: profiles/r01_spconv_notes.md.  Both were removed.)
+// has a per-row cost -- and a hybrid LSU+TMA split gave no gain.  Both were removed.)
 int dz_spconv_fwd_tc3(const float* in, int cin, const int32_t* nbr, int K, int nbr_cap, const int32_t* order, const int* d_n_out, int out_cap,
                       const float* weight, const float* scale, const float* shift, const float* residual, int relu, float* out,
                       int cout, cudaStream_t st);

@@ -1,15 +1,15 @@
-// spconv_tc3.cu -- sparse convolution forward with fp32-LEVEL accuracy on the tensor cores ("3xTF32" split), sm_100a.
+// spconv_tc3.cu -- sparse convolution forward with fp32-LEVEL accuracy on the tensor cores ("3xTF32" split), sm_90a.
 //
 // spconv keeps TF32 off by default, so the reference arithmetic of SubMConv3d / SparseConv3d is fp32 FMA (SURVEY A.4).
 // A single TF32 pass (spconv_tc.cu) has a 2^-11 input rounding; here every fp32 operand is split into two TF32 pieces,
-// x = x_hi + x_lo (x_hi = RN_tf32(x), x_lo = x - x_hi exactly), and the product is accumulated in fp32 TMEM as
+// x = x_hi + x_lo (x_hi = RN_tf32(x), x_lo = x - x_hi exactly), and the product is accumulated in fp32 registers as
 //     A_hi*W_hi + A_lo*W_hi + A_hi*W_lo            (the dropped A_lo*W_lo term is ~2^-22 relative)
 // which reproduces fp32 FMA results to ~1e-6 relative (tests: <= 1e-5, the bar for the fp32-exact mode, SURVEY §8c) while
-// the math runs on tcgen05.  Three MMAs per k-step instead of one is free here: the kernel is bound by the gather, not by
-// the tensor pipe (profiles/r01_spconv_trace.txt).
+// the math runs on wgmma.  Three MMAs per k-step instead of one: the kernel is bound by the gather rather than by the
+// tensor pipe.
 //
 // Structure = spconv_tc.cu (128-row tile, (offset,channel) reduction in 128-byte blocks, one producer warp per stage,
-// one MMA-issuing thread, TMEM epilogue) except that the gather goes through registers: LDG.128 -> split -> two
+// two consumer warpgroups, epilogue from the staged accumulators) except that the gather goes through registers: LDG.128 -> split -> two
 // swizzled STS.128 (A_hi tile, A_lo tile); the weights are pre-split on the host and arrive by TMA.
 #include "common.cuh"
 #include "tc.cuh"
@@ -23,10 +23,11 @@ struct S3Cfg {
     static constexpr int W_BYTES = COUT * 128;
     static constexpr int STAGE_BYTES = 2 * S3_A_BYTES + 2 * W_BYTES;
     static constexpr int STAGES = 3;
-    static constexpr int THREADS = 32 * (STAGES + 1) < 160 ? 160 : 32 * (STAGES + 1);   // >= 4 warps for the epilogue + MMA warp
-    static constexpr int MMA_WARP = THREADS / 32 - 1;
+    static constexpr int CONSUMERS = 8;                          // two consumer warpgroups (64 rows each); warps 0-3 run the epilogue
+    static constexpr int THREADS = 32 * (CONSUMERS + STAGES);    // warp CONSUMERS + s fills stage s
+    static constexpr int ACC_LD = COUT + 4;
     static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 + S3_KMAX * S3_ROWS * 4 + 128 * 4 + 256;
-    static constexpr int TMEM_COLS = COUT < 32 ? 32 : COUT;
+    static_assert(S3_ROWS * ACC_LD * 4 <= STAGES * STAGE_BYTES, "accumulator staging must fit in the pipeline buffers");
 };
 
 template <int CIN_PAD, int COUT>
@@ -47,9 +48,7 @@ k_spconv_3xtf32(const __grid_constant__ CUtensorMap tmWhi, const __grid_constant
     int* s_blocks = s_nbr + S3_KMAX * S3_ROWS;
     uint64_t* full = reinterpret_cast<uint64_t*>(s_blocks + 124);
     uint64_t* empty = full + Cfg::STAGES;
-    uint64_t* tmem_full = empty + Cfg::STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);
-    int* s_nb = reinterpret_cast<int*>(tmem_slot + 1);
+    int* s_nb = reinterpret_cast<int*>(empty + Cfg::STAGES);
     unsigned* s_mask = reinterpret_cast<unsigned*>(s_nb + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -58,12 +57,10 @@ k_spconv_3xtf32(const __grid_constant__ CUtensorMap tmWhi, const __grid_constant
     if (threadIdx.x == 0) {
         tc::prefetch_tmap(&tmWhi);
         tc::prefetch_tmap(&tmWlo);
-        for (int s = 0; s < Cfg::STAGES; ++s) { tc::mbar_init(full + s, 32 + 1); tc::mbar_init(empty + s, 1); }
-        tc::mbar_init(tmem_full, 1);
+        for (int s = 0; s < Cfg::STAGES; ++s) { tc::mbar_init(full + s, 32 + 1); tc::mbar_init(empty + s, Cfg::CONSUMERS); }
         tc::fence_barrier_init();
         *s_mask = 0u;
     }
-    if (warp == Cfg::MMA_WARP) tc::tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
     __syncthreads();
     if (warp < 4) {
         const int r = row0 + threadIdx.x;
@@ -90,9 +87,7 @@ k_spconv_3xtf32(const __grid_constant__ CUtensorMap tmWhi, const __grid_constant
         mine = __reduce_or_sync(0xffffffffu, mine);
         if (lane == 0 && mine) atomicOr(s_mask, mine);
     }
-    tc::tcgen05_fence_before();
     __syncthreads();
-    tc::tcgen05_fence_after();
     if (threadIdx.x == 0) {
         const unsigned mask = *s_mask;
         int nb = 0;
@@ -106,15 +101,14 @@ k_spconv_3xtf32(const __grid_constant__ CUtensorMap tmWhi, const __grid_constant
     }
     __syncthreads();
     const int nb = *s_nb;
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp < Cfg::STAGES) {
+    if (warp >= Cfg::CONSUMERS) {
         // ================= producers: warp w fills stage w (A_hi, A_lo through registers; W_hi, W_lo by TMA) ==========
         const int j = lane & 7, rg = lane >> 3;         // lane covers chunk j of rows rg*32 .. rg*32+31
-        const int s = warp;
+        const int s = warp - Cfg::CONSUMERS;
         unsigned char* sa = smem + s * Cfg::STAGE_BYTES;
         unsigned char* sa_lo = sa + S3_A_BYTES;
-        for (int it = warp, round = 0; it < nb; it += Cfg::STAGES, ++round) {
+        for (int it = s, round = 0; it < nb; it += Cfg::STAGES, ++round) {
             const int kb = s_blocks[it];
             tc::mbar_wait(empty + s, (round & 1) ^ 1);
             if (lane == 0) {
@@ -162,61 +156,68 @@ k_spconv_3xtf32(const __grid_constant__ CUtensorMap tmWhi, const __grid_constant
             tc::fence_proxy_async();                  // generic-proxy smem writes -> visible to the tensor core (async proxy)
             tc::mbar_arrive(full + s);
         }
-    }
-    if (warp < 4) {
-        // ================= epilogue =================
-        const int q = warp;
-        const int pos = row0 + q * 32 + lane;       // tile position; the output row is order[pos] under a tile schedule
-        const int r = pos < n ? (order ? __ldg(order + pos) : pos) : n;
-        tc::mbar_wait(tmem_full, 0);
-        tc::tcgen05_fence_after();
+    } else {
+        // ================= consumers: warpgroup g accumulates rows [64g, 64g+64) of the tile =================
+        const int g = warp >> 2;
+        float acc[COUT / 2];
+#pragma unroll
+        for (int i = 0; i < COUT / 2; ++i) acc[i] = 0.f;
+        for (int it = 0; it < nb; ++it) {
+            const int s = it % Cfg::STAGES;
+            tc::mbar_wait(full + s, (it / Cfg::STAGES) & 1);
+            const uint32_t sa = tc::smem_u32(smem + s * Cfg::STAGE_BYTES) + g * 64 * 128;
+            const uint32_t sw = tc::smem_u32(smem + s * Cfg::STAGE_BYTES) + 2 * S3_A_BYTES;
+            const uint64_t a_hi = tc::smem_desc_sw128(sa), a_lo = tc::smem_desc_sw128(sa + S3_A_BYTES);
+            const uint64_t w_hi = tc::smem_desc_sw128(sw), w_lo = tc::smem_desc_sw128(sw + Cfg::W_BYTES);
+            tc::wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+                const uint64_t o = (uint64_t)(kk * 2);
+                tc::wgmma<COUT, tc::K_TF32>(acc, a_lo + o, w_hi + o, 1u);      // small terms first
+                tc::wgmma<COUT, tc::K_TF32>(acc, a_hi + o, w_lo + o, 1u);
+                tc::wgmma<COUT, tc::K_TF32>(acc, a_hi + o, w_hi + o, 1u);
+            }
+            tc::wgmma_commit();
+            tc::wgmma_wait_one();                       // this step's MMAs stay in flight; the previous step's stage is free
+            __syncwarp();
+            if (lane == 0 && it > 0) tc::mbar_arrive(empty + (it - 1) % Cfg::STAGES);
+        }
+        tc::wgmma_wait_all();
+        __syncwarp();
+        if (lane == 0 && nb > 0) tc::mbar_arrive(empty + (nb - 1) % Cfg::STAGES);
+        // every stage has been consumed: the pipeline buffers hold the accumulator tile for the epilogue
+        float* stg = reinterpret_cast<float*>(smem);
+        tc::named_sync(1, 32 * Cfg::CONSUMERS);
+        tc::acc_to_smem<COUT>(acc, stg, Cfg::ACC_LD, g * 64);
+        tc::named_sync(1, 32 * Cfg::CONSUMERS);
+        if (warp < 4) {
+            // ================= epilogue: thread = tile row =================
+            const int pos = row0 + threadIdx.x;     // tile position; the output row is order[pos] under a tile schedule
+            const int r = pos < n ? (order ? __ldg(order + pos) : pos) : n;
 #pragma unroll 1
-        for (int c0 = 0; c0 < COUT; c0 += 32) {
-            float v[32];
-            tc::tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0, v);
-            if (r < n) {
+            for (int c0 = 0; c0 < COUT; c0 += 32) {
+                float v[32];
+                if (c0 + 32 <= COUT) tc::smem_row32(stg, Cfg::ACC_LD, threadIdx.x, c0, v);
+                else { for (int i = 0; i < 16; ++i) v[i] = stg[threadIdx.x * Cfg::ACC_LD + c0 + i]; }
+                if (r < n) {
 #pragma unroll
-                for (int jj = 0; jj < 32; jj += 4) {
-                    const int ch = c0 + jj;
-                    if (ch >= COUT) break;
-                    float4 o = nb > 0 ? make_float4(v[jj], v[jj + 1], v[jj + 2], v[jj + 3]) : make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (scale) { float4 sc = __ldg(reinterpret_cast<const float4*>(scale + ch)); o.x *= sc.x; o.y *= sc.y; o.z *= sc.z; o.w *= sc.w; }
-                    if (shift) { float4 sh = __ldg(reinterpret_cast<const float4*>(shift + ch)); o.x += sh.x; o.y += sh.y; o.z += sh.z; o.w += sh.w; }
-                    if (residual) {
-                        float4 rr = __ldg(reinterpret_cast<const float4*>(residual + (size_t)r * COUT + ch));
-                        o.x += rr.x; o.y += rr.y; o.z += rr.z; o.w += rr.w;
+                    for (int jj = 0; jj < 32; jj += 4) {
+                        const int ch = c0 + jj;
+                        if (ch >= COUT) break;
+                        float4 o = nb > 0 ? make_float4(v[jj], v[jj + 1], v[jj + 2], v[jj + 3]) : make_float4(0.f, 0.f, 0.f, 0.f);
+                        if (scale) { float4 sc = __ldg(reinterpret_cast<const float4*>(scale + ch)); o.x *= sc.x; o.y *= sc.y; o.z *= sc.z; o.w *= sc.w; }
+                        if (shift) { float4 sh = __ldg(reinterpret_cast<const float4*>(shift + ch)); o.x += sh.x; o.y += sh.y; o.z += sh.z; o.w += sh.w; }
+                        if (residual) {
+                            float4 rr = __ldg(reinterpret_cast<const float4*>(residual + (size_t)r * COUT + ch));
+                            o.x += rr.x; o.y += rr.y; o.z += rr.z; o.w += rr.w;
+                        }
+                        if (relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
+                        *reinterpret_cast<float4*>(out + (size_t)r * COUT + ch) = o;
                     }
-                    if (relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-                    *reinterpret_cast<float4*>(out + (size_t)r * COUT + ch) = o;
                 }
             }
         }
     }
-    if (warp == Cfg::MMA_WARP) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = tc::instr_desc(2, 128, COUT);
-            for (int it = 0; it < nb; ++it) {
-                const int s = it % Cfg::STAGES;
-                tc::mbar_wait(full + s, (it / Cfg::STAGES) & 1);
-                tc::tcgen05_fence_after();
-                const uint32_t sa = tc::smem_u32(smem + s * Cfg::STAGE_BYTES);
-                const uint64_t a_hi = tc::smem_desc_sw128(sa), a_lo = tc::smem_desc_sw128(sa + S3_A_BYTES);
-                const uint64_t w_hi = tc::smem_desc_sw128(sa + 2 * S3_A_BYTES), w_lo = tc::smem_desc_sw128(sa + 2 * S3_A_BYTES + Cfg::W_BYTES);
-#pragma unroll
-                for (int kk = 0; kk < 4; ++kk) {
-                    const uint64_t o = (uint64_t)(kk * 2);
-                    tc::mma_tf32(tmem_base, a_lo + o, w_hi + o, idesc, (it | kk) ? 1u : 0u);      // small terms first
-                    tc::mma_tf32(tmem_base, a_hi + o, w_lo + o, idesc, 1u);
-                    tc::mma_tf32(tmem_base, a_hi + o, w_hi + o, idesc, 1u);
-                }
-                tc::mma_commit(empty + s);
-            }
-            tc::mma_commit(tmem_full);
-        }
-    }
-    tc::tcgen05_fence_before();
-    __syncthreads();
-    if (warp == Cfg::MMA_WARP) tc::tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
 }
 
 template <int CIN_PAD, int COUT>

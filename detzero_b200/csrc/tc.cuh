@@ -1,6 +1,6 @@
-// tc.cuh -- Blackwell (sm_100a) primitives used by the tensor-core kernels: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (alloc / mma / commit / ld) and UMMA descriptor construction.  Inline PTX only; no CUTLASS dependency.
-// Descriptor bit layouts follow cute/arch/mma_sm100_desc.hpp (SmemDescriptor, InstrDescriptor).
+// tc.cuh -- Hopper (sm_90a) primitives used by the tensor-core kernels: mbarrier, TMA (cp.async.bulk.tensor), wgmma
+// and its shared-memory matrix descriptors.  Inline PTX only; no CUTLASS dependency.
+// The descriptor layout is the one of the PTX ISA "Matrix Descriptor Format" for wgmma.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -68,61 +68,112 @@ __device__ __forceinline__ void tma_store_5d(const CUtensorMap* m, const void* s
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 
-// gather4: four rows (given by index) of a 2-D tensor, box = {cols, 1}; lands as 4 consecutive box-rows at smem_dst.
-// Row indices outside the tensor are zero-filled.
-__device__ __forceinline__ void tma_gather4(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int col, int r0, int r1, int r2, int r3) {
+// ---- wgmma (warpgroup MMA) ---------------------------------------------------------------------------------------
+// D[64 x N] (+)= A[64 x K] * B[N x K]^T for one warpgroup (128 threads, warps 4g .. 4g+3), A and B K-major in shared memory,
+// fp32 accumulator in registers.  Fragment: thread t (warp w = t/32 of the warpgroup, lane l) holds d[4j + 2r + c] =
+// D[16w + l/4 + 8r][8j + 2(l%4) + c].
+enum MmaKind { K_TF32, K_BF16 };
+template <int N, MmaKind KIND>
+__device__ __forceinline__ void wgmma(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t acc);
+template <> __device__ __forceinline__ void wgmma<16, K_TF32>(float (&d)[8], uint64_t a, uint64_t b, uint32_t acc) {
     asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.tile::gather4.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(col), "r"(r0), "r"(r1), "r"(r2), "r"(r3)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<32, K_TF32>(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<64, K_TF32>(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<128, K_TF32>(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<16, K_BF16>(float (&d)[8], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<32, K_BF16>(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<64, K_BF16>(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b), "r"(acc));
+}
+template <> __device__ __forceinline__ void wgmma<128, K_BF16>(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a), "l"(b), "r"(acc));
 }
 
-// ---- tcgen05 ------------------------------------------------------------------------------------------------------
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {      // one full warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "n"(NCOLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {        // same warp that allocated
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// all but the most recently committed group have completed (keeps one k-step of MMAs in flight while the next is issued)
+__device__ __forceinline__ void wgmma_wait_one() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem] * B[smem]^T ; kind::tf32 (fp32 containers) or kind::f16 (bf16/f16)
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrive on an mbarrier when all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
+// named barrier over `threads` threads (ids 1..15; 0 is __syncthreads)
+__device__ __forceinline__ void named_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
-// 32 lanes x 32 consecutive fp32 columns: thread t of the warp gets lane (base_lane + t), columns [col, col+32)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// accumulator fragment of warpgroup-local rows [0, 64) -> shared memory rows [row0, row0 + 64) of a row-major fp32 tile
+// with leading dimension ld (even)
+template <int N>
+__device__ __forceinline__ void acc_to_smem(const float (&d)[N / 2], float* tile, int ld, int row0) {
+    const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
 #pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+    for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+            *reinterpret_cast<float2*>(tile + (size_t)(row0 + 16 * w + (l >> 2) + 8 * r) * ld + 8 * j + 2 * (l & 3)) =
+                make_float2(d[4 * j + 2 * r], d[4 * j + 2 * r + 1]);
+}
+// columns [c0, c0 + ncols) of the same fragment (c0, ncols multiples of 8) -> tile columns [0, ncols)
+template <int N>
+__device__ __forceinline__ void acc_cols_to_smem(const float (&d)[N / 2], float* tile, int ld, int row0, int c0, int ncols) {
+    const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+        if (8 * j < c0 || 8 * j >= c0 + ncols) continue;
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+            *reinterpret_cast<float2*>(tile + (size_t)(row0 + 16 * w + (l >> 2) + 8 * r) * ld + 8 * j - c0 + 2 * (l & 3)) =
+                make_float2(d[4 * j + 2 * r], d[4 * j + 2 * r + 1]);
+    }
+}
+// 32 consecutive fp32 columns of one row of such a tile (16-byte aligned: ld % 4 == 0, c0 % 4 == 0)
+__device__ __forceinline__ void smem_row32(const float* tile, int ld, int row, int c0, float (&v)[32]) {
+    const float4* p = reinterpret_cast<const float4*>(tile + (size_t)row * ld + c0);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        const float4 x = p[i];
+        v[4 * i] = x.x; v[4 * i + 1] = x.y; v[4 * i + 2] = x.z; v[4 * i + 3] = x.w;
+    }
 }
 
 __device__ __forceinline__ float rna_tf32(float x) {
@@ -132,29 +183,15 @@ __device__ __forceinline__ float rna_tf32(float x) {
 }
 
 // ---- descriptors ------------------------------------------------------------------------------------------------
-// K-major operand tile, 128-byte swizzle: rows of 128 B, 8-row groups 1024 B apart (tile base 1024 B aligned).
-__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t smem_addr) {
+// K-major operand tile, 128-byte swizzle: rows of 128 B, 8-row groups `sbo` bytes apart (1024 for a dense tile, base 1024 B
+// aligned).  Advancing the start address by 32 B steps through the K dimension inside the swizzle atom.
+__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t smem_addr, uint32_t sbo = 1024) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);           // start address
-    d |= (uint64_t)1 << 16;                                // leading byte offset (unused for swizzled K-major) = 16 B
-    d |= (uint64_t)(1024 >> 4) << 32;                      // stride byte offset between 8-row groups
-    d |= (uint64_t)1 << 46;                                // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                                // SWIZZLE_128B
+    d |= (uint64_t)1 << 16;                                // leading byte offset (unused for swizzled K-major)
+    d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;            // stride byte offset between 8-row groups
+    d |= (uint64_t)1 << 62;                                // SWIZZLE_128B
     return d;
-}
-// K-major operand tile with 64-byte rows (16 fp32), 64-byte swizzle: 8-row groups 512 B apart
-__device__ __forceinline__ uint64_t smem_desc_sw64(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(512 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)4 << 61;                                // SWIZZLE_64B
-    return d;
-}
-// instruction descriptor: fp32 accumulate, A and B K-major.  fmt: 0 = f16, 1 = bf16, 2 = tf32
-__host__ __device__ constexpr uint32_t instr_desc(int fmt, int M, int N) {
-    return (1u << 4) | ((uint32_t)fmt << 7) | ((uint32_t)fmt << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
 }
 
 // host: cuTensorMapEncodeTiled through the runtime (no link-time libcuda dependency)

@@ -1,4 +1,4 @@
-// track.cu -- the steps either side of the detector / refiner kernels (SURVEY.md §8f rows 2 and 3), sm_100a:
+// track.cu -- the steps either side of the detector / refiner kernels (SURVEY.md §8f rows 2 and 3), sm_90a:
 //
 //   * tracker association matrices on the device, reading boxes straight from the all-gathered (F, 500, 9) tensor:
 //     rotated-BEV IoU, BEV overlap area, 3-D IoU and axis-aligned 2-D IoU.  Replaces

@@ -1,10 +1,10 @@
-// voxelize.cu -- grid-index scan, hard voxelization (+MeanVFE) and dynamic mean voxelization for sm_100a.
+// voxelize.cu -- grid-index scan, hard voxelization (+MeanVFE) and dynamic mean voxelization for sm_90a.
 //
 // Replaces spconv.utils.Point2VoxelCPU3d.point_to_voxel as driven by
 // detection/detzero_det/datasets/processor/data_processor.py:61-91, MeanVFE.forward (vfe.py:66-83) and
 // DynamicMeanVFE.forward (vfe.py:110-147).
 //
-// Design (B200-first, not the CPU algorithm): instead of a sequential dense-grid walk, cells are deduplicated with
+// Design (GPU-first, not the CPU algorithm): instead of a sequential dense-grid walk, cells are deduplicated with
 // an L2-resident occupancy BITMAP (1 bit/cell, 11.6 MB for the 41x1504x1504 Waymo lattice) that is turned into a
 // rank structure by a popcount prefix scan.  "First appearance" order is recovered with atomicMin(first point id)
 // per occupied cell + an exclusive scan of leader flags in point order; the first max_pts points of every voxel

@@ -1,5 +1,5 @@
 """VoxelBackBone8x / VoxelResBackBone8x with the reference's module tree (=> identical state-dict keys), ctor kwargs
-and batch_dict contract (detection/detzero_det/models/centerpoint_modules/backbone3d.py:64-338), on the sm_100a
+and batch_dict contract (detection/detzero_det/models/centerpoint_modules/backbone3d.py:64-338), on the sm_90a
 sparse-conv kernels.  In eval mode every conv + BatchNorm1d + (bias) + (residual) + ReLU group is ONE launch."""
 from functools import partial
 

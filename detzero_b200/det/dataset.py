@@ -2,7 +2,7 @@
 (detection/detzero_det/datasets/processor/data_processor.py:10-138, point_feature_encoder.py:4-57,
 dataset.py:260-303) plus a synthetic Waymo-shape cloud source (there is no Waymo data or network here).
 
-On the B200 path voxelization is NOT done in DataLoader workers: ``transform_points_to_voxels`` only records the
+In this package voxelization is NOT done in DataLoader workers: ``transform_points_to_voxels`` only records the
 grid (like the reference's ``..._placeholder`` step, data_processor.py:51-59) and the raw points go to the device,
 where MeanVFE voxelizes them."""
 from functools import partial

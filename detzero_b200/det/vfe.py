@@ -1,7 +1,7 @@
 """Voxel feature encoders with the reference's names / ctor kwargs / batch_dict contract
 (detection/detzero_det/models/centerpoint_modules/vfe.py:58-147), running on libdetzero_b200.
 
-B200 ownership (SURVEY.md §8b): when the batch carries raw ``points`` (b,x,y,z,...) but no ``voxels`` (i.e. the data
+GPU ownership (SURVEY.md §8b): when the batch carries raw ``points`` (b,x,y,z,...) but no ``voxels`` (i.e. the data
 processor used ``transform_points_to_voxels_placeholder``), ``MeanVFE`` runs the order-exact hard voxelizer on the
 device, fused with the mean, and hands the level-0 grid index to the 3D backbone -- no CPU voxelization, no H2D of
 8 MB of voxels, no host sync."""

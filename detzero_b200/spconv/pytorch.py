@@ -1,4 +1,4 @@
-"""``spconv.pytorch``-shaped API on top of libdetzero_b200 (sm_100a).
+"""``spconv.pytorch``-shaped API on top of libdetzero_b200 (sm_90a).
 
 Mirrors exactly the surface the reference touches (SURVEY.md §8b): ``SparseConvTensor(features=, indices=,
 spatial_shape=, batch_size=)`` with ``.features .indices .spatial_shape .batch_size .indice_dict
@@ -7,7 +7,7 @@ with spconv-2.x weight layout ``(Cout, KD, KH, KW, Cin)`` (state-dict compatible
 ``SparseSequential``; ``SparseModule``; ``SparseInverseConv3d`` (never constructed by the shipped configs).
 Reference call sites: detection/detzero_det/models/centerpoint_modules/backbone3d.py:68-73,93-100,135-195.
 
-B200-native differences (behaviour-preserving):
+Differences from spconv (behaviour-preserving):
   * tensors carry a *capacity* and a device-side row count, so a whole backbone runs without a host sync;
     ``.features`` / ``.indices`` slice to the true row count lazily (one D2H only if the caller asks)
   * the rulebook is a neighbour table built from an L2-resident grid index (no hash table, no sort);
@@ -219,7 +219,7 @@ class _SparseConv(SparseModule):
     #: build a tile schedule (rows grouped by neighbour mask) with every rulebook used by a tensor-core layer
     SCHEDULE_TILES = True
     #: batches: sort the schedule by (frame, mask) so that the tiles in flight gather from ONE frame's (L2-resident) feature map
-    FRAME_MAJOR = bool(os.environ.get('DZ_FRAME_MAJOR'))      # measured (profiles/r02_spconv_notes.md): the 3 digest bits it costs outweigh the L2 gain
+    FRAME_MAJOR = bool(os.environ.get('DZ_FRAME_MAJOR'))      # the 3 digest bits it costs outweigh the L2 gain
 
     def __init__(self, in_channels, out_channels, kernel_size, stride=1, padding=0, dilation=1, groups=1, bias=True,
                  indice_key=None, subm=False, algo=None, mode='fp32'):

@@ -1,7 +1,7 @@
 """GPU voxel generator with the constructor / call surface of ``spconv.utils.Point2VoxelCPU3d`` as used at
 detection/detzero_det/datasets/processor/data_processor.py:70-83.
 
-The reference creates the CPU generator lazily inside each DataLoader worker; the B200 path instead keeps raw points
+The reference creates the CPU generator lazily inside each DataLoader worker; this package instead keeps raw points
 on the device (``transform_points_to_voxels_placeholder``, data_processor.py:51-59) and voxelizes in the main process
 (SURVEY.md §8b "Ownership / threading").  Results are order-exact with the CPU generator (first-appearance voxel
 ids, first ``max_num_points_per_voxel`` points per voxel in input order, voxel cap in appearance order)."""
@@ -72,5 +72,5 @@ class Point2VoxelGPU3d:
         return r['voxels'][:m], r['coords'][:m, 1:4].contiguous(), r['num'][:m]
 
 
-# the reference imports this name (data_processor.py:6); on the B200 path it resolves to the GPU generator
+# the reference imports this name (data_processor.py:6); here it resolves to the GPU generator
 Point2VoxelCPU3d = Point2VoxelGPU3d

@@ -1,5 +1,5 @@
 /*
- * detzero_b200.h -- C ABI of libdetzero_b200.so (sm_100a).
+ * detzero_b200.h -- C ABI of libdetzero_b200.so (sm_90a).
  *
  * The reference (PJLab-ADG/DetZero) has no C ABI: its native ops are pybind11 modules taking at::Tensor
  * (utils/detzero_utils/ops/iou3d_nms/src/iou3d_nms_api.cpp:10-17) and its sparse-conv / voxelizer arithmetic
@@ -29,12 +29,12 @@ typedef void* dz_stream_t;           /* cudaStream_t */
 
 enum { DZ_OK = 0, DZ_ERR_ARG = -1, DZ_ERR_CUDA = -2, DZ_ERR_WORKSPACE = -3, DZ_ERR_UNSUPPORTED = -4 };
 enum { DZ_F32 = 0, DZ_TF32 = 1, DZ_BF16 = 2, DZ_TF32X3 = 3, DZ_BF16X2 = 4 };   /* arithmetic mode of GEMM-shaped kernels:
-   F32 = fp32 FMA; TF32 = one tcgen05 TF32 pass; TF32X3 = hi/lo split, 3 TF32 passes, fp32-level accuracy (sparse conv);
+   F32 = fp32 FMA; TF32 = one wgmma TF32 pass; TF32X3 = hi/lo split, 3 TF32 passes, fp32-level accuracy (sparse conv);
    BF16 / BF16X2 = bf16 operand planes (1 plane: bf16 storage; 2 planes: x = p0 + p1, 16 significand bits in 4 bytes,
    fp32-level accuracy at the cost of one TF32 pass), sparse conv only: dz_spconv_fwd_planes */
 
 int         dz_version(void);
-int         dz_sm_arch(void);                      /* 100 : built for sm_100a */
+int         dz_sm_arch(void);                      /* 90 : built for sm_90a */
 const char* dz_last_error_string(void);            /* host string, thread-local */
 
 /* ---- grid index ---------------------------------------------------------------------------------------- */
@@ -138,7 +138,7 @@ int dz_rulebook_schedule(const int32_t* tab, int cap, const int* d_n, int32_t* o
  * Replaces SubMConv3d/SparseConv3d forward + BatchNorm1d(eval) + bias + residual add + ReLU
  * (backbone3d.py:64-83,105-121).  weight packed (K, cin, cout) f32 (host side repacks spconv's
  * (cout,KD,KH,KW,cin) layout, SURVEY A.3; DZ_TF32 expects (cout, K*cin_pad)).  in_rows = allocated rows of `in`
- * (bounds the TMA gather).  mode: DZ_F32 exact-fp32 FMA (nbr = k-major table), DZ_TF32 / DZ_TF32X3 tcgen05 tensor
+ * (bounds the TMA gather).  mode: DZ_F32 exact-fp32 FMA (nbr = k-major table), DZ_TF32 / DZ_TF32X3 wgmma tensor
  * cores (nbr = ROW-major table `tab`, nbr_cap = its rows).
  * row_order: NULL, or the tile schedule of dz_rulebook_schedule (tensor-core modes only). */
 int dz_spconv_fwd(const float* in, int cin, int in_rows, const int32_t* nbr, int K, int nbr_cap,
@@ -156,7 +156,7 @@ int dz_spconv_wgrad(const float* in, int cin, const int32_t* nbr, int K, int nbr
                     const float* dout, int cout, float* dW, dz_stream_t stream);
 
 /* The same layer on bf16 operand PLANES (modes DZ_BF16: planes = 1, DZ_BF16X2: planes = 2), csrc/spconv_bf16.cu: a persistent
- * warp-specialised tcgen05 kernel.  Feature tensors `in`, `residual`, `out` are (rows, planes * C) bf16, a row = [p0 | p1] with
+ * warp-specialised wgmma kernel.  Feature tensors `in`, `residual`, `out` are (rows, planes * C) bf16, a row = [p0 | p1] with
  * x ~ p0 (+ p1), p0 = RN_bf16(x), p1 = RN_bf16(x - p0); cin <= 8 is stored padded to 8 channels per plane.  weight: (planes * cout,
  * K * cin_pad) bf16, rows [w0 ; w1] split the same way.  tab = ROW-major table, row_order = NULL or the tile schedule,
  * tab_tiles = NULL or the tile-major table dz_rulebook_schedule wrote next to row_order (fast path).

@@ -1,5 +1,5 @@
 """GPU parity tests for the detector hot path: every kernel of libdetzero_b200 against the CPU oracle on the same
-seeded inputs (SURVEY.md §8c parity definitions).  Run on the B200 box: pytest -m gpu."""
+seeded inputs (SURVEY.md §8c parity definitions).  Run on an H100: pytest -m gpu."""
 import numpy as np
 import pytest
 import torch
@@ -139,7 +139,7 @@ def test_spconv_fwd_fp32(cuda, cin, cout):
         out = ops.spconv_fwd(t._feat, nbr, t._count, n, wp, scale.to(cuda), shift.to(cuda), res.to(cuda), True, mode,
                              kshape=(27, cin, cout))
         assert util.rel_err(out.cpu(), ref) < tol, mode
-    # bf16 operand planes (persistent tcgen05 kernel): 2 planes = fp32-level, 1 plane = bf16 storage
+    # bf16 operand planes (persistent wgmma kernel): 2 planes = fp32-level, 1 plane = bf16 storage
     tab = ops.table_to_rows(nbr)
     cin_pad = 8 if cin <= 8 else cin
     for mode, tol in ((_lib.DZ_BF16X2, 2e-5), (_lib.DZ_BF16, 1e-2)):
@@ -302,7 +302,7 @@ def test_conv2d_fp32(cuda, cin, cout, k, stride, pad, H, W):
 
 @pytest.mark.parametrize('cin,cout,H,W,coff,cstride', [(128, 128, 136, 184, 0, 128), (64, 64, 152, 168, 32, 160), (256, 256, 94, 94, 0, 256)])
 def test_conv2d_tf32_many_tiles(cuda, cin, cout, H, W, coff, cstride):
-    """enough 8x16 patches (>= 148 per cout slice) for the two-CTAs-per-SM single-patch configuration of the tensor-core conv,
+    """many 8x16 patches (more than one per SM and cout slice) through the tensor-core conv,
     ragged edges (H, W not multiples of the patch), output written at a channel offset of a wider (concat) tensor through the
     TMA-store epilogue -- the neighbouring channels must stay untouched"""
     from detzero_b200 import ops
@@ -530,7 +530,7 @@ def test_dynamic_vfe_into_backbone(cuda):
         return [k for k, ok in checks.items() if not ok]
 
     # round 1 saw an intermittent failure here: id()-keyed global caches of folded BN / packed weights handed a freed model's
-    # tensors to the next model (ADVICE.md); the caches now live on the modules.  No retry, no xfail.
+    # tensors to the next model; the caches now live on the modules.  No retry, no xfail.
     failed = attempt()
     assert not failed, failed
 
@@ -672,14 +672,14 @@ def test_frame_major_schedule(cuda):
 @pytest.mark.parametrize('cin,cout,k,stride,pad,H,W,B,coff,cstride', [(128, 128, 3, 1, 1, 188, 188, 2, 0, 128), (256, 256, 3, 1, 1, 94, 94, 8, 0, 256),
                                                                       (128, 256, 3, 2, 1, 187, 189, 4, 0, 256), (256, 128, 3, 1, 1, 100, 84, 4, 64, 256),
                                                                       (128, 256, 1, 1, 0, 150, 150, 2, 256, 512),
-                                                                      # 3x3 stride-1 -> the halo kernel at every tile width: 64 (shared conv), 32 with a
-                                                                      # ragged Cout (fused head stage 2), 3 x 128 (fused head stage 1), ragged image edges
+                                                                      # 3x3 stride-1 at every tile width: 64 (shared conv), 32 with a ragged Cout
+                                                                      # (fused head stage 2), 3 x 128 (fused head stage 1), ragged image edges
                                                                       (512, 64, 3, 1, 1, 188, 188, 2, 0, 64), (384, 12, 3, 1, 1, 100, 90, 4, 0, 12),
                                                                       (64, 384, 3, 1, 1, 95, 93, 4, 0, 384), (128, 128, 3, 1, 1, 61, 67, 8, 128, 384)])
 def test_conv2d_tf32_cta_pair_kernel(cuda, cin, cout, k, stride, pad, H, W, B, coff, cstride):
-    """enough tiles for the CTA-pair kernel (tcgen05 cta_group::2: two M tiles share one weight tile, each CTA loads half of its rows;
-    BN = 256 for Cout = 256) and, for 3x3 stride-1 shapes, the HALO kernel (one (16+2) x (8+2) activation tile per 32-channel slice, nine
-    shifted UMMA descriptors): odd tile counts (duplicate tail tile), ragged edges, stride 2, channel-offset (concat) output"""
+    """the BEV-backbone and head shapes at batch sizes that give several tiles per SM: Cout = 256 (two 128-wide weight tiles per
+    patch), odd tile counts, ragged edges, stride 2, 1x1, channel-offset (concat) output; the 3x3 stride-1 shapes run through the
+    HALO variant (one (16+2) x (8+2) activation tile per 32-channel slice, nine shifted wgmma descriptors) at every tile width"""
     from detzero_b200 import ops
     g = torch.Generator().manual_seed(13)
     x = torch.randn(B, cin, H, W, generator=g)

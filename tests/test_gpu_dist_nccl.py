@@ -61,7 +61,7 @@ def _free_port():
 def test_sequence_gather_nccl_world2(cuda, tmp_path):
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip('needs 2 GPUs (gpurun --gpus 2)')
+        pytest.skip('needs 2 GPUs')
     w = tmp_path / 'worker.py'
     w.write_text(WORKER)
     port, num_frames, out = _free_port(), 7, str(tmp_path / 'out.json')

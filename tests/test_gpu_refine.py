@@ -86,7 +86,7 @@ def test_prm_vs_reference_golden(cuda, mode, tol):
 
 @pytest.mark.parametrize('mode,tol', [('fp32', 1e-3), ('tf32', 3e-2)])
 def test_grm_vs_reference_golden(cuda, mode, tol):
-    """fp32: the exact-FMA kernels; tf32: the tcgen05 linears + attention the production configuration runs"""
+    """fp32: the exact-FMA kernels; tf32: the wgmma linears + attention the production configuration runs"""
     from detzero_b200.refine import GeometryTransformer
     cfg = ri.grm_cfg()
     cfg.COMPUTE_MODE = mode

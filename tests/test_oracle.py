@@ -170,7 +170,7 @@ def test_c_abi_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(l, name), name
     assert declared == set(_lib.exported_symbols())
-    assert l.dz_sm_arch() == 100 and l.dz_version() >= 100
+    assert l.dz_sm_arch() == 90 and l.dz_version() >= 100
 
 
 def test_product_path_fails_loudly_without_cuda():
@@ -207,21 +207,12 @@ def test_data_processor_and_collate():
 
 
 def test_rotated_iou_restatement_matches_compiled_reference():
-    """oracle/_ref = the reference's own iou3d_cpu.cpp compiled in place (oracle/build_ref.py): the C restatement of
-    the rotated-BEV IoU agrees with it bit for bit"""
-    from oracle import build_ref
-    if not os.path.exists(build_ref.SO):
-        if not os.path.exists(build_ref.REF_SRC):
-            pytest.skip('oracle/_ref not built and /root/reference not mounted')
-        build_ref.build()
-    m = build_ref.load()
-    g = np.random.default_rng(7)
-    n = 300
-    b = np.concatenate([g.uniform(-10, 10, (n, 3)), g.uniform(1, 5, (n, 3)), g.uniform(-3.2, 3.2, (n, 1))], 1).astype(np.float32)
-    b[100:200, :2] = b[:100, :2] + g.normal(0, 0.2, (100, 2)).astype(np.float32)
-    out = torch.zeros(n, n)
-    m.boxes_iou_bev_cpu(torch.from_numpy(b), torch.from_numpy(b), out)
-    assert np.array_equal(out.numpy(), oracle.boxes_iou_bev(b, b))
+    """the C restatement of the rotated-BEV IoU agrees bit for bit with the reference's own iou3d_cpu.cpp on the same seeded boxes
+    (tests/golden/iou_bev.npz, written by tests/golden/make_golden_host.py from the compiled reference source)"""
+    from tests.golden.make_golden_host import iou_boxes
+    want = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'iou_bev.npz'))['iou']
+    b = iou_boxes()
+    assert np.array_equal(want, oracle.boxes_iou_bev(b, b))
 
 
 def test_yaml_config_builds_registry_model():

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Refiner throughput (BASELINE.json configs[3] shape family): GRM / PRM / CRM tracks per second on one B200, next to the
+"""Refiner throughput (BASELINE.json configs[3] shape family): GRM / PRM / CRM tracks per second on one GPU, next to the
 same modules' CPU restatement timing is in BASELINE.md (reference PRM 1.12 s/track on 8 cores).
 
     python tools/bench_refine.py [--tracks 16] [--steps 5]

@@ -1,5 +1,5 @@
 """Clock trace of one CTA of the tensor-core sparse conv (64->64 SubM, ~35 K sites): who waits on whom in the
-producer -> tcgen05 pipeline.  usage: [DZ_SPCONV_PW=1|2] python tools/trace_spconv.py"""
+producer -> wgmma pipeline.  usage: [DZ_SPCONV_PW=1|2] python tools/trace_spconv.py"""
 import ctypes, numpy as np, torch, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from detzero_b200 import ops, _lib
