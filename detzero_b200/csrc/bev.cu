@@ -138,15 +138,13 @@ static int conv2d_f32_launch(const Conv2dParams& p, cudaStream_t st) {
 
 int dz_conv2d_fwd_tc(const Conv2dParams& p, int mode, cudaStream_t st);
 
-static int conv2d_dbg() { static int v = getenv("DZ_CONV2D_DBG") ? atoi(getenv("DZ_CONV2D_DBG")) : 0; return v; }
-
 extern "C" int dz_conv2d_fwd(const float* in, int B, int H, int W, int cin, int in_cstride, const float* weight, int KH,
                              int KW, int stride, int pad, const float* scale, const float* shift, int relu, float* out,
                              int Ho, int Wo, int cout, int out_coff, int out_cstride, int mode, dz_stream_t stream) {
     DZ_CHECK_ARG(in && weight && out && B >= 1 && cin % C2_BK == 0 && in_cstride % 4 == 0 && cout % 4 == 0);
     DZ_CHECK_ARG(Ho == (H + 2 * pad - KH) / stride + 1 && Wo == (W + 2 * pad - KW) / stride + 1);
     Conv2dParams p{in, weight, scale, shift, out, B, H, W, cin, in_cstride, KH, KW, stride, pad, Ho, Wo, cout,
-                   Ho, Wo, 1, 0, 0, out_coff, out_cstride, relu, conv2d_dbg()};
+                   Ho, Wo, 1, 0, 0, out_coff, out_cstride, relu};
     if (mode == DZ_F32) return conv2d_f32_launch(p, (cudaStream_t)stream);
     return dz_conv2d_fwd_tc(p, mode, (cudaStream_t)stream);
 }
@@ -155,11 +153,17 @@ extern "C" int dz_deconv2d_fwd(const float* in, int B, int H, int W, int cin, co
                                const float* scale, const float* shift, int relu, float* out, int cout, int out_coff,
                                int out_cstride, int mode, dz_stream_t stream) {
     DZ_CHECK_ARG(in && weight && out && s >= 1 && cin % C2_BK == 0 && cout % 4 == 0);
+    if (mode != DZ_F32) {
+        // tensor cores: one GEMM with N = s * s * cout over the input pixels (weights (dy, dx, cout, cin))
+        Conv2dParams p{in, weight, scale, shift, out, B, H, W, cin, cin, 1, 1, 1, 0, H, W, cout, H * s, W * s, s, 0, 0,
+                       out_coff, out_cstride, relu};
+        return dz_conv2d_fwd_tc(p, mode, (cudaStream_t)stream);
+    }
     for (int dy = 0; dy < s; ++dy)
         for (int dx = 0; dx < s; ++dx) {
             Conv2dParams p{in, weight + (size_t)(dy * s + dx) * cin * cout, scale, shift, out, B, H, W, cin, cin,
-                           1, 1, 1, 0, H, W, cout, H * s, W * s, s, dy, dx, out_coff, out_cstride, relu, conv2d_dbg()};
-            int rc = (mode == DZ_F32) ? conv2d_f32_launch(p, (cudaStream_t)stream) : dz_conv2d_fwd_tc(p, mode, (cudaStream_t)stream);
+                           1, 1, 1, 0, H, W, cout, H * s, W * s, s, dy, dx, out_coff, out_cstride, relu};
+            int rc = conv2d_f32_launch(p, (cudaStream_t)stream);
             if (rc) return rc;
         }
     return DZ_OK;

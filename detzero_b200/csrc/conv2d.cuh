@@ -7,8 +7,7 @@ struct Conv2dParams {
     int Ho, Wo, cout;
     int OH, OW, os, oy0, ox0;        // physical output: pixel (ho*os+oy0, wo*os+ox0) of an (OH, OW) map
     int out_coff, out_cstride, relu;
-    int dbg;                         // experiment switches (DZ_CONV2D_DBG): 1 = skip weight loads, 2 = skip activation loads (timing only)
-    int tma_store;                   // epilogue through shared memory + TMA store (tensor-core kernel, os == 1)
+    int tma_store;                   // tensor-core kernel: epilogue through shared memory + TMA stores (1: NHWC, 2: strided, os >= 2)
     const float* gshift; int gsize;  // optional per-row-group shift (linear layers only): + gshift[(row / gsize) * cout + n], row = y * W + x
     int grow0;                       // row index of pixel (0, 0) (tail calls of a linear layer)
     float* gmax; int gmax_rows;      // optional (linear layers): instead of storing y, atomically max-pool it over row groups of gmax_rows

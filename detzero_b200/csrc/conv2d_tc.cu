@@ -8,11 +8,11 @@
 // canonical K-major 128B-swizzled layout (row = pixel, 128 B = 32 fp32 channels); out-of-image pixels are
 // zero-filled by the TMA unit, which implements the conv padding (and ZeroPad2d) for free.  Weights are a 2-D TMA
 // load of W[cout][(r,s,cin)].  Two consumer warpgroups (64 pixels each) issue wgmma (M=64, N=BN, K=8) into register
-// accumulators; a ring of mbarrier-guarded stages overlaps TMA with MMA.  After the main loop the accumulators go to a
-// shared-memory tile and the same 8 warps run the epilogue (each one quarter of the pixels and half of the channels):
-// folded BatchNorm / bias / ReLU, NHWC rows written through TMA stores (optionally into a channel slice / strided pixels:
-// fused torch.cat and ConvTranspose2d with kernel == stride), or a fused max over row groups.
-#include <stdlib.h>
+// accumulators; a ring of mbarrier-guarded stages overlaps TMA with MMA.  The kernel is persistent (every resident CTA walks
+// a static list of tiles) and the producer warp loads the next tile while the consumers run the epilogue straight from
+// their accumulator registers: folded BatchNorm / bias / ReLU, NHWC rows written through TMA stores (optionally into a
+// channel slice / strided pixels: fused torch.cat and ConvTranspose2d with kernel == stride as one GEMM), or a fused max
+// over row groups.
 #include "common.cuh"
 #include "conv2d.cuh"
 #include "tc.cuh"
@@ -32,8 +32,9 @@ EncodeTiledFn get_encode_tiled() {
 
 static constexpr int CT_TH = 8, CT_TW = 16, CT_BK = 32;       // pixel patch, channels per k-step group (128 B)
 static constexpr int CT_A_BYTES = CT_TH * CT_TW * CT_BK * 4;  // 16 KB
-static constexpr int CT_CONSUMERS = 8;                        // warps 0-7: two wgmma warpgroups, then the epilogue
+static constexpr int CT_CONSUMERS = 8;                        // warps 0-7: two wgmma warpgroups, each runs its own epilogue
 static constexpr int CT_THREADS = 32 * (CT_CONSUMERS + 1);    // warp 8: TMA producer
+static constexpr int CT_BOX_BYTES = 16 * 128;                 // epilogue: one consumer warp's 16 pixels x 32 channels
 
 // HALO variant (3x3 stride-1 convolutions, 16 of the 22 dense convs of the BEV backbone + head).  The generic kernel re-reads its
 // 128-pixel activation patch from L2 once per filter tap: 9 x 16 KB per 32-channel slice.  The halo kernel loads the (16+2) x (8+2)
@@ -52,47 +53,41 @@ template <int BN, bool HALO>
 struct CtCfg {
     static constexpr int TH = HALO ? HL_TH : CT_TH, TW = HALO ? HL_TW : CT_TW;        // output patch (TH x TW = 128 pixels)
     static constexpr int B_BYTES = BN * CT_BK * 4;
-    static constexpr int ACC_LD = BN + 4;                               // row pitch of the staged accumulator tile
-    static constexpr int ACC_BYTES = CT_TH * CT_TW * ACC_LD * 4;
-    static constexpr int BUDGET = 227 * 1024 - 1024 - 256 - ACC_BYTES;  // H100: 227 KB of shared memory per block
+    // epilogue staging, separate from the pipeline buffers (those already hold the next tile's operands): 8 warps x BN/32 boxes
+    static constexpr int STG_BYTES = CT_CONSUMERS * (BN / 32) * CT_BOX_BYTES;
+    static constexpr int BUDGET = 227 * 1024 - 1024 - 256 - STG_BYTES;  // H100: 227 KB of shared memory per block
     // generic: STAGES x (A patch + B tile); halo: HL_A_STAGES halo slots + STAGES B tiles
     static constexpr int STAGE_BYTES = HALO ? B_BYTES : CT_A_BYTES + B_BYTES;
     static constexpr int A_REGION = HALO ? HL_A_STAGES * HL_A_SLOT : 0;
     static constexpr int FIT = (BUDGET - A_REGION) / STAGE_BYTES;
     static constexpr int STAGES = FIT > (HALO ? 9 : 8) ? (HALO ? 9 : 8) : FIT;
-    static constexpr int BUF = A_REGION + STAGES * STAGE_BYTES;         // pipeline buffers (epilogue staging slots afterwards)
-    static constexpr int SMEM = BUF + ACC_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+    static constexpr int BUF = A_REGION + STAGES * STAGE_BYTES;         // pipeline buffers
+    static constexpr int SMEM = BUF + STG_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 };
 
-__device__ long long g_ct_trace[64];          // DZ_CONV2D_DBG & 4: clock stamps of CTA 0 (dz_debug_conv2d_trace)
-extern "C" int dz_debug_conv2d_trace(long long* host) {
-    cudaDeviceSynchronize();
-    return cudaMemcpyFromSymbol(host, g_ct_trace, sizeof(long long) * 64) == cudaSuccess ? 0 : -1;
-}
+__device__ __forceinline__ float2 ldg2(const float* p) { return __ldg(reinterpret_cast<const float2*>(p)); }
 
+// Persistent: grid = min(tiles, resident CTAs), CTA i takes tiles i, i + grid, ... (static order; a tile's accumulation order is fixed, so
+// results do not depend on the grid).  Tile t = (pixel patch t / tiles_n, channel tile t % tiles_n): the channel tiles of one
+// patch run back to back and re-read its activations from L2.  The producer warp runs on across tile boundaries, so the next
+// tile's operands load while the consumers run the epilogue of the current one; the epilogue works straight from the wgmma
+// accumulator registers and its TMA stores drain during the next tile's main loop.
 template <int BN, bool HALO>
 __global__ void __launch_bounds__(CT_THREADS, 1)
 k_conv2d_tf32(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
-              Conv2dParams p, int tiles_x, int tiles_y) {
+              Conv2dParams p, int tiles_x, int tiles_y, int tiles_n, int tiles) {
     using Cfg = CtCfg<BN, HALO>;
     constexpr int TH = Cfg::TH, TW = Cfg::TW;
     extern __shared__ unsigned char smem_raw[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     unsigned char* smB = smem + Cfg::A_REGION;                              // halo: the B ring follows the halo slots
-    float* acc_stg = reinterpret_cast<float*>(smem + Cfg::BUF);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::BUF + Cfg::ACC_BYTES);
+    unsigned char* stg_all = smem + Cfg::BUF;
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::BUF + Cfg::STG_BYTES);
     uint64_t* empty = full + Cfg::STAGES;
     uint64_t* a_full = empty + Cfg::STAGES;                                 // halo slots
     uint64_t* a_empty = a_full + HL_A_STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const bool tr = (p.dbg & 4) && blockIdx.x == 0 && blockIdx.y == 0;
-    if (tr && threadIdx.x == 0) g_ct_trace[0] = clock64();
-    int mt = blockIdx.x;
-    const int tx0 = (mt % tiles_x) * TW; mt /= tiles_x;
-    const int ty0 = (mt % tiles_y) * TH;
-    const int b = mt / tiles_y;
-    const int n0 = blockIdx.y * BN;
     const int cchunks = p.cin / CT_BK;
     const int iters = p.KH * p.KW * cchunks;
 
@@ -105,48 +100,74 @@ k_conv2d_tf32(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         tc::fence_barrier_init();
     }
     __syncthreads();
-    if (tr && threadIdx.x == 0) g_ct_trace[1] = clock64();
 
+    // ring positions (k-steps and halo slices) run on across the tiles of this CTA, in the producer and the consumers alike
+    int bit = 0, hs = 0;
     if (warp == CT_CONSUMERS) {
-        if (HALO && lane == 0) {
-            int bit = 0;
-            for (int cc = 0; cc < cchunks; ++cc) {
-                const int a = cc % HL_A_STAGES;
-                tc::mbar_wait(a_empty + a, ((cc / HL_A_STAGES) & 1) ^ 1);
-                tc::mbar_arrive_expect_tx(a_full + a, HL_A_BYTES);
-                tc::tma_load_4d(smem + a * HL_A_SLOT, &tmA, a_full + a, cc * CT_BK, tx0 - p.pad, ty0 - p.pad, b);
-                for (int tap = 0; tap < 9; ++tap, ++bit) {
+        if (lane != 0) return;
+        for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+            const int n0 = (t % tiles_n) * BN;
+            int mt = t / tiles_n;
+            const int tx0 = (mt % tiles_x) * TW; mt /= tiles_x;
+            const int ty0 = (mt % tiles_y) * TH;
+            const int b = mt / tiles_y;
+            if (HALO) {
+                for (int cc = 0; cc < cchunks; ++cc, ++hs) {
+                    const int a = hs % HL_A_STAGES;
+                    tc::mbar_wait(a_empty + a, ((hs / HL_A_STAGES) & 1) ^ 1);
+                    tc::mbar_arrive_expect_tx(a_full + a, HL_A_BYTES);
+                    tc::tma_load_4d(smem + a * HL_A_SLOT, &tmA, a_full + a, cc * CT_BK, tx0 - p.pad, ty0 - p.pad, b);
+                    for (int tap = 0; tap < 9; ++tap, ++bit) {
+                        const int s = bit % Cfg::STAGES;
+                        tc::mbar_wait(empty + s, ((bit / Cfg::STAGES) & 1) ^ 1);
+                        tc::mbar_arrive_expect_tx(full + s, Cfg::B_BYTES);
+                        tc::tma_load_2d(smB + s * Cfg::B_BYTES, &tmB, full + s, tap * p.cin + cc * CT_BK, n0);
+                    }
+                }
+            } else {
+                for (int it = 0; it < iters; ++it, ++bit) {
                     const int s = bit % Cfg::STAGES;
                     tc::mbar_wait(empty + s, ((bit / Cfg::STAGES) & 1) ^ 1);
-                    tc::mbar_arrive_expect_tx(full + s, Cfg::B_BYTES);
-                    tc::tma_load_2d(smB + s * Cfg::B_BYTES, &tmB, full + s, tap * p.cin + cc * CT_BK, n0);
+                    unsigned char* sa = smem + s * Cfg::STAGE_BYTES;
+                    unsigned char* sb = sa + CT_A_BYTES;
+                    const int tap = it / cchunks, cc = it - tap * cchunks;
+                    const int r = tap / p.KW, sx = tap - r * p.KW;
+                    tc::mbar_arrive_expect_tx(full + s, CT_A_BYTES + Cfg::B_BYTES);
+                    tc::tma_load_4d(sa, &tmA, full + s, cc * CT_BK, tx0 * p.stride + sx - p.pad, ty0 * p.stride + r - p.pad, b);
+                    tc::tma_load_2d(sb, &tmB, full + s, tap * p.cin + cc * CT_BK, n0);
                 }
             }
-        } else if (lane == 0) {
-            for (int it = 0; it < iters; ++it) {
-                const int s = it % Cfg::STAGES;
-                tc::mbar_wait(empty + s, ((it / Cfg::STAGES) & 1) ^ 1);
-                unsigned char* sa = smem + s * Cfg::STAGE_BYTES;
-                unsigned char* sb = sa + CT_A_BYTES;
-                const int tap = it / cchunks, cc = it - tap * cchunks;
-                const int r = tap / p.KW, sx = tap - r * p.KW;
-                const bool ldA = !(p.dbg & 2) || it < Cfg::STAGES, ldB = !(p.dbg & 1) || it < Cfg::STAGES;
-                tc::mbar_arrive_expect_tx(full + s, (ldA ? CT_A_BYTES : 0) + (ldB ? Cfg::B_BYTES : 0));
-                if (ldA) tc::tma_load_4d(sa, &tmA, full + s, cc * CT_BK, tx0 * p.stride + sx - p.pad, ty0 * p.stride + r - p.pad, b);
-                if (ldB) tc::tma_load_2d(sb, &tmB, full + s, tap * p.cin + cc * CT_BK, n0);
-            }
         }
-    } else {
-        // ---- main loop: warpgroup g accumulates pixels [64g, 64g+64) of the patch
-        const int g = warp >> 2;
-        float acc[BN / 2];
+        return;
+    }
+
+    // ---- consumers: warpgroup g accumulates pixels [64g, 64g+64) of the patch; fragment row r of this thread is tile row
+    // 16 * warp + lane / 4 + 8 r, its columns are 8 j + 2 (lane % 4) + {0, 1} (tc.cuh)
+    const int g = warp >> 2;
+    const int N = p.cout * p.os * p.os;          // GEMM columns: os x os sub-pixel groups of cout channels (ConvTranspose2d, kernel == stride)
+    unsigned char* stg = stg_all + warp * (BN / 32) * CT_BOX_BYTES;      // this warp's BN/32 staging boxes (16 rows x 128 B each)
+    float acc[BN / 2];
+    for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+        const int n0 = (t % tiles_n) * BN;
+        int mt = t / tiles_n;
+        const int tx0 = (mt % tiles_x) * TW; mt /= tiles_x;
+        const int ty0 = (mt % tiles_y) * TH;
+        const int b = mt / tiles_y;
+        // this thread's per-column scale / shift, loaded before the main loop so that the epilogue does not wait for them
+        float2 scl[BN / 8], shf[BN / 8];
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+            const int n = n0 + 8 * j + 2 * (lane & 3);
+            const int c = p.os == 1 ? n : n % p.cout;                  // n, n + 1 share the sub-pixel group: cout % 4 == 0
+            scl[j] = (n < N && p.scale) ? ldg2(p.scale + c) : make_float2(1.f, 1.f);
+            shf[j] = (n < N && p.shift) ? ldg2(p.shift + c) : make_float2(0.f, 0.f);
+        }
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
         if (HALO) {
-            int bit = 0;
-            for (int cc = 0; cc < cchunks; ++cc) {
-                const int a = cc % HL_A_STAGES;
-                tc::mbar_wait(a_full + a, (cc / HL_A_STAGES) & 1);
+            for (int cc = 0; cc < cchunks; ++cc, ++hs) {
+                const int a = hs % HL_A_STAGES;
+                tc::mbar_wait(a_full + a, (hs / HL_A_STAGES) & 1);
                 const uint32_t ha = tc::smem_u32(smem + a * HL_A_SLOT);
                 for (int tap = 0; tap < 9; ++tap, ++bit) {
                     const int s = bit % Cfg::STAGES;
@@ -163,18 +184,17 @@ k_conv2d_tf32(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
                     tc::wgmma_commit();
                     tc::wgmma_wait_one();               // this tap's MMAs stay in flight; the previous tap's weight tile is free
                     __syncwarp();
-                    if (lane == 0 && bit > 0) tc::mbar_arrive(empty + (bit - 1) % Cfg::STAGES);
+                    if (lane == 0 && (cc > 0 || tap > 0)) tc::mbar_arrive(empty + (bit - 1) % Cfg::STAGES);
                     // every MMA of the previous slice has completed: its halo slot is free
-                    if (lane == 0 && tap == 0 && cc > 0) tc::mbar_arrive(a_empty + (cc - 1) % HL_A_STAGES);
+                    if (lane == 0 && tap == 0 && cc > 0) tc::mbar_arrive(a_empty + (hs - 1) % HL_A_STAGES);
                 }
             }
             tc::wgmma_wait_all();
+            if (lane == 0) { tc::mbar_arrive(empty + (bit - 1) % Cfg::STAGES); tc::mbar_arrive(a_empty + (hs - 1) % HL_A_STAGES); }
         } else {
-            for (int it = 0; it < iters; ++it) {
-                const int s = it % Cfg::STAGES;
-                if (tr && threadIdx.x == 0 && it < 20) g_ct_trace[8 + it * 2] = clock64();
-                tc::mbar_wait(full + s, (it / Cfg::STAGES) & 1);
-                if (tr && threadIdx.x == 0 && it < 20) g_ct_trace[9 + it * 2] = clock64();
+            for (int it = 0; it < iters; ++it, ++bit) {
+                const int s = bit % Cfg::STAGES;
+                tc::mbar_wait(full + s, (bit / Cfg::STAGES) & 1);
                 const uint32_t sa = tc::smem_u32(smem + s * Cfg::STAGE_BYTES);
                 const uint64_t adesc = tc::smem_desc_sw128(sa + g * 64 * 128), bdesc = tc::smem_desc_sw128(sa + CT_A_BYTES);
                 tc::wgmma_fence();
@@ -184,144 +204,152 @@ k_conv2d_tf32(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
                 tc::wgmma_commit();
                 tc::wgmma_wait_one();                   // this step's MMAs stay in flight; the previous step's stage is free
                 __syncwarp();
-                if (lane == 0 && it > 0) tc::mbar_arrive(empty + (it - 1) % Cfg::STAGES);
+                if (lane == 0 && it > 0) tc::mbar_arrive(empty + (bit - 1) % Cfg::STAGES);
             }
             tc::wgmma_wait_all();
+            if (lane == 0) tc::mbar_arrive(empty + (bit - 1) % Cfg::STAGES);
         }
-        // (no stage is released after the last step: the producer has nothing left to load)
-        if (tr && threadIdx.x == 0) g_ct_trace[2] = clock64();
-        tc::acc_to_smem<BN>(acc, acc_stg, Cfg::ACC_LD, g * 64);
-        // the pipeline buffers are idle from here on: the epilogue stages its output tiles there
-        tc::named_sync(1, 32 * CT_CONSUMERS);
-        if (tr && threadIdx.x == 0) g_ct_trace[3] = clock64();
 
-        // ---- epilogue: warp w handles pixels [32*(w%4), +32) and channel half w/4 of the accumulator
-        const int q = warp & 3;
-        const int row = q * 32 + lane;                          // pixel index inside the TH x TW patch
-        constexpr int PER = BN >= 64 ? BN / 2 : BN;
-        const int half = warp >> 2;
-        const int y = ty0 + row / TW, x = tx0 + row % TW;
-        const bool valid = (y < p.Ho) && (x < p.Wo);
-        if (half == 1 && BN < 64) { /* nothing left for the second warp group */ } else
-#pragma unroll 1
-        for (int mc = half * PER; mc < half * PER + PER; mc += 32) {
-            const int c0 = mc;
-            float* orow = p.out + (((size_t)b * p.OH + (y * p.os + p.oy0)) * p.OW + (x * p.os + p.ox0)) * p.out_cstride + p.out_coff;
-            float v[32];
-            tc::smem_row32(acc_stg, Cfg::ACC_LD, row, mc, v);
-            if (p.gmax) {
-                // fused max-pool over the points of a crop (torch.max(dim=points), position_transformer.py:109,118): the 128 rows of this
-                // tile belong to ONE group (gmax_rows % 128 == 0); warp-shuffle max over its 32 rows per column, one atomic per warp and
-                // column.  The (rows, cout) activation is never written to HBM, the group_max pass never reads it back.
-                const int grp = (p.grow0 + ty0 * p.Wo + tx0) / p.gmax_rows;
-                // transpose through the (idle) pipeline buffers: row stride 33 floats => conflict-free scalar stores and column reads
-                float* stg = reinterpret_cast<float*>(smem + ((mc / 32) * 4 + q) * 4352);
+        // ---- epilogue from the accumulator registers: folded BatchNorm / bias / group shift / ReLU (separately rounded multiply
+        // and add), then the warp's 16 pixels through its staging boxes and TMA stores, a fused max over row groups, or per-thread
+        // stores
+        if (p.tma_store) {                            // this warp's previous TMA stores must have read its staging boxes
+            if (lane == 0) tc::tma_store_wait_read();
+            __syncwarp();
+        }
+        const uint32_t stg_u = tc::smem_u32(stg);
+        // staging element (row q = lane / 4 + 8 r, columns 8 j + 2 (lane % 4) + {0, 1}): box j / 4, 128-byte swizzle (16-byte
+        // chunk k of row q sits at chunk k ^ (q % 8))
+        auto stg_addr = [&](int j, int r) {
+            const int q = (lane >> 2) + 8 * r, k16 = 2 * (j & 3) + ((lane & 3) >> 1);
+            return stg_u + (uint32_t)((j >> 2) * CT_BOX_BYTES + q * 128 + ((k16 ^ (q & 7)) << 4) + (lane & 1) * 8);
+        };
+        if (p.tma_store && !p.gshift) {
+            // the BEV / head convolutions: nothing but arithmetic and shared-memory stores
 #pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const int n = n0 + c0 + j;
-                    float o = v[j];
-                    if (n < p.cout) {
-                        if (p.scale) o *= __ldg(p.scale + n);
-                        if (p.shift) o += __ldg(p.shift + n);
-                        if (p.relu) o = fmaxf(o, 0.f);
-                    }
-                    stg[lane * 33 + j] = valid ? o : -INFINITY;
-                }
-                __syncwarp();
-                float cm = -INFINITY;
+            for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
-                for (int r = 0; r < 32; ++r) cm = fmaxf(cm, stg[r * 33 + lane]);      // lane = column
-                const int n = n0 + c0 + lane;
-                if (n < p.cout) {
-                    float* addr = p.gmax + (size_t)grp * p.cout + n;
-                    if (cm >= 0.f) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(cm));
-                    else atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(cm));
+                for (int r = 0; r < 2; ++r) {
+                    float ox = __fmul_rn(acc[4 * j + 2 * r], scl[j].x), oy = __fmul_rn(acc[4 * j + 2 * r + 1], scl[j].y);
+                    if (p.shift) { ox = __fadd_rn(ox, shf[j].x); oy = __fadd_rn(oy, shf[j].y); }
+                    if (p.relu) { ox = tc::rna_tf32(fmaxf(ox, 0.f)); oy = tc::rna_tf32(fmaxf(oy, 0.f)); }   // feeds another TF32 conv
+                    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(stg_addr(j, r)), "f"(ox), "f"(oy) : "memory");
                 }
-                __syncwarp();
-            } else if (p.tma_store) {
-                // Per-pixel strided stores (32 lanes -> 32 different lines per instruction) would make the epilogue as long as the
-                // main loop.  Here the warp's 32 pixels x 32 channels go to the (now idle) pipeline buffers in the 128B-swizzled box
-                // layout and ONE TMA store per warp writes them (edge tiles clipped by the tensor map, channel range clipped at
-                // out_coff + cout).  Staging slots (16 KB each, 4 KB per warp) are carved from the pipeline buffers; each warp group
-                // owns half of them and a warp re-uses its 4 KB only after its own earlier TMA store has read it.
-                constexpr int SLOTS_H = (Cfg::BUF / CT_A_BYTES) / 2;
-                const int cj = (mc - half * PER) / 32;
-                if (cj >= SLOTS_H) { if (lane == 0) tc::tma_store_wait_read(); __syncwarp(); }
-                unsigned char* stg = smem + (half * SLOTS_H + cj % SLOTS_H) * CT_A_BYTES + q * 4096;        // 32 rows x 128 B
-                const uint32_t stg_u = tc::smem_u32(stg) + (uint32_t)((lane >> 3) * 1024 + (lane & 7) * 128);
+        } else {
+            int ys[2], xs[2];
+            bool valid[2];
 #pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    const int n = n0 + c0 + j;
-                    float4 o = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-                    if (n < p.cout) {
-                        if (p.scale) { float4 sc = __ldg(reinterpret_cast<const float4*>(p.scale + n)); o.x *= sc.x; o.y *= sc.y; o.z *= sc.z; o.w *= sc.w; }
-                        if (p.shift) { float4 sh = __ldg(reinterpret_cast<const float4*>(p.shift + n)); o.x += sh.x; o.y += sh.y; o.z += sh.z; o.w += sh.w; }
-                        if (p.gshift && valid) {
-                            float4 sh = __ldg(reinterpret_cast<const float4*>(p.gshift + (size_t)((p.grow0 + y * p.Wo + x) / p.gsize) * p.cout + n));
-                            o.x += sh.x; o.y += sh.y; o.z += sh.z; o.w += sh.w;
-                        }
-                    }
-                    if (p.relu) {
-                        o.x = tc::rna_tf32(fmaxf(o.x, 0.f)); o.y = tc::rna_tf32(fmaxf(o.y, 0.f));
-                        o.z = tc::rna_tf32(fmaxf(o.z, 0.f)); o.w = tc::rna_tf32(fmaxf(o.w, 0.f));
-                    }
-                    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(stg_u + (uint32_t)((((j >> 2) ^ (lane & 7))) << 4)),
-                                 "f"(o.x), "f"(o.y), "f"(o.z), "f"(o.w) : "memory");
-                }
-                tc::fence_proxy_async();                 // generic-proxy smem writes -> visible to the TMA (async proxy)
-                __syncwarp();
-                if (lane == 0 && n0 + c0 < p.cout) {
-                    const int row0 = ty0 + q * (32 / TW);      // the warp's 32 pixels = 32/TW patch rows
-                    if (p.tma_store == 2) {
-                        // ConvTranspose2d with kernel == stride: output pixel (y*os + oy0, x*os + ox0) through the 5-D view
-                        // [C][dx][x][dy][b*Ho + y] of the NHWC tensor.  The merged (batch, y) axis cannot clip rows past Ho: skip them
-                        // (Ho is even and row0 is even, so a 2-row box is either entirely inside or entirely outside)
-                        if (row0 < p.Ho) tc::tma_store_5d(&tmO, stg, p.out_coff + n0 + c0, p.ox0, tx0, p.oy0, b * p.Ho + row0);
-                    } else {
-                        tc::tma_store_4d(&tmO, stg, p.out_coff + n0 + c0, tx0, row0, b);
-                    }
-                    tc::tma_store_commit();
-                }
-            } else if (valid) {
+            for (int r = 0; r < 2; ++r) {
+                const int m = 16 * warp + (lane >> 2) + 8 * r;
+                ys[r] = ty0 + m / TW; xs[r] = tx0 + m % TW;
+                valid[r] = ys[r] < p.Ho && xs[r] < p.Wo;
+            }
 #pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    const int n = n0 + c0 + j;
-                    if (n >= p.cout) break;
-                    float4 o = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-                    if (p.scale) { float4 sc = __ldg(reinterpret_cast<const float4*>(p.scale + n)); o.x *= sc.x; o.y *= sc.y; o.z *= sc.z; o.w *= sc.w; }
-                    if (p.shift) { float4 sh = __ldg(reinterpret_cast<const float4*>(p.shift + n)); o.x += sh.x; o.y += sh.y; o.z += sh.z; o.w += sh.w; }
-                    if (p.gshift) {
-                        float4 sh = __ldg(reinterpret_cast<const float4*>(p.gshift + (size_t)((p.grow0 + y * p.Wo + x) / p.gsize) * p.cout + n));
-                        o.x += sh.x; o.y += sh.y; o.z += sh.z; o.w += sh.w;
+            for (int j = 0; j < BN / 8; ++j) {
+                const int n = n0 + 8 * j + 2 * (lane & 3);
+                const int grp = p.os == 1 ? 0 : n / p.cout;               // sub-pixel (dy, dx) of a strided output
+                const int c = n - grp * p.cout;                            // output channel
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    float2 o = make_float2(__fmul_rn(acc[4 * j + 2 * r], scl[j].x), __fmul_rn(acc[4 * j + 2 * r + 1], scl[j].y));
+                    if (p.shift) { o.x = __fadd_rn(o.x, shf[j].x); o.y = __fadd_rn(o.y, shf[j].y); }
+                    if (p.gshift && valid[r] && n < N) {
+                        const float2 gs = ldg2(p.gshift + (size_t)((p.grow0 + ys[r] * p.Wo + xs[r]) / p.gsize) * p.cout + c);
+                        o.x = __fadd_rn(o.x, gs.x); o.y = __fadd_rn(o.y, gs.y);
                     }
-                    if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-                    if (p.relu) { o.x = tc::rna_tf32(o.x); o.y = tc::rna_tf32(o.y); o.z = tc::rna_tf32(o.z); o.w = tc::rna_tf32(o.w); }  // feeds another TF32 conv
-                    *reinterpret_cast<float4*>(orow + n) = o;
+                    if (p.relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
+                    if (p.gmax) {
+                        // max over this thread's two rows (rows past the image do not count), kept in acc for the reduction below
+                        if (!valid[r]) o = make_float2(-INFINITY, -INFINITY);
+                        if (r == 0) { acc[4 * j] = o.x; acc[4 * j + 1] = o.y; }
+                        else { acc[4 * j] = fmaxf(acc[4 * j], o.x); acc[4 * j + 1] = fmaxf(acc[4 * j + 1], o.y); }
+                        continue;
+                    }
+                    if (p.relu) { o.x = tc::rna_tf32(o.x); o.y = tc::rna_tf32(o.y); }
+                    if (p.tma_store) {
+                        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(stg_addr(j, r)), "f"(o.x), "f"(o.y) : "memory");
+                    } else if (valid[r] && n < N) {
+                        const int dy = grp / p.os, dx = grp - dy * p.os;
+                        float* orow = p.out + (((size_t)b * p.OH + (ys[r] * p.os + dy)) * p.OW + (xs[r] * p.os + dx)) * p.out_cstride + p.out_coff;
+                        *reinterpret_cast<float2*>(orow + c) = o;
+                    }
                 }
             }
         }
-        if (p.tma_store && lane == 0) tc::tma_store_wait_read();      // the stores must have read the staging buffers
+        if (p.gmax) {
+            // fused max-pool over the points of a crop (torch.max(dim=points), position_transformer.py:109,118): the 128 rows of this
+            // tile belong to ONE group (gmax_rows % 128 == 0).  Shuffle max over the warp's 16 rows, a max over the 8 warps through
+            // shared memory, one atomic per column and tile.  The (rows, cout) activation is never written to HBM.
+            float* red = reinterpret_cast<float*>(stg_all);                 // [8 warps][BN]
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+                for (int c = 0; c < 2; ++c) {
+                    float v = acc[4 * j + c];
+                    v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 4));
+                    v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 8));
+                    v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 16));
+                    if (lane < 4) red[warp * BN + 8 * j + 2 * lane + c] = v;
+                }
+            }
+            tc::named_sync(1, 32 * CT_CONSUMERS);
+            if (threadIdx.x < BN && n0 + (int)threadIdx.x < N) {
+                float cm = red[threadIdx.x];
+#pragma unroll
+                for (int w = 1; w < CT_CONSUMERS; ++w) cm = fmaxf(cm, red[w * BN + threadIdx.x]);
+                const int grp = (p.grow0 + ty0 * p.Wo + tx0) / p.gmax_rows;
+                float* addr = p.gmax + (size_t)grp * p.cout + n0 + threadIdx.x;
+                if (cm >= 0.f) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(cm));
+                else atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(cm));
+            }
+            tc::named_sync(1, 32 * CT_CONSUMERS);                            // red is rewritten by the next tile
+        } else if (p.tma_store) {
+            tc::fence_proxy_async();                 // generic-proxy smem writes -> visible to the TMA (async proxy)
+            __syncwarp();
+            if (lane == 0) {
+#pragma unroll 1
+                for (int cj = 0; cj < BN / 32; ++cj) {
+                    const int n = n0 + 32 * cj;
+                    if (n >= N) break;
+                    if (p.tma_store == 2) {
+                        // ConvTranspose2d with kernel == stride: output pixel (y*os + dy, x*os + dx) through the 5-D view
+                        // [C][dx][x][dy][b*Ho + y] of the NHWC tensor; the warp's 16 pixels are one patch row (TW == 16).  The merged
+                        // (batch, y) axis cannot clip rows past Ho: skip them
+                        const int grp = n / p.cout, dy = grp / p.os, y = ty0 + warp;
+                        if (y < p.Ho) tc::tma_store_5d(&tmO, stg + cj * CT_BOX_BYTES, p.out_coff + n - grp * p.cout, grp - dy * p.os, tx0, dy, b * p.Ho + y);
+                    } else {
+                        tc::tma_store_4d(&tmO, stg + cj * CT_BOX_BYTES, p.out_coff + n, tx0, ty0 + warp * (16 / TW), b);
+                    }
+                }
+                tc::tma_store_commit();
+            }
+        }
     }
-    if (tr && threadIdx.x == 0) g_ct_trace[4] = clock64();
+    if (p.tma_store && lane == 0) tc::tma_store_wait_read();      // the stores must have read the staging buffers
 }
 
 template <int BN, bool HALO>
 static int launch_tf32(const Conv2dParams& p, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmO, cudaStream_t st) {
     using Cfg = CtCfg<BN, HALO>;
-    static bool configured = false;
-    if (!configured) {
+    static int ctas_per_sm = 0;                   // the small configurations fit two CTAs per SM
+    if (!ctas_per_sm) {
         DZ_CUDA(cudaFuncSetAttribute(k_conv2d_tf32<BN, HALO>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM));
-        configured = true;
+        DZ_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas_per_sm, k_conv2d_tf32<BN, HALO>, CT_THREADS, Cfg::SMEM));
+        if (ctas_per_sm < 1) ctas_per_sm = 1;
     }
-    int tiles_x = dz_cdiv(p.Wo, Cfg::TW), tiles_y = dz_cdiv(p.Ho, Cfg::TH);
-    dim3 grid(tiles_x * tiles_y * p.B, dz_cdiv(p.cout, BN));
-    static_assert((BN / 32) * CT_A_BYTES <= Cfg::BUF, "epilogue staging must fit in the pipeline buffers");
-    k_conv2d_tf32<BN, HALO><<<grid, CT_THREADS, Cfg::SMEM, st>>>(tmA, tmB, tmO, p, tiles_x, tiles_y);
+    static_assert(CT_CONSUMERS * BN * 4 <= Cfg::STG_BYTES, "the group-max reduction must fit in the staging area");
+    const int tiles_x = dz_cdiv(p.Wo, Cfg::TW), tiles_y = dz_cdiv(p.Ho, Cfg::TH), tiles_n = dz_cdiv(p.cout * p.os * p.os, BN);
+    const long long tiles = (long long)tiles_x * tiles_y * p.B * tiles_n;
+    if (tiles > INT32_MAX) { dz_set_error("dz_conv2d_fwd(tf32): %lld tiles", tiles); return DZ_ERR_UNSUPPORTED; }
+    const int grid = (int)(tiles < (long long)DZ_NUM_SMS * ctas_per_sm ? tiles : (long long)DZ_NUM_SMS * ctas_per_sm);
+    k_conv2d_tf32<BN, HALO><<<grid, CT_THREADS, Cfg::SMEM, st>>>(tmA, tmB, tmO, p, tiles_x, tiles_y, tiles_n, (int)tiles);
     DZ_LAUNCH_CHECK();
     return DZ_OK;
 }
 
-// p.w must be in (cout, KH, KW, cin) layout for this path
+// p.w must be in (cout, KH, KW, cin) layout for this path.  p.os >= 2 (oy0 = ox0 = 0, KH = KW = 1) is a ConvTranspose2d with
+// kernel == stride as ONE GEMM over the input pixels: N = os * os * cout columns, weights in (dy, dx, cout, cin) layout; column
+// n goes to channel n % cout of output pixel (y * os + dy, x * os + dx), (dy, dx) = (n / cout) / os, % os.
 int dz_conv2d_fwd_tc(const Conv2dParams& p_in, int mode, cudaStream_t st) {
     Conv2dParams p = p_in;
     if (mode != DZ_TF32) { dz_set_error("dz_conv2d_fwd: tensor-core mode %d not built (tf32 only)", mode); return DZ_ERR_UNSUPPORTED; }
@@ -329,16 +357,20 @@ int dz_conv2d_fwd_tc(const Conv2dParams& p_in, int mode, cudaStream_t st) {
         dz_set_error("dz_conv2d_fwd(tf32): needs cin %% 32 == 0 and 16-byte aligned channel slices (cin=%d cout=%d)", p.cin, p.cout);
         return DZ_ERR_UNSUPPORTED;
     }
+    if (p.oy0 != 0 || p.ox0 != 0 || p.OH != p.Ho * p.os || p.OW != p.Wo * p.os || (p.os > 1 && (p.KH != 1 || p.KW != 1 || p.gmax))) {
+        dz_set_error("dz_conv2d_fwd(tf32): unsupported output geometry (os=%d)", p.os);
+        return DZ_ERR_UNSUPPORTED;
+    }
     tc::EncodeTiledFn enc = tc::get_encode_tiled();
     if (!enc) { dz_set_error("cuTensorMapEncodeTiled unavailable"); return DZ_ERR_CUDA; }
-    static const int no_tma_store = getenv("DZ_CONV2D_NO_TMA_STORE") ? 1 : 0;
-    p.tma_store = (!p.gmax && !no_tma_store && p.os == 1 && p.oy0 == 0 && p.ox0 == 0 && p.OH == p.Ho && p.OW == p.Wo &&
-                   (reinterpret_cast<uintptr_t>(p.out) & 15) == 0) ? 1 : 0;
-    // 3x3 stride-1 convolutions with at least two patches per SM and 128-channel slice: the halo variant (DZ_CONV2D_HALO=0 switches it off)
-    static const int use_halo = getenv("DZ_CONV2D_HALO") ? atoi(getenv("DZ_CONV2D_HALO")) : 1;
+    const bool aligned = (reinterpret_cast<uintptr_t>(p.out) & 15) == 0;
+    // TMA-store epilogue unless the output pointer is misaligned or a 32-channel store box would straddle two sub-pixels
+    p.tma_store = (p.gmax || !aligned) ? 0 : p.os == 1 ? 1 : (p.cout % 32 == 0 ? 2 : 0);
+    const int N = p.cout * p.os * p.os;
+    const int bn = N > 64 ? 128 : (N > 32 ? 64 : 32);
+    // 3x3 stride-1 convolutions with at least two patches per SM and 128-channel slice: the halo variant
     const long long tiles_m = (long long)dz_cdiv(p.Wo, CT_TW) * dz_cdiv(p.Ho, CT_TH) * p.B;
-    const bool halo = use_halo && p.KH == 3 && p.KW == 3 && p.stride == 1 && p.tma_store == 1 && !p.gshift && !(p.dbg & 3) &&
-                      tiles_m * dz_cdiv(p.cout, 128) >= 2 * DZ_NUM_SMS;
+    const bool halo = p.KH == 3 && p.KW == 3 && p.stride == 1 && p.tma_store == 1 && !p.gshift && tiles_m * dz_cdiv(p.cout, 128) >= 2 * DZ_NUM_SMS;
     const int TW = halo ? HL_TW : CT_TW;
     CUtensorMap tmA, tmB;
     {
@@ -353,10 +385,9 @@ int dz_conv2d_fwd_tc(const Conv2dParams& p_in, int mode, cudaStream_t st) {
                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { dz_set_error("cuTensorMapEncodeTiled(A) failed: %d", (int)r); return DZ_ERR_CUDA; }
     }
-    const int bn = p.cout > 64 ? 128 : (p.cout > 32 ? 64 : 32);
     {
         cuuint64_t ktot = (cuuint64_t)p.KH * p.KW * p.cin;
-        cuuint64_t dims[2] = {ktot, (cuuint64_t)p.cout};
+        cuuint64_t dims[2] = {ktot, (cuuint64_t)N};
         cuuint64_t strides[1] = {ktot * 4};
         cuuint32_t box[2] = {(cuuint32_t)CT_BK, (cuuint32_t)bn};
         cuuint32_t estr[2] = {1, 1};
@@ -365,15 +396,12 @@ int dz_conv2d_fwd_tc(const Conv2dParams& p_in, int mode, cudaStream_t st) {
         if (r != CUDA_SUCCESS) { dz_set_error("cuTensorMapEncodeTiled(B) failed: %d", (int)r); return DZ_ERR_CUDA; }
     }
     CUtensorMap tmO = tmB;
-    if (!p.tma_store && !p.gmax && !no_tma_store && p.os >= 2 && p.OH == p.Ho * p.os && p.OW == p.Wo * p.os && p.Ho % 2 == 0 &&
-        p.oy0 < p.os && p.ox0 < p.os && (reinterpret_cast<uintptr_t>(p.out) & 15) == 0) {
-        // strided output (ConvTranspose2d as os*os 1x1 convs): 5-D view [C][dx][x][dy][b*Ho + y], one TMA store per warp as above instead of
-        // per-thread strided stores
-        p.tma_store = 2;
+    if (p.tma_store == 2) {
+        // strided output: 5-D view [C][dx][x][dy][b*Ho + y] of the NHWC tensor, box = one warp's 16 pixels (one patch row) x 32 channels
         cuuint64_t dims[5] = {(cuuint64_t)(p.out_coff + p.cout), (cuuint64_t)p.os, (cuuint64_t)p.Wo, (cuuint64_t)p.os, (cuuint64_t)p.Ho * p.B};
         cuuint64_t strides[4] = {(cuuint64_t)p.out_cstride * 4, (cuuint64_t)p.os * p.out_cstride * 4, (cuuint64_t)p.OW * p.out_cstride * 4,
                                  (cuuint64_t)p.os * p.OW * p.out_cstride * 4};
-        cuuint32_t box[5] = {32, 1, (cuuint32_t)CT_TW, 1, 2};
+        cuuint32_t box[5] = {32, 1, (cuuint32_t)CT_TW, 1, 1};
         cuuint32_t estr[5] = {1, 1, 1, 1, 1};
         CUresult r = enc(&tmO, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, (void*)p.out, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -382,7 +410,7 @@ int dz_conv2d_fwd_tc(const Conv2dParams& p_in, int mode, cudaStream_t st) {
         // channels [0, out_coff + cout) of the (possibly wider, concatenated) output tensor: stores past cout are clipped
         cuuint64_t dims[4] = {(cuuint64_t)(p.out_coff + p.cout), (cuuint64_t)p.OW, (cuuint64_t)p.OH, (cuuint64_t)p.B};
         cuuint64_t strides[3] = {(cuuint64_t)p.out_cstride * 4, (cuuint64_t)p.OW * p.out_cstride * 4, (cuuint64_t)p.OH * p.OW * p.out_cstride * 4};
-        cuuint32_t box[4] = {32, (cuuint32_t)TW, (cuuint32_t)(32 / TW), 1};      // one warp's 32 pixels
+        cuuint32_t box[4] = {32, (cuuint32_t)TW, (cuuint32_t)(16 / TW), 1};      // one warp's 16 pixels
         cuuint32_t estr[4] = {1, 1, 1, 1};
         CUresult r = enc(&tmO, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)p.out, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -399,7 +427,6 @@ int dz_conv2d_fwd_tc(const Conv2dParams& p_in, int mode, cudaStream_t st) {
         default: return launch_tf32<32, false>(p, tmA, tmB, tmO, st);
     }
 }
-
 
 // y = act((x @ W^T) * scale + shift) on the tensor cores: a linear layer is a 1x1 convolution over an "image" of width 16
 // whose pixels are the rows of x (an 8 x 16 patch == 128 consecutive rows), so the implicit-GEMM kernel above serves

@@ -406,7 +406,7 @@ def deconv2d(x, weight_packed, kshape, scale, shift, relu, out=None, out_coff=0,
         out = torch.empty((B, H * s, W * s, cout), dtype=torch.float32, device=x.device)
     check(lib().dz_deconv2d_fwd(_p(_f32c(x)), B, H, W, cin, _p(_f32c(weight_packed)), s, _p(scale), _p(shift),
                                 int(relu), _p(out), cout, out_coff, out.shape[3], mode, _stream()), 'deconv2d_fwd')
-    _count(s * s)
+    _count(s * s if mode == _lib.DZ_F32 else 1)          # tensor cores: one GEMM over all s*s sub-pixels
     return out
 
 

@@ -1,5 +1,4 @@
-"""time one dense BEV conv (default 128->128 3x3 at 188x188) through the C ABI; DZ_CONV2D_DBG=1/2/3 drops the weight /
-activation / both TMA loads after the pipeline fill (timing experiment, results are then meaningless)"""
+"""time one dense BEV conv (default 128->128 3x3 at 188x188) through the C ABI"""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from detzero_b200 import ops, _lib
@@ -23,7 +22,7 @@ for i in range(13):
     if i >= 3: ts.append(e0.elapsed_time(e1) * 1000)
 ts.sort()
 fl = 2.0 * NB * hw * hw * cin * cout * 9
-print('DZ_CONV2D_DBG=%s HALO=%s batch %d conv %d->%d 3x3 @%d^2: median %.1f us  (%.0f TFLOP/s)' % (os.environ.get('DZ_CONV2D_DBG', '0'), os.environ.get('DZ_CONV2D_HALO', '-'), NB, cin, cout, hw, ts[len(ts) // 2], fl / ts[len(ts) // 2] / 1e6))
+print('batch %d conv %d->%d 3x3 @%d^2: median %.1f us  (%.0f TFLOP/s)' % (NB, cin, cout, hw, ts[len(ts) // 2], fl / ts[len(ts) // 2] / 1e6))
 # steady state: a CUDA graph of 10 back-to-back convs (x -> y -> x ...): no host latency, warm L2, real launch gaps
 if cin == cout:
     y = torch.empty_like(x)
@@ -44,12 +43,3 @@ if cin == cout:
         tg.append(e0.elapsed_time(e1) * 100)
     tg.sort()
     print('  back-to-back in a CUDA graph (10 convs): %.1f us per conv (%.0f TFLOP/s)' % (tg[len(tg) // 2], fl / tg[len(tg) // 2] / 1e6))
-if int(os.environ.get('DZ_CONV2D_DBG', '0')) & 4:
-    import ctypes, numpy as np
-    l = ctypes.CDLL(_lib.LIB_PATH)
-    buf = np.zeros(64, np.int64)
-    l.dz_debug_conv2d_trace(ctypes.c_void_p(buf.ctypes.data))
-    t0 = buf[0]
-    print('CTA 0 cycles: setup %d | mma thread done issuing at %d | epilogue starts %d | epilogue warp 2 done (stores read) %d' % (buf[1] - t0, buf[2] - t0, buf[3] - t0, buf[5] - t0))
-    st = (buf[8:48].reshape(-1, 2) - t0)
-    print('k-step: [wait_full_start, full_ok]', st[:20].tolist())
