@@ -37,10 +37,10 @@ _SIGS = {
     'dz_mean_vfe': (ci, [vp, vp, ci, ci, ci, vp, vp]),
     'dz_voxelize_dynamic_ws_bytes': (sz, [ci, ci, ci, ci, ci, ci]),
     'dz_voxelize_dynamic_mean': (ci, [vp, ci, ci, ci, vp, vp, vp, vp, vp, ci, vp, vp, sz, vp]),
-    'dz_rulebook_subm': (ci, [vp, vp, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp, vp, vp, ci, vp]),
-    'dz_rulebook_conv': (ci, [vp, vp, ci, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, ci, vp, vp, vp, vp, vp, sz, vp, ci, vp]),
+    'dz_rulebook_subm': (ci, [vp, vp, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp, vp, vp, vp]),
+    'dz_rulebook_conv': (ci, [vp, vp, ci, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, ci, vp, vp, vp, vp, vp, sz, vp, vp]),
     'dz_rulebook_schedule_ws_bytes': (sz, [ci]),
-    'dz_rulebook_schedule': (ci, [vp, ci, vp, vp, vp, sz, ci, ci, ci, vp, vp]),
+    'dz_rulebook_schedule': (ci, [vp, ci, vp, vp, vp, sz, ci, vp, vp]),
     'dz_spconv_fwd': (ci, [vp, ci, ci, vp, ci, ci, vp, vp, ci, vp, vp, vp, vp, ci, vp, ci, ci, vp]),
     'dz_rulebook_transpose': (ci, [vp, ci, ci, vp, vp, ci, vp]),
     'dz_spconv_wgrad': (ci, [vp, ci, vp, ci, ci, vp, ci, vp, ci, vp, vp]),

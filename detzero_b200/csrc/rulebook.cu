@@ -23,17 +23,7 @@ struct TableOut {
     int* masks;                                     // [cap]        neighbour bit masks (compact copy for the schedule pass)
     int* hist;                                      // [SCHED_BINS] digest histogram -> exclusive offsets (last block)
     int* ticket;                                    // block-completion counter
-    int fb;                                         // frame bits of the schedule key (0 = digest only)
-    int B;                                          // frames in the batch
 };
-
-// schedule key = (frame group, digest): frame-major order keeps the rows a CTA wave gathers inside ONE frame's feature map
-// (L2-resident) instead of spreading every tile over the whole batch; the digest gives up its fb lowest-priority bits
-__device__ __forceinline__ uint32_t sched_key(const TableOut& to, uint32_t digest, int frame) {
-    if (to.fb == 0) return digest;
-    const uint32_t fg = ((uint32_t)frame << to.fb) / (uint32_t)to.B;
-    return (fg << (12 - to.fb)) | (digest >> to.fb);
-}
 
 // Rows are grouped by DESCENDING digest so that the tiles with many offsets come first (launch order ~ tile order).
 __device__ __forceinline__ uint32_t sched_digest(uint32_t m, int K) {
@@ -49,7 +39,7 @@ __device__ __forceinline__ uint32_t sched_digest(uint32_t m, int K) {
 
 // one table row: v[0..K-1] neighbour rows (or -1).  s_hist: the block's digest histogram in shared memory (hot digests
 // are shared by thousands of rows: per-row or per-warp global atomics on them serialise in L2)
-__device__ __forceinline__ void table_emit(const TableOut& to, bool valid, int i, int cap, const int (&v)[27], int K, int* s_hist, int frame) {
+__device__ __forceinline__ void table_emit(const TableOut& to, bool valid, int i, int cap, const int (&v)[27], int K, int* s_hist) {
     uint32_t mask = 0;
 #pragma unroll
     for (int k = 0; k < 27; ++k) mask |= (k < K && v[k] >= 0 ? 1u : 0u) << k;
@@ -70,7 +60,7 @@ __device__ __forceinline__ void table_emit(const TableOut& to, bool valid, int i
         }
     }
     if (to.keys && valid) {
-        const uint32_t key = sched_key(to, sched_digest(mask, K), frame);
+        const uint32_t key = sched_digest(mask, K);
         to.keys[i] = (uint16_t)key;
         to.masks[i] = (int)mask;
         atomicAdd(s_hist + key, 1);
@@ -118,12 +108,10 @@ __global__ void __launch_bounds__(256) k_subm_nbr(const int32_t* __restrict__ co
     for (int base = blockIdx.x * blockDim.x + threadIdx.x - lane; base < n; base += gridDim.x * blockDim.x) {     // warp-uniform trip count
         const int i = base + lane;
         int v[27];
-        int frame = 0;
 #pragma unroll
         for (int k = 0; k < 27; ++k) v[k] = -1;
         if (i < n) {
             int4 c = __ldg(reinterpret_cast<const int4*>(coords) + i);    // b,z,y,x
-            frame = c.x;
             int kz = 0, ky = 0, kx = 0;
 #pragma unroll
             for (int k = 0; k < 27; ++k) {
@@ -134,21 +122,15 @@ __global__ void __launch_bounds__(256) k_subm_nbr(const int32_t* __restrict__ co
                 }
             }
         }
-        table_emit(to, i < n, i, cap, v, K, s_hist, frame);
+        table_emit(to, i < n, i, cap, v, K, s_hist);
     }
     table_finish(to, s_hist);
 }
 
 // workspace layout shared by the rulebook kernels (which emit digests + histogram) and dz_rulebook_schedule:
 // hist[SCHED_BINS] | tile_mask[tiles] | tickets[8] | masks[cap] | keys[cap] (u16)
-static int sched_frame_bits(int B, int frame_major) {
-    if (!frame_major || B <= 1) return 0;
-    int fb = 1;
-    while ((1 << fb) < B && fb < 4) ++fb;
-    return fb;
-}
-static TableOut table_out(int32_t* nbr, int32_t* tab, void* sched_ws, int cap, int B = 1, int frame_major = 0) {
-    TableOut to{nbr, tab, nullptr, nullptr, nullptr, nullptr, sched_frame_bits(B, frame_major), B};
+static TableOut table_out(int32_t* nbr, int32_t* tab, void* sched_ws, int cap) {
+    TableOut to{nbr, tab, nullptr, nullptr, nullptr, nullptr};
     if (sched_ws) {
         to.hist = reinterpret_cast<int*>(sched_ws);
         to.ticket = to.hist + SCHED_BINS + dz_cdiv(cap, 128);
@@ -162,11 +144,11 @@ extern "C" size_t dz_rulebook_schedule_ws_bytes(int cap) { return sched_zero_byt
 
 extern "C" int dz_rulebook_subm(const int32_t* coords, const int* d_n, int cap, int B, int D, int H, int W,
                                 const int* ks, const uint32_t* bitmap, const uint32_t* prefix, const int32_t* perm,
-                                int32_t* nbr, int32_t* tab, void* sched_ws, int sched_frame_major, dz_stream_t stream) {
+                                int32_t* nbr, int32_t* tab, void* sched_ws, dz_stream_t stream) {
     DZ_CHECK_ARG(coords && d_n && bitmap && prefix && (nbr || tab) && cap >= 1);
     DZ_CHECK_ARG(ks[0] % 2 == 1 && ks[1] % 2 == 1 && ks[2] % 2 == 1 && ks[0] * ks[1] * ks[2] <= 27);
     DZ_CHECK_ARG(!sched_ws || tab);
-    TableOut to = table_out(nbr, tab, sched_ws, cap, B, sched_frame_major);
+    TableOut to = table_out(nbr, tab, sched_ws, cap);
     if (sched_ws) DZ_CUDA(cudaMemsetAsync(sched_ws, 0, sched_zero_bytes(cap), (cudaStream_t)stream));
     GridIndex g{bitmap, prefix, perm, B, D, H, W, dz_cells_pad(D, H, W)};
     int blocks = max(1, min(dz_cdiv(cap, 256), DZ_NUM_SMS * 8));
@@ -244,12 +226,10 @@ __global__ void __launch_bounds__(256) k_conv_nbr(const int32_t* __restrict__ ou
     for (int base = blockIdx.x * blockDim.x + threadIdx.x - lane; base < n; base += gridDim.x * blockDim.x) {     // warp-uniform trip count
         const int o = base + lane;
         int v[27];
-        int frame = 0;
 #pragma unroll
         for (int k = 0; k < 27; ++k) v[k] = -1;
         if (o < n) {
             int4 c = __ldg(reinterpret_cast<const int4*>(out_coords) + o);
-            frame = c.x;
             int kz = 0, ky = 0, kx = 0;
 #pragma unroll
             for (int k = 0; k < 27; ++k) {
@@ -259,7 +239,7 @@ __global__ void __launch_bounds__(256) k_conv_nbr(const int32_t* __restrict__ ou
                 }
             }
         }
-        table_emit(to, o < n, o, out_cap, v, K, s_hist, frame);
+        table_emit(to, o < n, o, out_cap, v, K, s_hist);
     }
     table_finish(to, s_hist);
 }
@@ -272,7 +252,7 @@ extern "C" int dz_rulebook_conv(const int32_t* in_coords, const int* d_n_in, int
                                 const int* ks, const int* st_, const int* pd, const uint32_t* in_bitmap,
                                 const uint32_t* in_prefix, const int32_t* in_perm, int32_t* out_coords, int* d_n_out,
                                 int out_cap, uint32_t* out_bitmap, uint32_t* out_prefix, int32_t* nbr, int32_t* tab, void* ws,
-                                size_t ws_bytes, void* sched_ws, int sched_frame_major, dz_stream_t stream) {
+                                size_t ws_bytes, void* sched_ws, dz_stream_t stream) {
     DZ_CHECK_ARG(in_coords && d_n_in && in_bitmap && in_prefix && out_coords && d_n_out && out_bitmap && out_prefix && (nbr || tab));
     DZ_CHECK_ARG(!sched_ws || tab);
     DZ_CHECK_ARG(in_cap >= 1 && out_cap >= 1 && B >= 1);
@@ -295,7 +275,7 @@ extern "C" int dz_rulebook_conv(const int32_t* in_coords, const int* d_n_in, int
                                                 out_cp, out_cap, out_coords);
     GridIndex gin{in_bitmap, in_prefix, in_perm, B, in_dhw[0], in_dhw[1], in_dhw[2], dz_cells_pad(in_dhw[0], in_dhw[1], in_dhw[2])};
     int blocks_out = max(1, min(dz_cdiv(out_cap, 256), DZ_NUM_SMS * 8));
-    TableOut to = table_out(nbr, tab, sched_ws, out_cap, B, sched_frame_major);
+    TableOut to = table_out(nbr, tab, sched_ws, out_cap);
     if (sched_ws) DZ_CUDA(cudaMemsetAsync(sched_ws, 0, sched_zero_bytes(out_cap), st));
     k_conv_nbr<<<blocks_out, 256, 0, st>>>(out_coords, d_n_out, out_cap, cg, gin, to);
     DZ_LAUNCH_CHECK();
@@ -321,13 +301,11 @@ extern "C" int dz_rulebook_conv(const int32_t* in_coords, const int* d_n_in, int
 // order[p].  Every row's accumulation order over k is unchanged, so results are bit-identical to the unscheduled launch.
 // =====================================================================================================================
 static constexpr int SCHED_CHUNK = 512;            // rows per scatter block
-__device__ __forceinline__ int tile_bin(int tm) {
-    const int m = tm & 0x7ffffff;
-    return m ? ((tm >> 27) & 15) * 28 + (27 - __popc(m)) : 511;
-}
+static constexpr int TILE_BINS = 28;               // tile order: 27 .. 1 live offsets, then the empty capacity tiles
+__device__ __forceinline__ int tile_bin(int m) { return m ? 27 - __popc(m) : 27; }
 __global__ void __launch_bounds__(256) k_sched_scatter(const int32_t* __restrict__ masks, int cap, const int* __restrict__ d_n,
                                                        const uint16_t* __restrict__ keys, int* __restrict__ offs, int* __restrict__ tile_mask,
-                                                       int* __restrict__ ticket, int32_t* __restrict__ order, int fb) {
+                                                       int* __restrict__ ticket, int32_t* __restrict__ order) {
     // block-aggregated counting-sort scatter: count this block's rows per digest in shared memory, reserve one global range
     // per (block, digest) with a single atomic, then hand out positions from shared memory
     __shared__ int s_cnt[SCHED_BINS];
@@ -345,18 +323,16 @@ __global__ void __launch_bounds__(256) k_sched_scatter(const int32_t* __restrict
     for (int i = r0 + threadIdx.x; i < r1; i += blockDim.x) {
         const int pos = atomicAdd(s_cnt + keys[i], 1);
         order[pos] = i;
-        int m = __ldg(masks + i);
+        const int m = __ldg(masks + i);
         int* tm = tile_mask + (pos >> 7);
-        if (fb && (pos & 127) == 0) m |= (int)(keys[i] >> (12 - fb)) << 27;      // the tile's frame group = its first row's (bits 27..30)
         if ((__ldcg(tm) & m) != m) atomicOr(tm, m);              // plain read first: after a few rows the tile's mask is complete
     }
-    // ---- the last block orders the tiles by descending work (counting sort over popc(mask) = 0..27)
-    // frame-major: bin = frame group * 28 + (27 - live offsets); empty capacity tiles (mask 0) go last (bin 511)
-    __shared__ int s_last, bins[512];
+    // ---- the last block orders the tiles by descending work (counting sort over popc(mask) = 27..1, empty tiles last)
+    __shared__ int s_last, bins[TILE_BINS];
     __threadfence();
     __syncthreads();
     if (threadIdx.x == 0) s_last = (atomicAdd(ticket, 1) == (int)gridDim.x - 1);
-    for (int b = threadIdx.x; b < 512; b += blockDim.x) bins[b] = 0;
+    for (int b = threadIdx.x; b < TILE_BINS; b += blockDim.x) bins[b] = 0;
     __syncthreads();
     if (!s_last) return;
     __threadfence();
@@ -373,7 +349,7 @@ __global__ void __launch_bounds__(256) k_sched_scatter(const int32_t* __restrict
     __syncthreads();
     if (threadIdx.x == 0) {
         int run = 0;
-        for (int b = 0; b < 512; ++b) { int c = bins[b]; bins[b] = run; run += c; }
+        for (int b = 0; b < TILE_BINS; ++b) { int c = bins[b]; bins[b] = run; run += c; }
     }
     __syncthreads();
     for (int t0 = threadIdx.x - lane; t0 < tiles; t0 += blockDim.x) {
@@ -397,7 +373,7 @@ __global__ void __launch_bounds__(256) k_sched_tiles(const int32_t* __restrict__
     const int tiles_n = (n + 127) >> 7;
     const int tiles = (cap + 127) >> 7;
     int32_t* mask_out = const_cast<int32_t*>(order) + cap + tiles;                 // order[cap + tiles + j] = OR of tile j's row masks
-    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < tiles; j += gridDim.x * blockDim.x) mask_out[j] = __ldg(tile_mask + j) & 0x7ffffff;
+    for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < tiles; j += gridDim.x * blockDim.x) mask_out[j] = __ldg(tile_mask + j);
     for (int pos = blockIdx.x * blockDim.x + threadIdx.x; pos < tiles_n * 128; pos += gridDim.x * blockDim.x) {
         const int i = pos < n ? __ldg(order + pos) : -1;
         int w[28];
@@ -416,12 +392,11 @@ __global__ void __launch_bounds__(256) k_sched_tiles(const int32_t* __restrict__
 }
 
 extern "C" int dz_rulebook_schedule(const int32_t* tab, int cap, const int* d_n, int32_t* order, void* sched_ws, size_t ws_bytes,
-                                    int B, int sched_frame_major, int K, int32_t* tab_tiles, dz_stream_t stream) {
+                                    int K, int32_t* tab_tiles, dz_stream_t stream) {
     DZ_CHECK_ARG(tab && d_n && order && sched_ws && cap >= 1);
     if (ws_bytes < dz_rulebook_schedule_ws_bytes(cap)) { dz_set_error("dz_rulebook_schedule: workspace too small"); return DZ_ERR_WORKSPACE; }
     TableOut to = table_out(nullptr, const_cast<int32_t*>(tab), sched_ws, cap);
-    k_sched_scatter<<<dz_cdiv(cap, SCHED_CHUNK), 256, 0, (cudaStream_t)stream>>>(to.masks, cap, d_n, to.keys, to.hist, to.hist + SCHED_BINS, to.ticket + 1, order,
-                                                                                 sched_frame_bits(B, sched_frame_major));
+    k_sched_scatter<<<dz_cdiv(cap, SCHED_CHUNK), 256, 0, (cudaStream_t)stream>>>(to.masks, cap, d_n, to.keys, to.hist, to.hist + SCHED_BINS, to.ticket + 1, order);
     DZ_LAUNCH_CHECK();
     if (tab_tiles) {
         DZ_CHECK_ARG(K >= 1 && K <= 27);

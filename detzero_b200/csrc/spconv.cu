@@ -180,6 +180,7 @@ static int launch_f32(const float* in, int cin, const int32_t* nbr, int K, int n
     return DZ_OK;
 }
 
+// DZ_TF32 / DZ_TF32X3: csrc/spconv_tc.cu
 int dz_spconv_fwd_tc(const float* in, int cin, int in_rows, const int32_t* nbr, int K, int nbr_cap, const int32_t* order, const int* d_n_out, int out_cap,
                      const float* weight, const float* scale, const float* shift, const float* residual, int relu,
                      float* out, int cout, int mode, cudaStream_t st);

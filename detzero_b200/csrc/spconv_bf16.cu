@@ -27,13 +27,9 @@
 // so a tile's prologue (table load) hides under the neighbouring tile's main loop and the producers run ahead into the next
 // tile while the consumers run the epilogue.  No atomics: deterministic; a row's accumulation order over
 // the reduction blocks never depends on the schedule, so results are bit-identical with or without it.
-#include <stdlib.h>
 #include <cuda_bf16.h>
 #include "common.cuh"
 #include "tc.cuh"
-
-extern long long* g_dbgbuf;          // spconv_tc.cu: clock-trace buffer (dz_debug_trace), NULL in normal runs
-extern bool g_trace_on;
 
 namespace {
 
@@ -66,13 +62,6 @@ struct SbCfg {
     static constexpr int SMEM = STAGES * STAGE_BYTES + NBR_BYTES + MISC_BYTES + STG_BYTES + 1024;
 };
 
-__device__ __forceinline__ void cp_async16_zfill(uint32_t dst, const void* src, bool valid) {
-    const int sz = valid ? 16 : 0;
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(sz) : "memory");
-}
-__device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t* bar) {
-    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(tc::smem_u32(bar)) : "memory");
-}
 // bounded wait: a protocol bug turns into a trap (CUDA error) instead of a hung GPU
 __device__ __forceinline__ void mbar_wait_bounded(uint64_t* bar, uint32_t parity) {
     uint32_t spins = 0;
@@ -98,7 +87,7 @@ __global__ void __launch_bounds__(SbCfg<COUT, PLANES>::THREADS, 1)
 k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restrict__ in, const int32_t* __restrict__ tab, int K, int tab_rows,
               const int32_t* __restrict__ order, const int* __restrict__ d_n_out, int out_cap, const float* __restrict__ scale,
               const float* __restrict__ shift, const uint16_t* __restrict__ residual, int relu, uint16_t* __restrict__ out,
-              const int32_t* __restrict__ tab_tiles, long long* __restrict__ dbg) {
+              const int32_t* __restrict__ tab_tiles) {
     using Cfg = SbCfg<COUT, PLANES>;
     constexpr int S = Cfg::STAGES;
     const int n = min(*d_n_out, out_cap);
@@ -120,10 +109,6 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
     uint64_t* nbr_empty = nbr_full + 2;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const bool tr = dbg && blockIdx.x == 0;                            // clock trace of CTA 0 (dz_debug_trace)
-    long long tr_a = 0, tr_b = 0, tr_c = 0, tr_n = 0;                  // per-role wait / work accumulators
-    const long long tr_t0 = tr ? clock64() : 0;
-#define TR_WAIT(acc, stmt) do { if (tr) { const long long c0__ = clock64(); stmt; acc += clock64() - c0__; } else { stmt; } } while (0)
     const int ktot = K * CIN_PAD;
     const int nb_tot = (ktot + 63) / 64;
 
@@ -156,13 +141,12 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
                 if (tile * SB_ROWS >= n) continue;                       // capacity tile beyond the live rows
             }
             const int b = t & 1;
-            if (t >= 2) TR_WAIT(tr_a, mbar_wait_bounded(nbr_empty + b, (((t >> 1) - 1) & 1)));
+            if (t >= 2) mbar_wait_bounded(nbr_empty + b, (((t >> 1) - 1) & 1));
             int* nb_b = s_nbr + b * SB_NPLANES * SB_ROWS;
             if (end) {
                 if (lane == 0) s_blk[b * 64 + 62] = -1;
                 __syncwarp();
                 if (lane == 0) tc::mbar_arrive(nbr_full + b);
-                if (tr && lane == 0) { dbg[2048 + 0] = tr_a; dbg[2048 + 1] = t; dbg[2048 + 2] = clock64() - tr_t0; }
                 break;
             }
             unsigned mask = 0;
@@ -227,19 +211,15 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
         int g = 0;                                   // CTA-wide step counter (same sequence in every role)
         for (int t = 0;; ++t) {
             const int b = t & 1;
-            TR_WAIT(tr_a, mbar_wait_bounded(nbr_full + b, (t >> 1) & 1));
-            if (s_blk[b * 64 + 62] < 0) {
-                if (tr && pw == 0 && lane == 0) { dbg[2048 + 8] = tr_a; dbg[2048 + 9] = tr_b; dbg[2048 + 10] = tr_c; dbg[2048 + 11] = tr_n; }
-                break;
-            }
+            mbar_wait_bounded(nbr_full + b, (t >> 1) & 1);
+            if (s_blk[b * 64 + 62] < 0) break;
             const int nb = s_blk[b * 64 + 63];
             const int* nb_b = s_nbr + b * SB_NPLANES * SB_ROWS;
             for (int i = 0; i < nb; ++i) {
                 const int gi = g + i;
                 const int my_s = gi % S;
                 const int kb = s_blk[b * 64 + i];
-                TR_WAIT(tr_b, mbar_wait_bounded(empty + my_s, ((gi / S) & 1) ^ 1));
-                const long long tr_i0 = tr ? clock64() : 0;
+                mbar_wait_bounded(empty + my_s, ((gi / S) & 1) ^ 1);
                 const uint32_t sa_u = smem_u + (uint32_t)(my_s * Cfg::STAGE_BYTES);
                 if (pw == 0 && lane == 0) {
                     tc::mbar_arrive_expect_tx(landed + my_s, Cfg::W_BYTES);
@@ -264,11 +244,10 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
                         const uint16_t* src = ok ? in_c + (size_t)src_row * (PLANES * CIN_PAD) : in;
 #pragma unroll
                         for (int p = 0; p < PLANES; ++p)
-                            cp_async16_zfill(dst + p * SB_A_BYTES, src + (ok ? p * CIN_PAD : 0), ok);
+                            tc::cp_async16_zfill(dst + p * SB_A_BYTES, src + (ok ? p * CIN_PAD : 0), ok);
                     }
                 }
-                cp_async_mbar_arrive_noinc(landed + my_s);           // asynchronous: arrives when this thread's copies have landed
-                if (tr) { tr_c += clock64() - tr_i0; ++tr_n; }
+                tc::cp_async_mbar_arrive_noinc(landed + my_s);       // asynchronous: arrives when this thread's copies have landed
             }
             g += nb;
             __syncwarp();
@@ -300,11 +279,8 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
         int g = 0;
         for (int t = 0;; ++t) {
             const int b = t & 1;
-            TR_WAIT(tr_a, mbar_wait_bounded(nbr_full + b, (t >> 1) & 1));
-            if (s_blk[b * 64 + 62] < 0) {
-                if (tr && threadIdx.x == 0) { dbg[2048 + 24] = tr_a; dbg[2048 + 25] = tr_b; dbg[2048 + 26] = tr_c; dbg[2048 + 27] = t; }
-                break;
-            }
+            mbar_wait_bounded(nbr_full + b, (t >> 1) & 1);
+            if (s_blk[b * 64 + 62] < 0) break;
             const int nb = s_blk[b * 64 + 63];
             const int r = warp < 4 ? s_nbr[b * SB_NPLANES * SB_ROWS + K * SB_ROWS + threadIdx.x] : -1;
             __syncwarp();
@@ -314,7 +290,7 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
             for (int i = 0; i < COUT / 2; ++i) acc[i] = 0.f;
             for (int i = 0; i < nb; ++i, ++g) {
                 const int s = g % S;
-                TR_WAIT(tr_b, mbar_wait_bounded(full + s, (g / S) & 1));
+                mbar_wait_bounded(full + s, (g / S) & 1);
                 // (the generic->async proxy fence is executed by the fence warp before it arrives)
                 const uint32_t sa = smem_u + (uint32_t)(s * Cfg::STAGE_BYTES) + cg * 64 * 128;
                 const uint32_t sw = smem_u + (uint32_t)(s * Cfg::STAGE_BYTES + PLANES * SB_A_BYTES);
@@ -338,7 +314,6 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
             tc::wgmma_wait_all();
             __syncwarp();
             if (lane == 0 && nb > 0) tc::mbar_arrive(empty + (g - 1) % S);
-            const long long tr_e0 = tr ? clock64() : 0;
 #pragma unroll
             for (int c0 = 0; c0 < COUT; c0 += CW) {
                 tc::named_sync(1, 32 * Cfg::CONSUMERS);             // the previous pass has read the staging tile
@@ -384,10 +359,8 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
                     }
                 }
             }
-            if (tr) tr_c += clock64() - tr_e0;
         }
     }
-#undef TR_WAIT
 }
 
 // ---- tensor-map cache: the weight matrix of a layer never moves, encode its map once ---------------------------------------
@@ -414,8 +387,6 @@ static const CUtensorMap* weight_map(const void* w, int rows, int ktot) {
     return m;
 }
 
-static int g_ctas = -1;
-
 template <int CIN_PAD, int COUT, int PLANES>
 int launch(const void* in, const int32_t* tab, int K, int tab_rows, const int32_t* order, const int* d_n_out, int out_cap, const void* weight,
            const float* scale, const float* shift, const void* residual, int relu, void* out, const int32_t* tab_tiles, cudaStream_t st) {
@@ -426,13 +397,12 @@ int launch(const void* in, const int32_t* tab, int K, int tab_rows, const int32_
         DZ_CUDA(cudaFuncSetAttribute(k_spconv_bf16<CIN_PAD, COUT, PLANES>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM));
         configured = true;
     }
-    if (g_ctas < 0) { const char* e = getenv("DZ_SPCONV_CTAS"); g_ctas = e ? atoi(e) : DZ_NUM_SMS; if (g_ctas < 1) g_ctas = DZ_NUM_SMS; }
     const CUtensorMap* tm = weight_map(weight, Cfg::WROWS, K * CIN_PAD);
     if (!tm) return DZ_ERR_CUDA;
-    const int grid = min(g_ctas, dz_cdiv(out_cap, SB_ROWS));
+    const int grid = min(DZ_NUM_SMS, dz_cdiv(out_cap, SB_ROWS));
     k_spconv_bf16<CIN_PAD, COUT, PLANES><<<grid, Cfg::THREADS, Cfg::SMEM, st>>>(
         *tm, (const uint16_t*)in, tab, K, tab_rows, order, d_n_out, out_cap, scale, shift, (const uint16_t*)residual, relu, (uint16_t*)out,
-        order ? tab_tiles : nullptr, g_trace_on ? g_dbgbuf : nullptr);
+        order ? tab_tiles : nullptr);
     DZ_LAUNCH_CHECK();
     return DZ_OK;
 }

@@ -1,22 +1,31 @@
 // spconv_tc.cu -- sparse convolution forward on the Hopper tensor cores (wgmma, TF32 operands, fp32 register accumulators).
 //
 // Same contract as the exact-fp32 kernel in spconv.cu (SubMConv3d / SparseConv3d + folded BatchNorm1d + bias + residual
-// + ReLU, backbone3d.py:64-83,105-121) for DZ_TF32.  spconv's own default keeps TF32 off (SURVEY A.4), so this mode
-// is opt-in (COMPUTE_MODE: tf32) with a stated 2e-3 tolerance.
+// + ReLU, backbone3d.py:64-83,105-121) for two modes:
+//   DZ_TF32   one TF32 pass.  spconv's own default keeps TF32 off (SURVEY A.4), so this mode is opt-in
+//             (COMPUTE_MODE: tf32) with a stated 2e-3 tolerance.
+//   DZ_TF32X3 fp32-level accuracy ("3xTF32" split): every fp32 operand is split into two TF32 pieces, x = x_hi + x_lo
+//             (x_hi = RN_tf32(x), x_lo = RN_tf32(x - x_hi)), and the product is accumulated in fp32 registers as
+//                 A_lo*W_hi + A_hi*W_lo + A_hi*W_hi          (the dropped A_lo*W_lo term is ~2^-22 relative)
+//             which reproduces fp32 FMA results to ~1e-6 relative (tests: <= 1e-5, the bar for the fp32-exact mode,
+//             SURVEY §8c).  Three MMAs per k-step instead of one: the kernel is bound by the gather, not the tensor pipe.
 //
 // Design: output-stationary implicit GEMM.  A CTA owns 128 output rows -- the rows order[p] of one tile of the rulebook's
 // tile schedule (rows with alike neighbour masks, csrc/rulebook.cu), tiles taken heaviest-first -- and reads their
 // neighbour lists from the row-major table (one 128-byte line per row).  The reduction dimension is the concatenation
 // (kernel offset k, input channel c) of length K*Cin, cut into 32-float (128-byte) blocks -- for Cin = 16 one block spans
 // two offsets, for Cin = 64 an offset spans two blocks -- so narrow layers still fill the MMA K dimension.  Blocks whose
-// offsets no row of the tile uses are skipped (that is what the schedule maximises).  Per block, the producer warps (PW
-// per pipeline stage) gather the neighbour rows straight from global/L2 into shared memory with cp.async (zero-fill for
-// missing neighbours) in the canonical K-major 128B-swizzled layout, one thread TMA-loads the matching W[cout][k-block]
-// tile, and two consumer warpgroups (64 rows each) issue wgmma (M=64, N=Cout, K=8) into register accumulators.  After the
-// last block the accumulators go through the (then idle) pipeline buffers and warps 0-3 run the epilogue, one row per
-// thread: scale/shift (+residual) -> ReLU -> 128-bit stores to row order[p].  No atomics: deterministic, and bit-identical
-// with or without a schedule (a row's accumulation order over k never changes).
-#include <stdlib.h>
+// offsets no row of the tile uses are skipped (that is what the schedule maximises).  Per block, producer warps gather the
+// neighbour rows into shared memory in the canonical K-major 128B-swizzled layout, one thread TMA-loads the matching
+// W[cout][k-block] tile(s), and two consumer warpgroups (64 rows each) issue wgmma (M=64, N=Cout, K=8) into register
+// accumulators.  The gather differs by mode:
+//   tf32   two warps per stage, cp.async straight from global/L2 (zero-fill for missing neighbours); the copies arrive on
+//          the stage's barrier asynchronously and the consumers fence the generic -> async proxy after their wait.
+//   tf32x3 one warp per stage, through registers: LDG.128 -> hi/lo split -> two swizzled STS.128 (A_hi, A_lo tiles), then a
+//          proxy fence and the arrive.  The weights are pre-split on the host and arrive as two TMA tiles.
+// After the last block the accumulators go through the (then idle) pipeline buffers and warps 0-3 run the epilogue, one
+// row per thread: scale/shift (+residual) -> ReLU (-> RN_tf32 for tf32) -> 128-bit stores to row order[p].  No atomics:
+// deterministic, and bit-identical with or without a schedule (a row's accumulation order over k never changes).
 #include "common.cuh"
 #include "tc.cuh"
 
@@ -24,43 +33,38 @@ static constexpr int ST_ROWS = 128;
 static constexpr int ST_A_BYTES = ST_ROWS * 128;        // one 32-float block for 128 rows
 static constexpr int ST_KMAX = 27;
 
-template <int COUT, int PW>
+template <int COUT, bool SPLIT>
 struct StCfg {
+    static constexpr int PLANES = SPLIT ? 2 : 1;               // operand pieces: [A_hi | A_lo] and [W_hi | W_lo] under SPLIT
     static constexpr int W_BYTES = COUT * 128;
-    static constexpr int STAGE_BYTES = ST_A_BYTES + W_BYTES;
+    static constexpr int STAGE_BYTES = PLANES * (ST_A_BYTES + W_BYTES);
     // Cout = 128 only occurs with K = 3 (conv_out): few k-steps, so a shallow ring suffices
-    static constexpr int STAGES = COUT >= 128 ? 3 : 4;
+    static constexpr int STAGES = SPLIT ? 3 : (COUT >= 128 ? 3 : 4);
     // PW producer warps per stage: warp w gathers its 128/PW rows of the steps it = s, s+STAGES, ... into stage s = (w-8) % STAGES
-    // (one warp alone cannot keep enough cp.async gathers in flight); warps 0-7 are the two consumer
-    // warpgroups, warps 0-3 double as the epilogue
+    // (one warp alone cannot keep enough cp.async gathers in flight; the register gather of SPLIT keeps 8 loads per lane in
+    // flight itself); warps 0-7 are the two consumer warpgroups, warps 0-3 double as the epilogue
+    static constexpr int PW = SPLIT ? 1 : 2;
     static constexpr int PRODUCERS = STAGES * PW;
     static constexpr int CONSUMERS = 8;
     static constexpr int THREADS = 32 * (CONSUMERS + PRODUCERS);
+    static constexpr int MIN_BLOCKS = SPLIT ? 1 : 0;                // __launch_bounds__ minimum blocks per SM (0: unspecified)
     static constexpr int ACC_LD = COUT + 4;                    // row pitch of the accumulator tile staged for the epilogue
     static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 + ST_KMAX * ST_ROWS * 4 + 128 * 4 + 256;
     static_assert(ST_ROWS * ACC_LD * 4 <= STAGES * STAGE_BYTES, "accumulator staging must fit in the pipeline buffers");
 };
 
-__device__ __forceinline__ void cp_async16_zfill(uint32_t dst, const void* src, bool valid) {
-    int sz = valid ? 16 : 0;
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(sz) : "memory");
-}
-__device__ __forceinline__ void cp_async4_zfill(uint32_t dst, const void* src, bool valid) {
-    int sz = valid ? 4 : 0;
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(sz) : "memory");
-}
-__device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t* bar) {
-    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(tc::smem_u32(bar)) : "memory");
-}
+// weight tensor maps of one launch: [W] or [W_hi, W_lo]
+template <int PLANES>
+struct WeightMaps { CUtensorMap m[PLANES]; };
 
-template <int CIN_PAD, int COUT, int PW>
-__global__ void __launch_bounds__(StCfg<COUT, PW>::THREADS)
-k_spconv_tf32(const __grid_constant__ CUtensorMap tmW, const float* __restrict__ in, int cin, const int32_t* __restrict__ nbr, int K,
-              int nbr_cap, const int32_t* __restrict__ order, const int* __restrict__ d_n_out, int out_cap, const float* __restrict__ scale,
-              const float* __restrict__ shift, const float* __restrict__ residual, int relu, float* __restrict__ out, long long* __restrict__ dbgbuf) {
-    using Cfg = StCfg<COUT, PW>;
-    const bool tr = dbgbuf && blockIdx.x == 1;      // clock trace of CTA 1 (dz_debug_trace); dbgbuf is NULL in normal runs
-    if (tr && threadIdx.x == 0) dbgbuf[0] = clock64();
+template <int CIN_PAD, int COUT, bool SPLIT>
+__global__ void __launch_bounds__(StCfg<COUT, SPLIT>::THREADS, StCfg<COUT, SPLIT>::MIN_BLOCKS)
+k_spconv_tf32(const __grid_constant__ WeightMaps<StCfg<COUT, SPLIT>::PLANES> tmW, const float* __restrict__ in, int cin,
+              const int32_t* __restrict__ nbr, int K, int nbr_cap, const int32_t* __restrict__ order, const int* __restrict__ d_n_out,
+              int out_cap, const float* __restrict__ scale, const float* __restrict__ shift, const float* __restrict__ residual, int relu,
+              float* __restrict__ out) {
+    using Cfg = StCfg<COUT, SPLIT>;
+    constexpr int PLANES = Cfg::PLANES;
     const int n = min(*d_n_out, out_cap);
     // under a tile schedule CTAs take the tiles heaviest-first (launch order ~ blockIdx order): order[nbr_cap + i]
     const int row0 = (order ? __ldg(order + nbr_cap + blockIdx.x) : (int)blockIdx.x) * ST_ROWS;
@@ -80,8 +84,9 @@ k_spconv_tf32(const __grid_constant__ CUtensorMap tmW, const float* __restrict__
     const int nb_tot = (ktot + 31) / 32;
 
     if (threadIdx.x == 0) {
-        tc::prefetch_tmap(&tmW);
-        for (int s = 0; s < Cfg::STAGES; ++s) { tc::mbar_init(full + s, 32 * PW + 1); tc::mbar_init(empty + s, Cfg::CONSUMERS); }
+#pragma unroll
+        for (int p = 0; p < PLANES; ++p) tc::prefetch_tmap(&tmW.m[p]);
+        for (int s = 0; s < Cfg::STAGES; ++s) { tc::mbar_init(full + s, 32 * Cfg::PW + 1); tc::mbar_init(empty + s, Cfg::CONSUMERS); }
         tc::fence_barrier_init();
         *s_mask = 0u;
     }
@@ -126,57 +131,92 @@ k_spconv_tf32(const __grid_constant__ CUtensorMap tmW, const float* __restrict__
     }
     __syncthreads();
     const int nb = *s_nb;
-    if (tr && threadIdx.x == 0) { dbgbuf[1] = clock64(); dbgbuf[2] = nb; }
 
     if (warp >= Cfg::CONSUMERS) {
         // ================= producers: warp w fills rows [part*RPW, (part+1)*RPW) of stage s for the steps s, s+STAGES, ... ===
-        constexpr int RPW = ST_ROWS / PW;           // rows per producer warp
+        constexpr int RPW = ST_ROWS / Cfg::PW;      // rows per producer warp
         constexpr int RPL = RPW / 4;                // rows per 8-lane group
         const int j = lane & 7;                     // 16-byte chunk inside the 128-byte row
         const int rg = lane >> 3;                   // lane covers chunk j of rows rbase .. rbase+RPL-1
         const int s = (warp - Cfg::CONSUMERS) % Cfg::STAGES, part = (warp - Cfg::CONSUMERS) / Cfg::STAGES;
         const int rbase = part * RPW + rg * RPL;
         unsigned char* sa = smem + s * Cfg::STAGE_BYTES;
-        const uint32_t sa_u = tc::smem_u32(sa);
         for (int it = s, round = 0; it < nb; it += Cfg::STAGES, ++round) {
             const int kb = s_blocks[it];
-            if (tr && lane == 0 && part == 0 && it < 120) dbgbuf[8 + it * 8 + 0] = clock64();
             tc::mbar_wait(empty + s, (round & 1) ^ 1);
-            if (tr && lane == 0 && part == 0 && it < 120) dbgbuf[8 + it * 8 + 1] = clock64();
             if (part == 0 && lane == 0) {
-                tc::mbar_arrive_expect_tx(full + s, Cfg::W_BYTES);
-                tc::tma_load_2d(sa + ST_A_BYTES, &tmW, full + s, kb * 32, 0);
+                tc::mbar_arrive_expect_tx(full + s, PLANES * Cfg::W_BYTES);
+#pragma unroll
+                for (int p = 0; p < PLANES; ++p) tc::tma_load_2d(sa + PLANES * ST_A_BYTES + p * Cfg::W_BYTES, &tmW.m[p], full + s, kb * 32, 0);
             }
             const int kidx = kb * 32 + j * 4;       // position in the concatenated (offset, channel) dimension
             const int k = kidx / CIN_PAD, c = kidx % CIN_PAD;
             const bool k_ok = k < K;
             const int4* nb_k = reinterpret_cast<const int4*>(s_nbr + (k_ok ? k : 0) * ST_ROWS + rbase);
             const float* in_c = in + c;
+            if constexpr (!SPLIT) {
+                const uint32_t sa_u = tc::smem_u32(sa);
 #pragma unroll
-            for (int i0 = 0; i0 < RPL; i0 += 4) {
-                const int4 nq = nb_k[i0 / 4];
-                const int rows4[4] = {nq.x, nq.y, nq.z, nq.w};
+                for (int i0 = 0; i0 < RPL; i0 += 4) {
+                    const int4 nq = nb_k[i0 / 4];
+                    const int rows4[4] = {nq.x, nq.y, nq.z, nq.w};
 #pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int src_row = k_ok ? rows4[u] : -1;
-                    const int r = rbase + i0 + u;   // tile row: swizzle atom r/8, row-in-atom r%8
-                    const int rr = r & 7;
-                    const uint32_t dst = sa_u + (uint32_t)((r >> 3) * 1024 + rr * 128 + ((j ^ rr) << 4));
-                    if (CIN_PAD >= 16) {
-                        const bool ok = src_row >= 0;
-                        cp_async16_zfill(dst, ok ? (const void*)(in_c + (size_t)src_row * cin) : (const void*)in, ok);
-                    } else {
-                        // first layer (cin = 5 padded to 8): rows are not 16-byte aligned -> 4-byte copies
+                    for (int u = 0; u < 4; ++u) {
+                        const int src_row = k_ok ? rows4[u] : -1;
+                        const int r = rbase + i0 + u;   // tile row: swizzle atom r/8, row-in-atom r%8
+                        const int rr = r & 7;
+                        const uint32_t dst = sa_u + (uint32_t)((r >> 3) * 1024 + rr * 128 + ((j ^ rr) << 4));
+                        if (CIN_PAD >= 16) {
+                            const bool ok = src_row >= 0;
+                            tc::cp_async16_zfill(dst, ok ? (const void*)(in_c + (size_t)src_row * cin) : (const void*)in, ok);
+                        } else {
+                            // first layer (cin = 5 padded to 8): rows are not 16-byte aligned -> 4-byte copies
 #pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            const bool ok = src_row >= 0 && (c + e) < cin;
-                            cp_async4_zfill(dst + 4 * e, ok ? (const void*)(in_c + (size_t)src_row * cin + e) : (const void*)in, ok);
+                            for (int e = 0; e < 4; ++e) {
+                                const bool ok = src_row >= 0 && (c + e) < cin;
+                                tc::cp_async4_zfill(dst + 4 * e, ok ? (const void*)(in_c + (size_t)src_row * cin + e) : (const void*)in, ok);
+                            }
                         }
                     }
                 }
+                tc::cp_async_mbar_arrive_noinc(full + s);
+            } else {
+                unsigned char* sa_lo = sa + ST_A_BYTES;
+#pragma unroll 1
+                for (int i0 = 0; i0 < RPL; i0 += 8) {
+                    float4 v[8];
+                    const int4 n0 = nb_k[i0 / 4], n1 = nb_k[i0 / 4 + 1];
+                    const int rows8[8] = {n0.x, n0.y, n0.z, n0.w, n1.x, n1.y, n1.z, n1.w};
+#pragma unroll
+                    for (int u = 0; u < 8; ++u) {                       // 8 independent 128-bit loads in flight per lane
+                        const int src_row = k_ok ? rows8[u] : -1;
+                        v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+                        if (src_row >= 0) {
+                            if (CIN_PAD >= 16) v[u] = __ldg(reinterpret_cast<const float4*>(in_c + (size_t)src_row * cin));
+                            else {
+                                const float* p = in_c + (size_t)src_row * cin;     // cin = 5: unaligned rows, scalar loads
+                                if (c + 0 < cin) v[u].x = __ldg(p + 0);
+                                if (c + 1 < cin) v[u].y = __ldg(p + 1);
+                                if (c + 2 < cin) v[u].z = __ldg(p + 2);
+                                if (c + 3 < cin) v[u].w = __ldg(p + 3);
+                            }
+                        }
+                    }
+#pragma unroll
+                    for (int u = 0; u < 8; ++u) {
+                        // row r = rg*32 + i0 + u: 8-row group (r>>3) = rg*4 + i0/8, row in group = u
+                        const uint32_t off = (uint32_t)((rg * 4 + (i0 >> 3)) * 1024 + u * 128 + ((j ^ u) << 4));
+                        float4 hi, lo;
+                        hi.x = tc::rna_tf32(v[u].x); hi.y = tc::rna_tf32(v[u].y); hi.z = tc::rna_tf32(v[u].z); hi.w = tc::rna_tf32(v[u].w);
+                        lo.x = tc::rna_tf32(v[u].x - hi.x); lo.y = tc::rna_tf32(v[u].y - hi.y);      // RN (the tensor core would truncate)
+                        lo.z = tc::rna_tf32(v[u].z - hi.z); lo.w = tc::rna_tf32(v[u].w - hi.w);
+                        *reinterpret_cast<float4*>(sa + off) = hi;
+                        *reinterpret_cast<float4*>(sa_lo + off) = lo;
+                    }
+                }
+                tc::fence_proxy_async();                  // generic-proxy smem writes -> visible to the tensor core (async proxy)
+                tc::mbar_arrive(full + s);
             }
-            cp_async_mbar_arrive_noinc(full + s);
-            if (tr && lane == 0 && part == 0 && it < 120) dbgbuf[8 + it * 8 + 2] = clock64();
         }
     } else {
         // ================= consumers: warpgroup g accumulates rows [64g, 64g+64) of the tile =================
@@ -186,20 +226,29 @@ k_spconv_tf32(const __grid_constant__ CUtensorMap tmW, const float* __restrict__
         for (int i = 0; i < COUT / 2; ++i) acc[i] = 0.f;
         for (int it = 0; it < nb; ++it) {
             const int s = it % Cfg::STAGES;
-            if (tr && threadIdx.x == 0 && it < 120) dbgbuf[8 + it * 8 + 3] = clock64();
             tc::mbar_wait(full + s, (it / Cfg::STAGES) & 1);
-            if (tr && threadIdx.x == 0 && it < 120) dbgbuf[8 + it * 8 + 4] = clock64();
-            tc::fence_proxy_async();                // cp.async (generic proxy) writes -> tensor-core (async proxy) reads
-            const uint32_t sa = tc::smem_u32(smem + s * Cfg::STAGE_BYTES);
-            const uint64_t adesc = tc::smem_desc_sw128(sa + g * 64 * 128), bdesc = tc::smem_desc_sw128(sa + ST_A_BYTES);
+            if constexpr (!SPLIT) tc::fence_proxy_async();      // cp.async (generic proxy) writes -> tensor-core (async proxy) reads
+            const uint32_t sa = tc::smem_u32(smem + s * Cfg::STAGE_BYTES) + g * 64 * 128;
+            const uint32_t sw = tc::smem_u32(smem + s * Cfg::STAGE_BYTES) + PLANES * ST_A_BYTES;
+            const uint64_t a_hi = tc::smem_desc_sw128(sa), w_hi = tc::smem_desc_sw128(sw);
             tc::wgmma_fence();
+            if constexpr (!SPLIT) {
 #pragma unroll
-            for (int kk = 0; kk < 4; ++kk) tc::wgmma<COUT, tc::K_TF32>(acc, adesc + (uint64_t)(kk * 2), bdesc + (uint64_t)(kk * 2), 1u);
+                for (int kk = 0; kk < 4; ++kk) tc::wgmma<COUT, tc::K_TF32>(acc, a_hi + (uint64_t)(kk * 2), w_hi + (uint64_t)(kk * 2), 1u);
+            } else {
+                const uint64_t a_lo = tc::smem_desc_sw128(sa + ST_A_BYTES), w_lo = tc::smem_desc_sw128(sw + Cfg::W_BYTES);
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk) {
+                    const uint64_t o = (uint64_t)(kk * 2);
+                    tc::wgmma<COUT, tc::K_TF32>(acc, a_lo + o, w_hi + o, 1u);      // small terms first
+                    tc::wgmma<COUT, tc::K_TF32>(acc, a_hi + o, w_lo + o, 1u);
+                    tc::wgmma<COUT, tc::K_TF32>(acc, a_hi + o, w_hi + o, 1u);
+                }
+            }
             tc::wgmma_commit();
             tc::wgmma_wait_one();                       // this step's MMAs stay in flight; the previous step's stage is free
             __syncwarp();
             if (lane == 0 && it > 0) tc::mbar_arrive(empty + (it - 1) % Cfg::STAGES);
-            if (tr && threadIdx.x == 0 && it < 120) dbgbuf[8 + it * 8 + 5] = clock64();
         }
         tc::wgmma_wait_all();
         __syncwarp();
@@ -213,7 +262,6 @@ k_spconv_tf32(const __grid_constant__ CUtensorMap tmW, const float* __restrict__
             // ================= epilogue: thread = tile row =================
             const int pos = row0 + threadIdx.x;     // tile position; the output row is order[pos] under a tile schedule
             const int r = pos < n ? (order ? __ldg(order + pos) : pos) : n;
-            if (tr && threadIdx.x == 0) dbgbuf[3] = clock64();
 #pragma unroll 1
             for (int c0 = 0; c0 < COUT; c0 += 32) {
                 float v[32];
@@ -232,86 +280,67 @@ k_spconv_tf32(const __grid_constant__ CUtensorMap tmW, const float* __restrict__
                             o.x += rr.x; o.y += rr.y; o.z += rr.z; o.w += rr.w;
                         }
                         if (relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-                        // round-to-nearest to TF32: the next layer's truncating tensor-core read is then exact (no toward-zero bias)
-                        o.x = tc::rna_tf32(o.x); o.y = tc::rna_tf32(o.y); o.z = tc::rna_tf32(o.z); o.w = tc::rna_tf32(o.w);
+                        if constexpr (!SPLIT) {
+                            // round-to-nearest to TF32: the next layer's truncating tensor-core read is then exact (no toward-zero bias)
+                            o.x = tc::rna_tf32(o.x); o.y = tc::rna_tf32(o.y); o.z = tc::rna_tf32(o.z); o.w = tc::rna_tf32(o.w);
+                        }
                         *reinterpret_cast<float4*>(out + (size_t)r * COUT + ch) = o;
                     }
                 }
             }
         }
     }
-    if (tr && threadIdx.x == 0) dbgbuf[4] = clock64();
 }
 
-long long* g_dbgbuf = nullptr;          // shared with spconv_bf16.cu (clock traces, dz_debug_trace)
-bool g_trace_on = false;
-extern "C" int dz_debug_trace(long long* host, int n) {      // clock-trace helper (not part of the public header)
-    if (!g_dbgbuf) { if (cudaMalloc(&g_dbgbuf, 4096 * 8) != cudaSuccess) return -1; cudaMemset(g_dbgbuf, 0, 4096 * 8); g_trace_on = true; return 1; }
-    cudaDeviceSynchronize();
-    return cudaMemcpy(host, g_dbgbuf, (size_t)n * 8, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -1;
-}
-
-template <int CIN_PAD, int COUT, int PW>
-static int launch_pw(const CUtensorMap& tmW, const float* in, int cin, const int32_t* nbr, int K, int nbr_cap, const int32_t* order, const int* d_n_out,
-                     int out_cap, const float* scale, const float* shift, const float* residual, int relu, float* out, cudaStream_t st) {
-    using Cfg = StCfg<COUT, PW>;
+// weight layout: tf32 (cout, K*cin_pad) row-major, cin_pad = 8 for cin <= 8 else cin; tf32x3 (2, cout, K*cin_pad):
+// [0] = RN_tf32(W), [1] = RN_tf32(W - W_hi).
+// (A TMA tile::gather4 producer was built and measured 1.6x slower than the cp.async gather for 128-byte rows -- the TMA unit
+// has a per-row cost -- and a hybrid LSU+TMA split gave no gain.  Both were removed.)
+template <int CIN_PAD, int COUT, bool SPLIT>
+static int launch(const float* in, int cin, const int32_t* nbr, int K, int nbr_cap, const int32_t* order, const int* d_n_out, int out_cap,
+                  const float* weight, const float* scale, const float* shift, const float* residual, int relu, float* out, cudaStream_t st) {
+    using Cfg = StCfg<COUT, SPLIT>;
+    tc::EncodeTiledFn enc = tc::get_encode_tiled();
+    if (!enc) { dz_set_error("cuTensorMapEncodeTiled unavailable"); return DZ_ERR_CUDA; }
+    WeightMaps<Cfg::PLANES> tm;
+    const cuuint64_t ktot = (cuuint64_t)K * CIN_PAD;
+    for (int p = 0; p < Cfg::PLANES; ++p) {
+        cuuint64_t dims[2] = {ktot, (cuuint64_t)COUT};
+        cuuint64_t strides[1] = {ktot * 4};
+        cuuint32_t box[2] = {32, (cuuint32_t)COUT};
+        cuuint32_t estr[2] = {1, 1};
+        CUresult r = enc(&tm.m[p], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)(weight + (size_t)p * COUT * ktot), dims, strides, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        if (r != CUDA_SUCCESS) { dz_set_error("cuTensorMapEncodeTiled(W) failed: %d", (int)r); return DZ_ERR_CUDA; }
+    }
     static bool configured = false;
     if (!configured) {
-        DZ_CUDA(cudaFuncSetAttribute(k_spconv_tf32<CIN_PAD, COUT, PW>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM));
+        DZ_CUDA(cudaFuncSetAttribute(k_spconv_tf32<CIN_PAD, COUT, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM));
         configured = true;
     }
-    k_spconv_tf32<CIN_PAD, COUT, PW><<<dz_cdiv(out_cap, ST_ROWS), Cfg::THREADS, Cfg::SMEM, st>>>(tmW, in, cin, nbr, K, nbr_cap, order, d_n_out, out_cap,
-                                                                                             scale, shift, residual, relu, out, g_trace_on ? g_dbgbuf : nullptr);
+    k_spconv_tf32<CIN_PAD, COUT, SPLIT><<<dz_cdiv(out_cap, ST_ROWS), Cfg::THREADS, Cfg::SMEM, st>>>(tm, in, cin, nbr, K, nbr_cap, order, d_n_out,
+                                                                                                  out_cap, scale, shift, residual, relu, out);
     DZ_LAUNCH_CHECK();
     return DZ_OK;
 }
 
-template <int CIN_PAD, int COUT>
-static int launch(const CUtensorMap& tmW, const float* in, int cin, int in_rows, const int32_t* nbr, int K, int nbr_cap, const int32_t* order, const int* d_n_out,
-                  int out_cap, const float* scale, const float* shift, const float* residual, int relu, float* out, cudaStream_t st) {
-    (void)in_rows;
-    static const int pw = getenv("DZ_SPCONV_PW") ? atoi(getenv("DZ_SPCONV_PW")) : 2;
-    if (pw == 1) return launch_pw<CIN_PAD, COUT, 1>(tmW, in, cin, nbr, K, nbr_cap, order, d_n_out, out_cap, scale, shift, residual, relu, out, st);
-    return launch_pw<CIN_PAD, COUT, 2>(tmW, in, cin, nbr, K, nbr_cap, order, d_n_out, out_cap, scale, shift, residual, relu, out, st);
-}
-
-// weight layout for this path: (cout, K * cin_pad) row-major, cin_pad = 8 for cin <= 8 else cin.
-// (A TMA tile::gather4 producer was built and measured 1.6x slower than the cp.async gather for 128-byte rows -- the TMA unit
-// has a per-row cost -- and a hybrid LSU+TMA split gave no gain.  Both were removed.)
-int dz_spconv_fwd_tc3(const float* in, int cin, const int32_t* nbr, int K, int nbr_cap, const int32_t* order, const int* d_n_out, int out_cap,
-                      const float* weight, const float* scale, const float* shift, const float* residual, int relu, float* out,
-                      int cout, cudaStream_t st);
-
 int dz_spconv_fwd_tc(const float* in, int cin, int in_rows, const int32_t* nbr, int K, int nbr_cap, const int32_t* order, const int* d_n_out, int out_cap,
                      const float* weight, const float* scale, const float* shift, const float* residual, int relu, float* out,
                      int cout, int mode, cudaStream_t st) {
-    if (mode == DZ_TF32X3) return dz_spconv_fwd_tc3(in, cin, nbr, K, nbr_cap, order, d_n_out, out_cap, weight, scale, shift, residual, relu, out, cout, st);
-    if (mode != DZ_TF32) { dz_set_error("dz_spconv_fwd: tensor-core mode %d not built (tf32 only)", mode); return DZ_ERR_UNSUPPORTED; }
-    if (K > ST_KMAX) { dz_set_error("dz_spconv_fwd(tf32): K=%d > 27", K); return DZ_ERR_UNSUPPORTED; }
+    (void)in_rows;
+    if (mode != DZ_TF32 && mode != DZ_TF32X3) { dz_set_error("dz_spconv_fwd: tensor-core mode %d not built (tf32, tf32x3)", mode); return DZ_ERR_UNSUPPORTED; }
+    const bool split = mode == DZ_TF32X3;
+    const char* name = split ? "tf32x3" : "tf32";
+    if (K > ST_KMAX) { dz_set_error("dz_spconv_fwd(%s): K=%d > 27", name, K); return DZ_ERR_UNSUPPORTED; }
     const int cin_pad = cin <= 8 ? 8 : cin;
-    tc::EncodeTiledFn enc = tc::get_encode_tiled();
-    if (!enc) { dz_set_error("cuTensorMapEncodeTiled unavailable"); return DZ_ERR_CUDA; }
-    CUtensorMap tmW;
-    {
-        cuuint64_t ktot = (cuuint64_t)K * cin_pad;
-        cuuint64_t dims[2] = {ktot, (cuuint64_t)cout};
-        cuuint64_t strides[1] = {ktot * 4};
-        cuuint32_t box[2] = {32, (cuuint32_t)cout};
-        cuuint32_t estr[2] = {1, 1};
-        CUresult r = enc(&tmW, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)weight, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) { dz_set_error("cuTensorMapEncodeTiled(W) failed: %d", (int)r); return DZ_ERR_CUDA; }
+#define DZ_ST(CP, CO)                                                                                                                       \
+    if (cin_pad == CP && cout == CO) {                                                                                                      \
+        if (split) return launch<CP, CO, true>(in, cin, nbr, K, nbr_cap, order, d_n_out, out_cap, weight, scale, shift, residual, relu, out, st); \
+        return launch<CP, CO, false>(in, cin, nbr, K, nbr_cap, order, d_n_out, out_cap, weight, scale, shift, residual, relu, out, st);     \
     }
-#define DZ_ST(CP, CO) return launch<CP, CO>(tmW, in, cin, in_rows, nbr, K, nbr_cap, order, d_n_out, out_cap, scale, shift, residual, relu, out, st)
-    if (cin_pad == 8 && cout == 16) DZ_ST(8, 16);
-    if (cin_pad == 16 && cout == 16) DZ_ST(16, 16);
-    if (cin_pad == 16 && cout == 32) DZ_ST(16, 32);
-    if (cin_pad == 32 && cout == 32) DZ_ST(32, 32);
-    if (cin_pad == 32 && cout == 64) DZ_ST(32, 64);
-    if (cin_pad == 64 && cout == 64) DZ_ST(64, 64);
-    if (cin_pad == 64 && cout == 128) DZ_ST(64, 128);
-    if (cin_pad == 128 && cout == 128) DZ_ST(128, 128);
+    DZ_ST(8, 16) DZ_ST(16, 16) DZ_ST(16, 32) DZ_ST(32, 32) DZ_ST(32, 64) DZ_ST(64, 64) DZ_ST(64, 128) DZ_ST(128, 128)
 #undef DZ_ST
-    dz_set_error("dz_spconv_fwd(tf32): (cin=%d, cout=%d) not instantiated", cin, cout);
+    dz_set_error("dz_spconv_fwd(%s): (cin=%d, cout=%d) not instantiated", name, cin, cout);
     return DZ_ERR_UNSUPPORTED;
 }

@@ -38,6 +38,21 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 // (a one-lane poll with __nanosleep back-off for the long waits was measured: no change for the dense conv, 20 % slower
 // sparse conv -- the wake-up latency of the producers matters more than the polling traffic)
 
+// ---- cp.async (LSU gathers into shared memory) ------------------------------------------------------------------
+// 16- / 4-byte copies that write zeros instead when !valid (src must still be a mapped address)
+__device__ __forceinline__ void cp_async16_zfill(uint32_t dst, const void* src, bool valid) {
+    const int sz = valid ? 16 : 0;
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(sz) : "memory");
+}
+__device__ __forceinline__ void cp_async4_zfill(uint32_t dst, const void* src, bool valid) {
+    const int sz = valid ? 4 : 0;
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(sz) : "memory");
+}
+// arrive on `bar` once this thread's outstanding cp.async copies have landed (without raising its expected count)
+__device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint64_t* bar) {
+    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+
 // ---- TMA ----------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");

@@ -164,37 +164,36 @@ def new_sched_ws(cap, device):
     return torch.empty(int(lib().dz_rulebook_schedule_ws_bytes(cap)), dtype=torch.uint8, device=device)
 
 
-def rulebook_subm(coords, d_n, cap, index, ksize, layout='k', sched_ws=None, frame_major=False):
+def rulebook_subm(coords, d_n, cap, index, ksize, layout='k', sched_ws=None):
     """layout 'k': k-major (K, cap) table (exact-fp32 kernel, parity tests); 'row': row-major (cap, 32) table for the
     tensor-core kernels; 'both': (nbr, tab).  sched_ws (row/both only): also leave the tile-schedule digests there."""
     K = ksize[0] * ksize[1] * ksize[2]
     nbr = torch.empty((K, cap), dtype=torch.int32, device=coords.device) if layout in ('k', 'both') else None
     tab = torch.empty((cap, 32), dtype=torch.int32, device=coords.device) if layout in ('row', 'both') else None
     check(lib().dz_rulebook_subm(_p(coords), _p(d_n), cap, index.B, *index.dhw, iarr(ksize), _p(index.bitmap),
-                                 _p(index.prefix), _p(index.perm), _p(nbr), _p(tab), _p(sched_ws), int(bool(frame_major)), _stream()),
+                                 _p(index.prefix), _p(index.perm), _p(nbr), _p(tab), _p(sched_ws), _stream()),
           'rulebook_subm')
     _count(1 if sched_ws is None else 2)
     return nbr if layout == 'k' else tab if layout == 'row' else (nbr, tab)
 
 
-def rulebook_schedule(tab, d_n, sched_ws, B=1, frame_major=False, K=None):
+def rulebook_schedule(tab, d_n, sched_ws, K=None):
     """tile schedule for the tensor-core conv from the scratch the rulebook call filled: returns `order`
-    (cap + ceil(cap/128),) = row order | tile launch order; see dz_rulebook_schedule.  frame_major (same value as in the
-    rulebook call): rows sorted by (frame, mask), tiles ordered frame by frame"""
+    (cap + ceil(cap/128),) = row order | tile launch order; see dz_rulebook_schedule"""
     _need_cuda(tab)
     cap = tab.shape[0]
     tiles = (cap + 127) // 128
     if K is None:                                       # row order | tile order
         order = torch.empty(cap + tiles, dtype=torch.int32, device=tab.device)
-        check(lib().dz_rulebook_schedule(_p(tab), cap, _p(d_n), _p(order), _p(sched_ws), sched_ws.numel(), int(B), int(bool(frame_major)),
-                                         0, None, _stream()), 'rulebook_schedule')
+        check(lib().dz_rulebook_schedule(_p(tab), cap, _p(d_n), _p(order), _p(sched_ws), sched_ws.numel(), 0, None, _stream()),
+              'rulebook_schedule')
         _count(1)
         return order
     # K given: also the TILE-major table (tiles, K+1, 128) for the persistent bf16-plane conv; order gets the tile masks appended
     order = torch.empty(cap + 2 * tiles, dtype=torch.int32, device=tab.device)
     tab_tiles = torch.empty((tiles, int(K) + 1, 128), dtype=torch.int32, device=tab.device)
-    check(lib().dz_rulebook_schedule(_p(tab), cap, _p(d_n), _p(order), _p(sched_ws), sched_ws.numel(), int(B), int(bool(frame_major)),
-                                     int(K), _p(tab_tiles), _stream()), 'rulebook_schedule')
+    check(lib().dz_rulebook_schedule(_p(tab), cap, _p(d_n), _p(order), _p(sched_ws), sched_ws.numel(), int(K), _p(tab_tiles), _stream()),
+          'rulebook_schedule')
     _count(2)
     return order, tab_tiles
 
@@ -214,7 +213,7 @@ def conv_out_dhw(in_dhw, ksize, stride, pad):
     return [(in_dhw[d] + 2 * pad[d] - (ksize[d] - 1) - 1) // stride[d] + 1 for d in range(3)]
 
 
-def rulebook_conv(coords, d_n, in_cap, in_index, ksize, stride, pad, out_cap, layout='k', sched_ws=None, frame_major=False):
+def rulebook_conv(coords, d_n, in_cap, in_index, ksize, stride, pad, out_cap, layout='k', sched_ws=None):
     dev = coords.device
     out_dhw = conv_out_dhw(in_index.dhw, ksize, stride, pad)
     out_index = GridIndex(in_index.B, out_dhw, dev)
@@ -227,7 +226,7 @@ def rulebook_conv(coords, d_n, in_cap, in_index, ksize, stride, pad, out_cap, la
     check(lib().dz_rulebook_conv(_p(coords), _p(d_n), in_cap, in_index.B, iarr(in_index.dhw), iarr(ksize), iarr(stride),
                                  iarr(pad), _p(in_index.bitmap), _p(in_index.prefix), _p(in_index.perm), _p(out_coords),
                                  _p(d_n_out), out_cap, _p(out_index.bitmap), _p(out_index.prefix), _p(nbr), _p(tab), _p(ws),
-                                 ws.numel(), _p(sched_ws), int(bool(frame_major)), _stream()), 'rulebook_conv')
+                                 ws.numel(), _p(sched_ws), _stream()), 'rulebook_conv')
     _count(6 if sched_ws is None else 7)
     return out_coords, d_n_out, out_index, (nbr if layout == 'k' else tab if layout == 'row' else (nbr, tab)), out_dhw
 

@@ -14,8 +14,6 @@ Differences from spconv (behaviour-preserving):
     strided-conv output sites are emitted sorted by (b,z,y,x) (spconv's order is implementation-defined)
   * in eval mode ``SparseSequential`` fuses conv + BatchNorm1d + ReLU (+ residual) into one launch.
 """
-import os
-
 import torch
 import torch.nn as nn
 
@@ -218,8 +216,6 @@ class _SparseConv(SparseModule):
     CAP_HEADROOM = 1.3
     #: build a tile schedule (rows grouped by neighbour mask) with every rulebook used by a tensor-core layer
     SCHEDULE_TILES = True
-    #: batches: sort the schedule by (frame, mask) so that the tiles in flight gather from ONE frame's (L2-resident) feature map
-    FRAME_MAJOR = bool(os.environ.get('DZ_FRAME_MAJOR'))      # the 3 digest bits it costs outweigh the L2 gain
 
     def __init__(self, in_channels, out_channels, kernel_size, stride=1, padding=0, dilation=1, groups=1, bias=True,
                  indice_key=None, subm=False, algo=None, mode='fp32'):
@@ -255,11 +251,9 @@ class _SparseConv(SparseModule):
             tc = _lib.MODES[self.mode] != _lib.DZ_F32
             layout = 'row' if tc else 'k'
             want = self._wants_schedule()
-            fm = self.FRAME_MAJOR and x.batch_size > 1
             if self.subm:
                 sws = ops.new_sched_ws(x._cap, x._idx.device) if want else None
-                t = ops.rulebook_subm(x._idx, x._count, x._cap, x.grid_index(), self.kernel_size, layout=layout, sched_ws=sws,
-                                      frame_major=fm)
+                t = ops.rulebook_subm(x._idx, x._count, x._cap, x.grid_index(), self.kernel_size, layout=layout, sched_ws=sws)
                 rule = _RuleSubm(None if tc else t, t if tc else None)
             else:
                 in_index = x.grid_index()
@@ -277,10 +271,9 @@ class _SparseConv(SparseModule):
                     out_cap = int(min(cells, max(128, (int(hint * self.CAP_HEADROOM) + 127) // 128 * 128)))
                 sws = ops.new_sched_ws(out_cap, x._idx.device) if want else None
                 oc, d_n_out, out_index, t, odhw = ops.rulebook_conv(x._idx, x._count, x._cap, in_index, self.kernel_size, self.stride,
-                                                                    self.padding, out_cap, layout=layout, sched_ws=sws, frame_major=fm)
+                                                                    self.padding, out_cap, layout=layout, sched_ws=sws)
                 rule = _RuleConv(oc, d_n_out, out_index, (None, t) if tc else (t, None), odhw, out_cap)
             rule.sched_ws = sws
-            rule.frame_major = fm
             rule.in_idx, rule.in_count, rule.in_cap, rule.in_dhw, rule.in_index = x._idx, x._count, x._cap, x.spatial_shape, x._index
             if key is not None:
                 x.indice_dict[key] = rule
@@ -296,11 +289,10 @@ class _SparseConv(SparseModule):
         """tile schedule of a rulebook (once per rulebook; only the tensor-core kernels use it)"""
         if rule.order is None and rule.sched_ws is not None:
             d_n = x._count if self.subm else rule.d_n_out
-            fm = getattr(rule, 'frame_major', False)
             if _lib.MODES[self.mode] in _lib.PLANES:        # persistent kernel: also the tile-major table (one bulk copy per tile)
-                rule.order, rule.tab_tiles = ops.rulebook_schedule(rule.tab, d_n, rule.sched_ws, x.batch_size, fm, K=self.kshape[0])
+                rule.order, rule.tab_tiles = ops.rulebook_schedule(rule.tab, d_n, rule.sched_ws, K=self.kshape[0])
             else:
-                rule.order = ops.rulebook_schedule(rule.tab, d_n, rule.sched_ws, x.batch_size, fm)
+                rule.order = ops.rulebook_schedule(rule.tab, d_n, rule.sched_ws)
 
     def _table(self, rule):
         """(table, row_order) for this layer's kernel"""

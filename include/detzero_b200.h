@@ -107,8 +107,7 @@ int dz_voxelize_dynamic_mean(const float* points, int n, int c, int B,
  * dz_rulebook_schedule needs (mask digests, scanned histogram) there. */
 int dz_rulebook_subm(const int32_t* coords, const int* d_n, int cap, int B, int D, int H, int W,
                      const int* ksize3_host, const uint32_t* bitmap, const uint32_t* prefix,
-                     const int32_t* perm, int32_t* nbr, int32_t* tab, void* sched_ws, int sched_frame_major,
-                     dz_stream_t stream);
+                     const int32_t* perm, int32_t* nbr, int32_t* tab, void* sched_ws, dz_stream_t stream);
 /* Strided conv: generates the output site set (sorted ascending (b,z,y,x)), its grid index and the table(s).
  * out_bitmap must be zero on entry. */
 int dz_rulebook_conv(const int32_t* in_coords, const int* d_n_in, int in_cap, int B,
@@ -116,18 +115,15 @@ int dz_rulebook_conv(const int32_t* in_coords, const int* d_n_in, int in_cap, in
                      const int* pad3_host, const uint32_t* in_bitmap, const uint32_t* in_prefix,
                      const int32_t* in_perm, int32_t* out_coords, int* d_n_out, int out_cap,
                      uint32_t* out_bitmap, uint32_t* out_prefix, int32_t* nbr, int32_t* tab,
-                     void* ws, size_t ws_bytes, void* sched_ws, int sched_frame_major, dz_stream_t stream);
+                     void* ws, size_t ws_bytes, void* sched_ws, dz_stream_t stream);
 /* Tile schedule for the tensor-core conv (no reference counterpart; spconv's implicit-GEMM "mask sort" plays the same
  * role).  order (cap + ceil(cap/128) ints): order[p] = output row at tile position p -- rows with alike neighbour
  * masks become adjacent, so a 128-row tile skips the kernel offsets none of its rows uses -- and order[cap + j] = the
- * tile the j-th CTA takes (most live offsets first).  Hand it to dz_spconv_fwd as row_order; results are bit-identical
- * to the unscheduled call.  sched_ws must be the one the rulebook call filled for this tab.
- * sched_frame_major (same value in the rulebook call and here; B = frames in the batch): sort by (frame, mask) and order the
- * tiles frame by frame (heaviest first inside a frame), so that the rows the CTAs gather at any moment belong to ONE frame's
- * feature map and stay L2-resident at batch sizes whose level no longer fits L2. */
+ * tile the j-th CTA takes (most live offsets first, capacity tiles beyond the count last).  Hand it to dz_spconv_fwd as
+ * row_order; results are bit-identical to the unscheduled call.  sched_ws must be the one the rulebook call filled for this tab. */
 size_t dz_rulebook_schedule_ws_bytes(int cap);
 int dz_rulebook_schedule(const int32_t* tab, int cap, const int* d_n, int32_t* order, void* sched_ws,
-                         size_t ws_bytes, int B, int sched_frame_major, int K, int32_t* tab_tiles, dz_stream_t stream);
+                         size_t ws_bytes, int K, int32_t* tab_tiles, dz_stream_t stream);
 /* tab_tiles (optional; ceil(cap/128) * (K+1) * 128 ints): the scheduled table again, TILE-major: tile j = (K+1) planes of 128
  * ints, plane k < K = neighbour row of tile position p through offset k, plane K = the output row order[j*128+p] (-1 beyond the
  * count).  With it `order` must have cap + 2*ceil(cap/128) ints: order[cap + tiles + j] = OR of tile j's row masks.  The
@@ -137,9 +133,10 @@ int dz_rulebook_schedule(const int32_t* tab, int cap, const int* d_n, int32_t* o
 /* out[o,:] = act( (sum_k in[nbr[k][o],:] @ W[k]) * scale + shift (+ residual[o,:]) )
  * Replaces SubMConv3d/SparseConv3d forward + BatchNorm1d(eval) + bias + residual add + ReLU
  * (backbone3d.py:64-83,105-121).  weight packed (K, cin, cout) f32 (host side repacks spconv's
- * (cout,KD,KH,KW,cin) layout, SURVEY A.3; DZ_TF32 expects (cout, K*cin_pad)).  in_rows = allocated rows of `in`
- * (bounds the TMA gather).  mode: DZ_F32 exact-fp32 FMA (nbr = k-major table), DZ_TF32 / DZ_TF32X3 wgmma tensor
- * cores (nbr = ROW-major table `tab`, nbr_cap = its rows).
+ * (cout,KD,KH,KW,cin) layout, SURVEY A.3; DZ_TF32 expects (cout, K*cin_pad), DZ_TF32X3 (2, cout, K*cin_pad) = [W_hi ; W_lo]
+ * with W_hi = RN_tf32(W), W_lo = RN_tf32(W - W_hi)).  in_rows = allocated rows of `in` (unused).  mode: DZ_F32 exact-fp32 FMA
+ * (nbr = k-major table), DZ_TF32 / DZ_TF32X3 one TF32 pass / hi-lo split on the wgmma tensor cores, csrc/spconv_tc.cu
+ * (nbr = ROW-major table `tab`, nbr_cap = its rows).
  * row_order: NULL, or the tile schedule of dz_rulebook_schedule (tensor-core modes only). */
 int dz_spconv_fwd(const float* in, int cin, int in_rows, const int32_t* nbr, int K, int nbr_cap,
                   const int32_t* row_order, const int* d_n_out,

@@ -171,21 +171,27 @@ def test_planes_roundtrip(cuda):
         assert ((back - x[:900]).abs() <= x[:900].abs() * (2.0 ** -8 if P == 1 else 2.0 ** -16)).all()
 
 
-@pytest.mark.parametrize('subm,cin,cout', [(True, 16, 16), (True, 64, 64), (False, 32, 64)])
-def test_tile_schedule_is_a_bit_exact_permutation(cuda, subm, cin, cout):
+@pytest.mark.parametrize('subm,cin,cout,B,spare', [(True, 16, 16, 2, 0), (True, 64, 64, 2, 0), (False, 32, 64, 2, 0),
+                                                   (True, 32, 32, 5, 300)],
+                         ids=['True-16-16', 'True-64-64', 'False-32-64', 'True-32-32-B5-spare300'])
+def test_tile_schedule_is_a_bit_exact_permutation(cuda, subm, cin, cout, B, spare):
     """Row-major table == k-major table; dz_rulebook_schedule: `order` is a permutation of the valid rows grouped by
     neighbour-mask digest, a 128-row tile then touches fewer kernel offsets than in coordinate order, the tile launch order
-    is heaviest-first, and the scheduled tensor-core conv returns bit-identical features (same per-row accumulation
-    order), incl. rows beyond the count being left alone."""
+    is heaviest-first with the capacity tiles beyond the count last, and the scheduled tensor-core conv returns
+    bit-identical features (same per-row accumulation order), incl. rows beyond the count being left alone.  `spare`:
+    capacity rows of a submanifold level beyond its count; the B = 5 case is a batch of more than two frames."""
     from detzero_b200 import ops
     from detzero_b200.spconv.pytorch import SparseConvTensor
-    shape, B = [13, 64, 64], 2
+    shape = [13, 64, 64]
     idx, f = _sparse_input(cuda, 77, B, shape, 0.05, cin)
     t = SparseConvTensor(f.to(cuda), torch.from_numpy(idx).to(cuda), shape, B)
     if subm:
-        cap = out_cap = len(idx)
+        n = len(idx)
+        cap = out_cap = n + spare
+        coords = torch.zeros((cap, 4), dtype=torch.int32, device=cuda)
+        coords[:n] = t._idx
         sws = ops.new_sched_ws(cap, cuda)
-        (nbr, tab), d_n, n = ops.rulebook_subm(t._idx, t._count, t._cap, t.grid_index(), [3, 3, 3], layout='both', sched_ws=sws), t._count, len(idx)
+        (nbr, tab), d_n = ops.rulebook_subm(coords, t._count, cap, t.grid_index(), [3, 3, 3], layout='both', sched_ws=sws), t._count
     else:
         cap = out_cap = len(idx) * 2
         sws = ops.new_sched_ws(cap, cuda)
@@ -210,6 +216,8 @@ def test_tile_schedule_is_a_bit_exact_permutation(cuda, subm, cin, cout):
         return v.reshape(27, tiles, 128).any(2).sum(0)
     work = tile_work(k_major[:, o] >= 0)
     assert np.all(np.diff(work[to]) <= 0)
+    live = to[to * 128 < n]
+    assert np.array_equal(np.sort(live), np.arange((n + 127) // 128)) and np.all(to[len(live):] * 128 >= n)   # empty tiles last
     # tile-major copy of the scheduled table: tile j = 27 neighbour planes + the row plane; tile masks appended to `order`
     tn = (n + 127) // 128
     tt = tab_tiles[:tn].cpu().numpy()
@@ -623,50 +631,6 @@ def test_batched_frames_equal_single_frames(cuda):
     for k in range(2):
         for key in ('pred_boxes', 'pred_scores', 'pred_labels'):
             assert torch.equal(both[k][key], singles[k][key]), (k, key)
-
-
-def test_frame_major_schedule(cuda):
-    """batches: the schedule sorts by (frame, mask): `order` stays a permutation, its frames are contiguous and ascending, the
-    tiles are ordered frame by frame and heaviest-first inside a frame (empty capacity tiles last), and the conv output is
-    bit-identical to the unscheduled launch"""
-    from detzero_b200 import ops
-    from detzero_b200.spconv.pytorch import SparseConvTensor
-    shape, B, cin, cout = [13, 64, 64], 5, 32, 32
-    idx, f = _sparse_input(cuda, 78, B, shape, 0.05, cin)
-    t = SparseConvTensor(f.to(cuda), torch.from_numpy(idx).to(cuda), shape, B)
-    n = len(idx)
-    cap = n + 300
-    feats = torch.zeros((cap, cin), device=cuda); feats[:n] = t._feat
-    coords = torch.zeros((cap, 4), dtype=torch.int32, device=cuda); coords[:n] = t._idx
-    d_n = torch.tensor([n], dtype=torch.int32, device=cuda)
-    sws = ops.new_sched_ws(cap, cuda)
-    tab = ops.rulebook_subm(coords, d_n, cap, t.grid_index(), [3, 3, 3], layout='row', sched_ws=sws, frame_major=True)
-    order, tab_tiles = ops.rulebook_schedule(tab, d_n, sws, B, True, K=27)
-    o = order[:n].cpu().numpy()
-    assert np.array_equal(np.sort(o), np.arange(n))
-    frames = idx[o, 0]
-    assert np.all(np.diff(frames) >= 0)                                       # frame-major row order
-    tiles = (cap + 127) // 128
-    to = order[cap:cap + tiles].cpu().numpy()
-    assert np.array_equal(np.sort(to), np.arange(tiles))
-    live = to[to * 128 < n]
-    assert np.array_equal(np.sort(live), np.arange((n + 127) // 128)) and np.all(to[len(live):] * 128 >= n)   # empty tiles last
-    masks = tab[:n, 27].cpu().numpy()
-    work = np.array([bin(int(np.bitwise_or.reduce(masks[o[j * 128:(j + 1) * 128]]))).count('1') for j in live])
-    tframe = frames[live * 128]
-    assert np.all(np.diff(tframe) >= 0)                                       # tiles frame by frame ...
-    for b in range(B):
-        assert np.all(np.diff(work[tframe == b]) <= 0)                        # ... heaviest-first inside a frame
-    g = np.random.default_rng(9)
-    w = torch.from_numpy(g.normal(0, 0.2, (cout, 3, 3, 3, cin)).astype(np.float32))
-    for mode in (_lib.DZ_TF32, _lib.DZ_BF16X2):
-        P = _lib.PLANES.get(mode, 0)
-        wp = ops.pack_spconv_weight(w, mode).to(cuda)
-        fin = ops.to_planes(feats, d_n, P) if P else feats
-        a = ops.spconv_fwd(fin, tab, d_n, cap, wp, None, None, None, True, mode, kshape=(27, cin, cout), layout='row')
-        b = ops.spconv_fwd(fin, tab, d_n, cap, wp, None, None, None, True, mode, kshape=(27, cin, cout), row_order=order, layout='row',
-                           tab_tiles=tab_tiles if P else None)
-        assert torch.equal(a[:n], b[:n]), mode
 
 
 @pytest.mark.parametrize('cin,cout,k,stride,pad,H,W,B,coff,cstride', [(128, 128, 3, 1, 1, 188, 188, 2, 0, 128), (256, 256, 3, 1, 1, 94, 94, 8, 0, 256),
