@@ -10,6 +10,8 @@ LIB_PATH = os.path.join(_HERE, 'libdetzero_b200.so')
 DZ_F32, DZ_TF32, DZ_BF16, DZ_TF32X3, DZ_BF16X2 = 0, 1, 2, 3, 4
 MODES = {'fp32': DZ_F32, 'f32': DZ_F32, 'tf32': DZ_TF32, 'bf16': DZ_BF16, 'tf32x3': DZ_TF32X3, 'fp32_tc': DZ_TF32X3,
          'bf16x2': DZ_BF16X2}
+#: test-time augmentation view ops (csrc/tta.cu)
+DZ_TTA_ORIGINAL, DZ_TTA_FLIP_X, DZ_TTA_FLIP_Y, DZ_TTA_FLIP_XY, DZ_TTA_ROT, DZ_TTA_SCALE = 0, 1, 2, 3, 4, 5
 #: bf16 operand planes per mode (sparse conv, csrc/spconv_bf16.cu)
 PLANES = {DZ_BF16: 1, DZ_BF16X2: 2}
 
@@ -63,6 +65,10 @@ _SIGS = {
     'dz_crop_points_ws_bytes': (sz, [ci, ci]),
     'dz_crop_points_in_boxes': (ci, [vp, ci, ci, vp, ci, ci, vp, ci, vp, vp, sz, vp]),
     'dz_points_in_boxes_mask': (ci, [vp, ci, ci, vp, ci, ci, vp, vp]),
+    'dz_tta_expand': (ci, [vp, ci, vp, ci, vp, ci, vp, vp]),
+    'dz_tta_unaugment': (ci, [vp, vp, ci, ci, vp, ci, vp, vp]),
+    'dz_wbf_3d_ws_bytes': (sz, [ci, ci, ci, ci]),
+    'dz_wbf_3d': (ci, [vp, vp, ci, ci, ci, vp, vp, ci, vp, vp, vp, sz, vp]),
     'dz_linear_fwd': (ci, [vp, ci, ci, vp, ci, vp, vp, ci, vp, ci, ci, vp]),
     'dz_linear_fwd_grouped': (ci, [vp, ci, ci, vp, ci, vp, vp, vp, ci, ci, vp, ci, ci, vp]),
     'dz_linear_max_fwd': (ci, [vp, ci, ci, vp, ci, vp, vp, ci, ci, vp, ci, vp]),
@@ -106,3 +112,7 @@ def farr(vals):
 
 def iarr(vals):
     return (ctypes.c_int * len(vals))(*[int(v) for v in vals])
+
+
+def darr(vals):
+    return (ctypes.c_double * len(vals))(*[float(v) for v in vals])

@@ -1,4 +1,5 @@
-// boxgeom.cuh -- rotated-BEV box geometry shared by the NMS / IoU kernels (head.cu) and the tracker / crop kernels (track.cu).
+// boxgeom.cuh -- rotated-BEV box geometry shared by the NMS / IoU kernels (head.cu), the tracker / crop kernels (track.cu) and the
+// weighted box fusion of test-time augmentation (tta.cu).
 // Same polygon-clip algorithm as the reference (utils/detzero_utils/ops/iou3d_nms/src/iou3d_nms_kernel.cu:42-335): the keep set of
 // the NMS and the tracker's association matrix depend on its 1e-2 in-box margin and atan2 ordering, so it is re-expressed, not changed.
 #pragma once
@@ -84,4 +85,12 @@ __device__ __forceinline__ float bev_iou(const float* a, const float* b) {
     float sa = a[3] * a[4], sb = b[3] * b[4];
     float so = bev_overlap(a, b);
     return so / fmaxf(sa + sb - so, 1e-8f);
+}
+
+// 3-D IoU of boxes_iou3d_gpu (iou3d_nms_utils.py:85-105): BEV overlap area times the z overlap, over the union volume
+__device__ __forceinline__ float iou3d(const float* a, const float* b) {
+    const float a_max = a[2] + a[5] / 2, a_min = a[2] - a[5] / 2, b_max = b[2] + b[5] / 2, b_min = b[2] - b[5] / 2;
+    const float oh = fmaxf(fminf(a_max, b_max) - fmaxf(a_min, b_min), 0.f);
+    const float o3 = bev_overlap(a, b) * oh;
+    return o3 / fmaxf(a[3] * a[4] * a[5] + b[3] * b[4] * b[5] - o3, 1e-6f);
 }

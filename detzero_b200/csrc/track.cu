@@ -29,10 +29,7 @@ __global__ void k_boxes_pairwise(const float* __restrict__ A, int na, int lda, c
     } else if (kind == DZ_PAIR_OVERLAP_BEV) {
         r = bev_overlap(a, b);                                                   // boxes_overlap_bev_gpu
     } else if (kind == DZ_PAIR_IOU_3D) {                                         // iou3d_nms_utils.py:85-105
-        const float a_max = a[2] + a[5] / 2, a_min = a[2] - a[5] / 2, b_max = b[2] + b[5] / 2, b_min = b[2] - b[5] / 2;
-        const float oh = fmaxf(fminf(a_max, b_max) - fmaxf(a_min, b_min), 0.f);
-        const float o3 = bev_overlap(a, b) * oh;
-        r = o3 / fmaxf(a[3] * a[4] * a[5] + b[3] * b[4] * b[5] - o3, 1e-6f);
+        r = iou3d(a, b);
     } else {                                                                     // distance.py:69-101 on (x, y, w, h) = box[0,1,3,4]
         const float ax1 = a[0] - a[3] * 0.5f, ay1 = a[1] - a[4] * 0.5f, ax2 = a[0] + a[3] * 0.5f, ay2 = a[1] + a[4] * 0.5f;
         const float bx1 = b[0] - b[3] * 0.5f, by1 = b[1] - b[4] * 0.5f, bx2 = b[0] + b[3] * 0.5f, by2 = b[1] + b[4] * 0.5f;

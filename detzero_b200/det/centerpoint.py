@@ -6,7 +6,8 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from . import backbone3d, dense, vfe
+from . import backbone3d, dense, tta, vfe
+from .. import ops
 
 #: module registry, same keys as detzero_det.models.centerpoint_modules.__all__ (PDVHead = 2nd stage, out of scope)
 cp_modules = {
@@ -33,6 +34,7 @@ class CenterPoint(nn.Module):
         if self.second_stage:
             raise NotImplementedError('PDVHead second stage is out of scope (SURVEY.md §2.1)')
         self.module_list = self.build_networks()
+        self._tta_views = {}                               # tta_ops names -> (expand, un-augment) view parameters
 
     @property
     def mode(self):
@@ -74,11 +76,60 @@ class CenterPoint(nn.Module):
         """all device work of one batch, no host sync (capturable in a CUDA graph); result =
         batch_dict['final_boxes_padded'] (B,500,9) + ['final_boxes_count'] (B) + ['overflow_flag'] (1,) int32: number of
         sparse levels (and the voxelizer) whose true row count exceeded the capacity the kernels clamped to -- nonzero
-        means rows were dropped and the step must be re-run with larger capacities (post_processing raises)"""
+        means rows were dropped and the step must be re-run with larger capacities (post_processing raises).
+
+        With test-time augmentation (the batch carries the reference's ``tta_ops`` and ``batch_size`` = B*V) the B original frames
+        are expanded into B*V views on the device, the modules run unchanged on them, and the final boxes are the per-frame
+        weighted box fusion of the un-augmented views: (B, V*500, 9) + (B,).  The per-view result stays in
+        ``tta_view_boxes_padded`` / ``tta_view_boxes_count``."""
+        if 'tta_ops' in batch_dict:
+            return self._forward_tta(batch_dict)
         for m in self.module_list:
             batch_dict = m(batch_dict)
         batch_dict['overflow_flag'] = self._overflow_flag(batch_dict)
         return batch_dict
+
+    def _forward_tta(self, batch_dict):
+        """CenterPoint.test_time_augment (detection/detzero_det/models/centerpoint.py:131-208) for B frames at once: each frame is
+        fused on its own (the reference handles one frame per batch)"""
+        if 'gather_slab' in batch_dict:
+            raise NotImplementedError('test-time augmentation with the per-sequence box gather (gather_slab) is not supported')
+        if len(self.dense_head.heads_list) != 1:
+            raise NotImplementedError('test-time augmentation needs a single CenterHead head (got %d)' % len(self.dense_head.heads_list))
+        names = tuple(batch_dict['tta_ops'])
+        aug = self._tta_views.get(names)
+        if aug is None:
+            a = tta.ops_from_names(names)
+            aug = self._tta_views[names] = (a.expand_views(), a.unaugment_views())
+        V = len(names)
+        BV = int(batch_dict['batch_size'])
+        if BV % V:
+            raise ValueError('batch_size %d is not a multiple of the %d test-time views' % (BV, V))
+        B = BV // V
+        points = batch_dict['points']
+        if 'points_per_frame' in batch_dict:                     # host-side frame sizes: no sync needed
+            sizes = [int(s) for s in batch_dict['points_per_frame']]
+        else:
+            sizes = torch.bincount(points[:, 0].long(), minlength=B).tolist()
+        if len(sizes) != B:
+            raise ValueError('points_per_frame has %d frames, tta batch_size %d / %d views = %d' % (len(sizes), BV, V, B))
+        inner = {k: v for k, v in batch_dict.items() if k != 'tta_ops'}
+        inner['points'] = ops.tta_expand(points.float().contiguous(), sizes, aug[0])
+        inner['points_per_frame'] = [s for s in sizes for _ in range(V)]
+        inner['batch_size'] = BV
+        for m in self.module_list:
+            inner = m(inner)
+        view_boxes, view_counts = inner['final_boxes_padded'], inner['final_boxes_count']
+        boxes = ops.tta_unaugment(view_boxes, view_counts, aug[1])
+        fused, counts = ops.wbf_3d(boxes, view_counts, V, tta.WBF_IOU_THR, tta.WBF_SKIP_BOX_THR)
+        out = dict(inner)
+        out.update(points=points, points_per_frame=batch_dict.get('points_per_frame'), tta_ops=list(names), batch_size=B,
+                   tta_view_boxes_padded=view_boxes, tta_view_boxes_count=view_counts,
+                   final_boxes_padded=fused, final_boxes_count=counts)
+        if out['points_per_frame'] is None:
+            del out['points_per_frame']
+        out['overflow_flag'] = self._overflow_flag(out)
+        return out
 
     @staticmethod
     def _levels(batch_dict):

@@ -10,6 +10,7 @@ from functools import partial
 import numpy as np
 
 from ..config import AttrDict
+from .tta import TestTimeAugmentor
 
 
 def mask_points_by_range(points, limit_range):
@@ -84,8 +85,12 @@ class DataProcessor:
             return partial(self.transform_points_to_voxels, config=config)
         return data_dict
 
-    def forward(self, data_dict):
+    def forward(self, data_dict, mask_range=True):
+        """mask_range=False skips mask_points_and_boxes_outside_range: with test-time augmentation the reference masks each
+        augmented view (dataset.py:240-246), and on the device the voxelizers drop exactly those points from each view"""
         for p in self.queue:
+            if not mask_range and p.func.__name__ == 'mask_points_and_boxes_outside_range':
+                continue
             data_dict = p(data_dict=data_dict)
         return data_dict
 
@@ -146,6 +151,10 @@ class SyntheticWaymoDataset:
         self.max_points_per_voxel = self.data_processor.max_points_per_voxel
         self.max_num_voxels = self.data_processor.max_num_voxels
         self.num_frames, self.n_points, self.seed0 = num_frames, n_points, seed0
+        tta_cfg = dataset_cfg.get('TEST_TIME_AUGMENTOR')
+        self.test_time_augmentor = TestTimeAugmentor(tta_cfg) if tta_cfg is not None else None
+        if self.tta and self.test_time_augmentor is None:
+            raise ValueError('TTA: True needs a TEST_TIME_AUGMENTOR block in the dataset config')
 
     def __len__(self):
         return self.num_frames
@@ -154,18 +163,32 @@ class SyntheticWaymoDataset:
         pts = synth_waymo_cloud(self.seed0 + index, self.n_points)
         d = {'points': pts, 'frame_id': 'synth_%06d' % index, 'sequence_name': 'synthetic', 'sample_idx': index}
         d = self.point_feature_encoder.forward(d)
-        d = self.data_processor.forward(d)
-        return d
+        return self.process(d)
+
+    def process(self, data_dict):
+        """the data processor; with TTA the original cloud stays unmasked and carries the view names (the views themselves are
+        built on the device by CenterPoint)"""
+        if not self.tta:
+            return self.data_processor.forward(data_dict)
+        data_dict = self.data_processor.forward(data_dict, mask_range=False)
+        data_dict['tta_ops'] = self.test_time_augmentor.names
+        return data_dict
 
     @staticmethod
     def collate_batch(batch_list):
+        """dataset.py:260-303; with TTA (items carry ``tta_ops``) the points stay the B original frames, and the batch gets the
+        view names and batch_size = B * views, as in the reference"""
         pts, sizes = [], []
         for b, d in enumerate(batch_list):
             p = d['points']
             pts.append(np.pad(p, ((0, 0), (1, 0)), mode='constant', constant_values=b))    # dataset.py:275-283
             sizes.append(p.shape[0])
-        return {'points': np.concatenate(pts, axis=0).astype(np.float32), 'points_per_frame': sizes,
-                'frame_id': np.array([d['frame_id'] for d in batch_list]), 'batch_size': len(batch_list)}
+        ret = {'points': np.concatenate(pts, axis=0).astype(np.float32), 'points_per_frame': sizes,
+               'frame_id': np.array([d['frame_id'] for d in batch_list]), 'batch_size': len(batch_list)}
+        if 'tta_ops' in batch_list[0]:
+            ret['tta_ops'] = list(batch_list[0]['tta_ops'])
+            ret['batch_size'] = len(batch_list) * len(ret['tta_ops'])
+        return ret
 
 
 def default_waymo_1sweep_cfg():
@@ -174,6 +197,13 @@ def default_waymo_1sweep_cfg():
         'DATASET': 'SyntheticWaymoDataset',
         'POINT_CLOUD_RANGE': [-75.2, -75.2, -2, 75.2, 75.2, 4],
         'TTA': False,
+        'TEST_TIME_AUGMENTOR': {
+            'DISABLE_AUG_LIST': ['placeholder'],
+            'AUG_CONFIG_LIST': [
+                {'NAME': 'world_flip', 'ALONG_AXIS_LIST': ['x', 'y', 'xy']},
+                {'NAME': 'world_rotation', 'ROT_ANGLE': [0, -0.39365818, -0.78539816, -1.17809724, -2.74889357, 0.39365818,
+                                                         0.78539816, 1.17809724, 2.74889357, 3.14159265]},
+                {'NAME': 'world_scaling', 'SCALE_RANGE': [0.95, 1.05]}]},
         'POINT_FEATURE_ENCODING': {'encoding_type': 'absolute_coordinates_encoding',
                                    'used_feature_list': ['x', 'y', 'z', 'intensity', 'elongation'],
                                    'src_feature_list': ['x', 'y', 'z', 'intensity', 'elongation', 'offset']},

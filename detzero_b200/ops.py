@@ -475,6 +475,49 @@ def boxes_iou_bev(a, b):
     return out
 
 
+def tta_expand(points, frame_sizes, views):
+    """collated points (N, stride) [b,x,y,z,...] with host-known frame sizes -> (V*N, stride), frame b view v at batch index
+    b*V+v; views (V, 4) host float32 [op, p1, p2, p3] (see dz_tta_expand)"""
+    _need_cuda(points)
+    _f32c(points)
+    n, stride = points.shape
+    V = len(views)
+    assert sum(int(s) for s in frame_sizes) == n
+    out = torch.empty((V * n, stride), dtype=torch.float32, device=points.device)
+    check(lib().dz_tta_expand(_p(points), stride, iarr(frame_sizes), len(frame_sizes), farr(views.reshape(-1).tolist()), V,
+                              _p(out), _stream()), 'tta_expand')
+    _count(len(frame_sizes))
+    return out
+
+
+def tta_unaugment(boxes, counts, views):
+    """boxes (B*V, K, 9) + counts (B*V,) int32 -> rows mapped back to the original frame (rows past the count are zeroed)"""
+    _need_cuda(boxes, counts)
+    BV, K, _ = boxes.shape
+    assert counts.dtype == torch.int32 and counts.shape == (BV,)
+    out = torch.empty_like(boxes)
+    check(lib().dz_tta_unaugment(_p(_f32c(boxes)), _p(counts), BV, K, farr(views.reshape(-1).tolist()), len(views), _p(out),
+                                 _stream()), 'tta_unaugment')
+    _count(1)
+    return out
+
+
+def wbf_3d(boxes, counts, V, iou_thr, skip_thr):
+    """3-D weighted box fusion per frame of V views: boxes (B*V, K, 9) + counts (B*V,) int32 -> fused (B, V*K, 9) rows in
+    descending score order + counts (B,) int32 (see dz_wbf_3d)"""
+    _need_cuda(boxes, counts)
+    BV, K, _ = boxes.shape
+    assert BV % V == 0 and counts.dtype == torch.int32 and counts.shape == (BV,) and len(iou_thr) == len(skip_thr)
+    B, L = BV // V, len(iou_thr)
+    out = torch.empty((B, V * K, 9), dtype=torch.float32, device=boxes.device)
+    d_n = torch.empty(B, dtype=torch.int32, device=boxes.device)
+    ws = workspace(lib().dz_wbf_3d_ws_bytes(B, V, K, L), boxes.device, 'wbf')
+    check(lib().dz_wbf_3d(_p(_f32c(boxes)), _p(counts), B, V, K, _lib.darr(iou_thr), _lib.darr(skip_thr), L, _p(out), _p(d_n),
+                          _p(ws), ws.numel(), _stream()), 'wbf_3d')
+    _count(3)
+    return out, d_n
+
+
 def linear(x, w, scale=None, shift=None, relu=False, out=None, mode=_lib.DZ_F32):
     """y = act((x @ w.T) * scale + shift); x (M,K), w (N,K)"""
     _need_cuda(x, w)

@@ -239,7 +239,35 @@ int dz_crop_points_in_boxes(const float* points, int n_pts, int pt_stride, const
 int dz_points_in_boxes_mask(const float* points, int n_pts, int pt_stride, const float* boxes, int n_boxes, int ldb,
                             int32_t* mask, dz_stream_t stream);
 
-/* ---- refiner (GRM / PRM / CRM) ------------------------------------------------------------------------- */
+/* ---- test-time augmentation (CenterPoint TTA) ------------------------------------------------------------- */
+/* A view is 4 host floats [op, p1, p2, p3]: DZ_TTA_ORIGINAL; DZ_TTA_FLIP_X (y = -y); DZ_TTA_FLIP_Y (x = -x); DZ_TTA_FLIP_XY;
+ * DZ_TTA_ROT with p1, p2 = cos, sin of the float32 angle (float32 torch on the CPU, as the reference computes them) and, for
+ * dz_tta_unaugment only, p3 = the float32 heading offset; DZ_TTA_SCALE with p1 = the float32 scale. */
+enum { DZ_TTA_ORIGINAL = 0, DZ_TTA_FLIP_X = 1, DZ_TTA_FLIP_Y = 2, DZ_TTA_FLIP_XY = 3, DZ_TTA_ROT = 4, DZ_TTA_SCALE = 5 };
+enum { DZ_TTA_MAX_VIEWS = 32, DZ_WBF_MAX_LABELS = 8 };
+/* points (N, stride) collated [b, x, y, z, feats...], frames contiguous with host-known sizes h_frame_sizes (B) ->
+ * out (V*N, stride): frame b view v at rows V*start_b + v*n_b .. with batch index b*V + v, x/y/z augmented, features copied.
+ * Replaces TestTimeAugmentor.forward (detection/detzero_det/datasets/augmentor/test_time_augmentor.py:32-100, rotation by
+ * common_utils.rotate_points_along_z, utils/detzero_utils/common_utils.py:220-244) and the TTA branch of collate_batch
+ * (detection/detzero_det/datasets/dataset.py:260-303), which build the views in numpy in the DataLoader workers. */
+int dz_tta_expand(const float* points, int stride, const int* h_frame_sizes, int B, const float* h_views, int V, float* out,
+                  dz_stream_t stream);
+/* boxes (BV, K, 9) [x,y,z,dx,dy,dz,heading,score,label] with counts (BV,) -> out (BV, K, 9) in the original frame (inverse of view
+ * bv % V; rows past the count are zeroed).  Replaces the restore loop of CenterPoint.test_time_augment
+ * (detection/detzero_det/models/centerpoint.py:157-202). */
+int dz_tta_unaugment(const float* boxes, const int* counts, int BV, int K, const float* h_views, int V, float* out,
+                     dz_stream_t stream);
+/* 3-D weighted box fusion of the V views of each of B frames: boxes (B*V, K, 9) + counts (B*V,) -> out (B, V*K, 9) fused rows
+ * [x,y,z,dx,dy,dz,heading,score,label] in descending score order (ties: the cluster's first member by (view, row)), out_count (B,).
+ * Labels 1..L with h_iou_thr / h_skip_thr (host, L doubles, indexed label-1); other labels are dropped.  conf_type 'avg', unit
+ * weights, allows_overflow False.  V*K <= 16384.  Replaces weighted_boxes_fusion_3d
+ * (detection/detzero_det/utils/ensemble_utils/wbf_3d.py:10-190) as called by wbf_online (ensemble.py:7-32), whose
+ * find_matching_box launches boxes_iou3d_gpu and reads the IoU back once per input box. */
+size_t dz_wbf_3d_ws_bytes(int B, int V, int K, int L);
+int dz_wbf_3d(const float* boxes, const int* counts, int B, int V, int K, const double* h_iou_thr, const double* h_skip_thr, int L,
+              float* out, int* out_count, void* ws, size_t ws_bytes, dz_stream_t stream);
+
+/* ---- refiner (GRM / PRM / CRM)------------------------------------------------------------------------- */
 /* y = act((x @ W^T) * scale + shift): x (M,K) row-major, W (N,K) row-major (nn.Linear / 1x1 Conv layout).
  * Replaces F.linear and the Conv1d/Conv2d(k=1)+BN+ReLU MLP stacks (utils/detzero_utils/model_utils.py:81-134). */
 int dz_linear_fwd(const float* x, int M, int K, const float* w, int N, const float* scale, const float* shift,
