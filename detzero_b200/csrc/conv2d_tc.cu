@@ -347,6 +347,190 @@ static int launch_tf32(const Conv2dParams& p, const CUtensorMap& tmA, const CUte
     return DZ_OK;
 }
 
+// HALO N=256 variant (the 3x3 stride-1 BEV / head convolutions with cout >= 64 and enough tiles to fill the machine): output
+// channels are the wgmma M side and 256 pixels the N side, the widest instruction wgmma has (m64n256k8).  Per instruction it reads
+// 2 KB of weights + 8 KB of activations for 262144 FLOP, against 2 KB + 4 KB for 131072 FLOP with the pixels on M, and every weight
+// tile is reused over twice the pixels: by a model of shared-memory reads plus TMA writes per MMA clock, the traffic falls from about
+// 1.0 to 0.8 of what the tensor cores need (measured on the BEV shapes: 10-30 % faster than the 128-pixel kernel).  A is the weight tile
+// W[cout][(tap, cin)] as loaded for the kernel above; B is the halo of a 32 x 8 output patch, (32+2) x (8+2) pixels per 32-channel
+// slice: its 32 core groups of 8 pixels are the 32 patch rows, SBO = the halo pitch, and the nine taps are nine shifted B descriptors
+// into it, exactly as the A descriptors of the 128-pixel halo kernel.  BM = 128: the two consumer warpgroups take 64 channels each of
+// one 32 x 8 patch.  BM = 64 (cout <= 64): a 32 x 16 patch, the warpgroups take its two 8-pixel column halves with the same 64
+// weight rows (two CTAs per SM with one warpgroup each cannot fit two halo slots and a weight ring in half the shared memory).
+// Per output the accumulation order (slice, tap, k8 step) is that of the kernels above, so results are bit-identical.
+static constexpr int H2_TH = 32, H2_ROWS = H2_TH + 2;
+static constexpr int H2_PIECE_PX = 32;                         // epilogue piece: 4 patch rows x 8 pixels
+static constexpr int H2_PIECE_BYTES = H2_PIECE_PX * 128;       // x 32 channels
+static constexpr int H2_STG_BYTES = 4 * 2 * H2_PIECE_BYTES;    // 4 warp pairs x 2 pieces in flight
+
+template <int BM>
+struct H2Cfg {
+    static constexpr int TW = BM == 128 ? 8 : 16, PITCH = TW + 2;
+    static constexpr int A_BYTES = H2_ROWS * PITCH * 128;            // halo tile delivered by the TMA unit
+    static constexpr int A_SLOT = (A_BYTES + 1023) / 1024 * 1024;
+    static constexpr int W_BYTES = BM * CT_BK * 4;                    // weight tile of one (tap, slice)
+    static constexpr int BUDGET = 227 * 1024 - 1024 - 256 - H2_STG_BYTES - HL_A_STAGES * A_SLOT;
+    static constexpr int STAGES = BUDGET / W_BYTES > 9 ? 9 : BUDGET / W_BYTES;
+    static constexpr int SMEM = HL_A_STAGES * A_SLOT + STAGES * W_BYTES + H2_STG_BYTES + 1024 + 256;
+};
+
+// Persistent with the static tile order of k_conv2d_tf32: tile t = (patch t / tiles_n, channel tile t % tiles_n).
+template <int BM>
+__global__ void __launch_bounds__(CT_THREADS, 1)
+k_conv2d_tf32_halo_n256(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmO,
+                        Conv2dParams p, int tiles_x, int tiles_y, int tiles_n, int tiles) {
+    using Cfg = H2Cfg<BM>;
+    constexpr int TW = Cfg::TW;
+    extern __shared__ unsigned char smem_raw[];
+    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    unsigned char* smW = smem + HL_A_STAGES * Cfg::A_SLOT;
+    unsigned char* stg_all = smW + Cfg::STAGES * Cfg::W_BYTES;
+    uint64_t* full = reinterpret_cast<uint64_t*>(stg_all + H2_STG_BYTES);
+    uint64_t* empty = full + Cfg::STAGES;
+    uint64_t* a_full = empty + Cfg::STAGES;
+    uint64_t* a_empty = a_full + HL_A_STAGES;
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int cchunks = p.cin / CT_BK;
+
+    if (threadIdx.x == 0) {
+        tc::prefetch_tmap(&tmA);
+        tc::prefetch_tmap(&tmW);
+        tc::prefetch_tmap(&tmO);
+        for (int s = 0; s < Cfg::STAGES; ++s) { tc::mbar_init(full + s, 1); tc::mbar_init(empty + s, CT_CONSUMERS); }
+        for (int s = 0; s < HL_A_STAGES; ++s) { tc::mbar_init(a_full + s, 1); tc::mbar_init(a_empty + s, CT_CONSUMERS); }
+        tc::fence_barrier_init();
+    }
+    __syncthreads();
+
+    int bit = 0, hs = 0;
+    if (warp == CT_CONSUMERS) {
+        if (lane != 0) return;
+        for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+            const int n0 = (t % tiles_n) * BM;
+            int mt = t / tiles_n;
+            const int tx0 = (mt % tiles_x) * TW; mt /= tiles_x;
+            const int ty0 = (mt % tiles_y) * H2_TH;
+            const int b = mt / tiles_y;
+            for (int cc = 0; cc < cchunks; ++cc, ++hs) {
+                const int a = hs % HL_A_STAGES;
+                tc::mbar_wait(a_empty + a, ((hs / HL_A_STAGES) & 1) ^ 1);
+                tc::mbar_arrive_expect_tx(a_full + a, Cfg::A_BYTES);
+                tc::tma_load_4d(smem + a * Cfg::A_SLOT, &tmA, a_full + a, cc * CT_BK, tx0 - p.pad, ty0 - p.pad, b);
+                for (int tap = 0; tap < 9; ++tap, ++bit) {
+                    const int s = bit % Cfg::STAGES;
+                    tc::mbar_wait(empty + s, ((bit / Cfg::STAGES) & 1) ^ 1);
+                    tc::mbar_arrive_expect_tx(full + s, Cfg::W_BYTES);
+                    tc::tma_load_2d(smW + s * Cfg::W_BYTES, &tmW, full + s, tap * p.cin + cc * CT_BK, n0);
+                }
+            }
+        }
+        return;
+    }
+
+    // ---- consumers: warpgroup g accumulates weight rows [cg, cg + 64) of the tile against patch columns [xg, xg + 8); fragment row
+    // r of this thread is channel cg + 16 (warp % 4) + lane / 4 + 8 r, its columns j = patch row, 2 (lane % 4) + {0, 1} = pixel of it
+    const int g = warp >> 2, wq = warp & 3;
+    const int cg = BM == 128 ? 64 * g : 0, xg = BM == 128 ? 0 : 8 * g;
+    // epilogue: warps 2k, 2k + 1 (a pair) stage 32 channels x 32 pixels per piece, the pair's first lane stores it
+    const int pair = warp >> 1;
+    const bool store_lane = (warp & 1) == 0 && lane == 0;
+    unsigned char* stg = stg_all + pair * 2 * H2_PIECE_BYTES;
+    const int cq = 16 * (warp & 1) + (lane >> 2);              // channel within the pair's 32 (+ 8 r)
+    float acc[128];
+    for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+        const int n0 = (t % tiles_n) * BM;
+        int mt = t / tiles_n;
+        const int tx0 = (mt % tiles_x) * TW; mt /= tiles_x;
+        const int ty0 = (mt % tiles_y) * H2_TH;
+        const int b = mt / tiles_y;
+        float scl[2], shf[2];
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+            const int c = n0 + cg + 16 * wq + (lane >> 2) + 8 * r;
+            scl[r] = (c < p.cout && p.scale) ? __ldg(p.scale + c) : 1.f;
+            shf[r] = (c < p.cout && p.shift) ? __ldg(p.shift + c) : 0.f;
+        }
+#pragma unroll
+        for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+        for (int cc = 0; cc < cchunks; ++cc, ++hs) {
+            const int a = hs % HL_A_STAGES;
+            tc::mbar_wait(a_full + a, (hs / HL_A_STAGES) & 1);
+            const uint32_t ha = tc::smem_u32(smem + a * Cfg::A_SLOT);
+            for (int tap = 0; tap < 9; ++tap, ++bit) {
+                const int s = bit % Cfg::STAGES;
+                tc::mbar_wait(full + s, (bit / Cfg::STAGES) & 1);
+                const int r = tap / 3, sx = tap - r * 3;
+                // window (r, sx) of the halo: patch row i = halo row r + i, columns [xg + sx, xg + sx + 8)
+                const uint64_t bdesc = tc::smem_desc_sw128(ha + (uint32_t)((r * Cfg::PITCH + sx + xg) * 128), Cfg::PITCH * 128);
+                const uint64_t adesc = tc::smem_desc_sw128(tc::smem_u32(smW + s * Cfg::W_BYTES) + cg * 128);
+                tc::wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < CT_BK / 8; ++k)
+                    tc::wgmma<256, tc::K_TF32>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), 1u);
+                tc::wgmma_commit();
+                tc::wgmma_wait_one();
+                __syncwarp();
+                if (lane == 0 && (cc > 0 || tap > 0)) tc::mbar_arrive(empty + (bit - 1) % Cfg::STAGES);
+                if (lane == 0 && tap == 0 && cc > 0) tc::mbar_arrive(a_empty + (hs - 1) % HL_A_STAGES);
+            }
+        }
+        tc::wgmma_wait_all();
+        if (lane == 0) { tc::mbar_arrive(empty + (bit - 1) % Cfg::STAGES); tc::mbar_arrive(a_empty + (hs - 1) % HL_A_STAGES); }
+
+        // ---- epilogue: folded BatchNorm / bias / ReLU (separately rounded multiply and add), transposed into NHWC pieces of 4 patch rows
+        // (staging row = pixel 8 (j % 4) + x, 32 channels, 128-byte swizzle), double-buffered per warp pair: before a piece is
+        // published the store lane waits until every earlier store has read its buffer, so the piece after it may reuse that buffer
+        const int c_pair = n0 + cg + 32 * (wq >> 1);
+        const uint32_t stg_u = tc::smem_u32(stg);
+#pragma unroll
+        for (int k = 0; k < H2_TH / 4; ++k) {
+            const uint32_t buf = stg_u + (uint32_t)((k & 1) * H2_PIECE_BYTES);
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+                const int j = 4 * k + jj;
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    const int q = cq + 8 * r;
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        float o = __fmul_rn(acc[4 * j + 2 * r + c], scl[r]);
+                        if (p.shift) o = __fadd_rn(o, shf[r]);
+                        if (p.relu) o = tc::rna_tf32(fmaxf(o, 0.f));      // feeds another TF32 conv
+                        const int pp = 8 * jj + 2 * (lane & 3) + c;
+                        asm volatile("st.shared.f32 [%0], %1;" ::"r"(buf + (uint32_t)(pp * 128 + (((q >> 2) ^ (pp & 7)) << 4) + (q & 3) * 4)), "f"(o)
+                                     : "memory");
+                    }
+                }
+            }
+            tc::fence_proxy_async();
+            if (store_lane) tc::tma_store_wait_read();
+            tc::named_sync(2 + pair, 64);
+            if (store_lane && c_pair < p.cout) {
+                tc::tma_store_4d(&tmO, stg + (k & 1) * H2_PIECE_BYTES, p.out_coff + c_pair, tx0 + xg, ty0 + 4 * k, b);
+                tc::tma_store_commit();
+            }
+        }
+    }
+    if (store_lane) tc::tma_store_wait_read();
+}
+
+template <int BM>
+static int launch_halo_n256(const Conv2dParams& p, const CUtensorMap& tmA, const CUtensorMap& tmW, const CUtensorMap& tmO, int tiles,
+                            cudaStream_t st) {
+    using Cfg = H2Cfg<BM>;
+    static bool attr = false;
+    if (!attr) {
+        DZ_CUDA(cudaFuncSetAttribute(k_conv2d_tf32_halo_n256<BM>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM));
+        attr = true;
+    }
+    const int tiles_x = dz_cdiv(p.Wo, Cfg::TW), tiles_y = dz_cdiv(p.Ho, H2_TH), tiles_n = dz_cdiv(p.cout, BM);
+    const int grid = tiles < DZ_NUM_SMS ? tiles : DZ_NUM_SMS;
+    k_conv2d_tf32_halo_n256<BM><<<grid, CT_THREADS, Cfg::SMEM, st>>>(tmA, tmW, tmO, p, tiles_x, tiles_y, tiles_n, tiles);
+    DZ_LAUNCH_CHECK();
+    return DZ_OK;
+}
+
 // p.w must be in (cout, KH, KW, cin) layout for this path.  p.os >= 2 (oy0 = ox0 = 0, KH = KW = 1) is a ConvTranspose2d with
 // kernel == stride as ONE GEMM over the input pixels: N = os * os * cout columns, weights in (dy, dx, cout, cin) layout; column
 // n goes to channel n % cout of output pixel (y * os + dy, x * os + dx), (dy, dx) = (n / cout) / os, % os.
@@ -368,9 +552,16 @@ int dz_conv2d_fwd_tc(const Conv2dParams& p_in, int mode, cudaStream_t st) {
     p.tma_store = (p.gmax || !aligned) ? 0 : p.os == 1 ? 1 : (p.cout % 32 == 0 ? 2 : 0);
     const int N = p.cout * p.os * p.os;
     const int bn = N > 64 ? 128 : (N > 32 ? 64 : 32);
-    // 3x3 stride-1 convolutions with at least two patches per SM and 128-channel slice: the halo variant
+    // 3x3 stride-1 convolutions: the N=256 halo variant for cout >= 64 when its tiles fill the machine, else the 128-pixel halo variant
+    // with at least two patches per SM and 128-channel slice
+    const bool halo3x3 = p.KH == 3 && p.KW == 3 && p.stride == 1 && p.tma_store == 1 && !p.gshift;
+    const int bm = p.cout > 64 ? 128 : 64;
+    const int h2_tw = bm == 128 ? H2Cfg<128>::TW : H2Cfg<64>::TW;
+    const long long tiles_h2 = (long long)dz_cdiv(p.Wo, h2_tw) * dz_cdiv(p.Ho, H2_TH) * p.B * dz_cdiv(p.cout, bm);
+    const bool halo_n256 = halo3x3 && p.cout >= 64 && tiles_h2 >= DZ_NUM_SMS;
+    if (halo_n256 && tiles_h2 > INT32_MAX) { dz_set_error("dz_conv2d_fwd(tf32): %lld tiles", tiles_h2); return DZ_ERR_UNSUPPORTED; }
     const long long tiles_m = (long long)dz_cdiv(p.Wo, CT_TW) * dz_cdiv(p.Ho, CT_TH) * p.B;
-    const bool halo = p.KH == 3 && p.KW == 3 && p.stride == 1 && p.tma_store == 1 && !p.gshift && tiles_m * dz_cdiv(p.cout, 128) >= 2 * DZ_NUM_SMS;
+    const bool halo = !halo_n256 && halo3x3 && tiles_m * dz_cdiv(p.cout, 128) >= 2 * DZ_NUM_SMS;
     const int TW = halo ? HL_TW : CT_TW;
     CUtensorMap tmA, tmB;
     {
@@ -380,6 +571,7 @@ int dz_conv2d_fwd_tc(const Conv2dParams& p_in, int mode, cudaStream_t st) {
         // on each side
         cuuint32_t box[4] = {(cuuint32_t)CT_BK, (cuuint32_t)((CT_TW - 1) * p.stride + 1), (cuuint32_t)((CT_TH - 1) * p.stride + 1), 1};
         if (halo) { box[1] = HL_PITCH; box[2] = HL_ROWS; }
+        if (halo_n256) { box[1] = h2_tw + 2; box[2] = H2_ROWS; }
         cuuint32_t estr[4] = {1, (cuuint32_t)p.stride, (cuuint32_t)p.stride, 1};
         CUresult r = enc(&tmA, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)p.in, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -411,11 +603,14 @@ int dz_conv2d_fwd_tc(const Conv2dParams& p_in, int mode, cudaStream_t st) {
         cuuint64_t dims[4] = {(cuuint64_t)(p.out_coff + p.cout), (cuuint64_t)p.OW, (cuuint64_t)p.OH, (cuuint64_t)p.B};
         cuuint64_t strides[3] = {(cuuint64_t)p.out_cstride * 4, (cuuint64_t)p.OW * p.out_cstride * 4, (cuuint64_t)p.OH * p.OW * p.out_cstride * 4};
         cuuint32_t box[4] = {32, (cuuint32_t)TW, (cuuint32_t)(16 / TW), 1};      // one warp's 16 pixels
+        if (halo_n256) { box[1] = 8; box[2] = H2_PIECE_PX / 8; }                // one epilogue piece of a warp pair
         cuuint32_t estr[4] = {1, 1, 1, 1};
         CUresult r = enc(&tmO, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)p.out, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) { dz_set_error("cuTensorMapEncodeTiled(out) failed: %d", (int)r); return DZ_ERR_CUDA; }
     }
+    if (halo_n256)
+        return bm == 128 ? launch_halo_n256<128>(p, tmA, tmB, tmO, (int)tiles_h2, st) : launch_halo_n256<64>(p, tmA, tmB, tmO, (int)tiles_h2, st);
     if (halo) switch (bn) {
         case 128: return launch_tf32<128, true>(p, tmA, tmB, tmO, st);
         case 64: return launch_tf32<64, true>(p, tmA, tmB, tmO, st);
