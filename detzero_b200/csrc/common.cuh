@@ -42,6 +42,7 @@ struct GridIndex {
     const int32_t* perm;      // may be null (identity)
     int B, D, H, W;
     long long cells_pad;      // round_up(D*H*W, 32)
+    int rows;                 // capacity of the indexed tensor: with an identity perm, a rank >= rows has no row
 };
 
 static inline long long dz_cells_pad(int D, int H, int W) {
@@ -57,7 +58,9 @@ __device__ __forceinline__ int grid_lookup(const GridIndex& g, int b, int z, int
     uint32_t word = __ldg(g.bitmap + w);
     if (!((word >> bit) & 1u)) return -1;
     int rank = (int)(__ldg(g.prefix + w) + __popc(word & ((1u << bit) - 1u)));
-    return g.perm ? __ldg(g.perm + rank) : rank;
+    // a level whose count overflowed its capacity still has every site in its bitmap; those beyond the capacity have no row
+    // (the overflow is reported and the frame re-run), so they must not reach a neighbour table
+    return g.perm ? __ldg(g.perm + rank) : (rank < g.rows ? rank : -1);
 }
 
 __device__ __forceinline__ int warp_inclusive_scan(int v, int lane) {

@@ -150,7 +150,7 @@ extern "C" int dz_rulebook_subm(const int32_t* coords, const int* d_n, int cap, 
     DZ_CHECK_ARG(!sched_ws || tab);
     TableOut to = table_out(nbr, tab, sched_ws, cap);
     if (sched_ws) DZ_CUDA(cudaMemsetAsync(sched_ws, 0, sched_zero_bytes(cap), (cudaStream_t)stream));
-    GridIndex g{bitmap, prefix, perm, B, D, H, W, dz_cells_pad(D, H, W)};
+    GridIndex g{bitmap, prefix, perm, B, D, H, W, dz_cells_pad(D, H, W), cap};
     int blocks = max(1, min(dz_cdiv(cap, 256), DZ_NUM_SMS * 8));
     k_subm_nbr<<<blocks, 256, 0, (cudaStream_t)stream>>>(coords, d_n, cap, g, ks[0], ks[1], ks[2], to);
     DZ_LAUNCH_CHECK();
@@ -273,7 +273,7 @@ extern "C" int dz_rulebook_conv(const int32_t* in_coords, const int* d_n_in, int
     int blocks_w = max(1, min(dz_cdiv((long long)out_words, 256), DZ_NUM_SMS * 8));
     k_index_to_coords<<<blocks_w, 256, 0, st>>>(out_bitmap, out_prefix, out_words, cg.out_dhw[0], cg.out_dhw[1], cg.out_dhw[2],
                                                 out_cp, out_cap, out_coords);
-    GridIndex gin{in_bitmap, in_prefix, in_perm, B, in_dhw[0], in_dhw[1], in_dhw[2], dz_cells_pad(in_dhw[0], in_dhw[1], in_dhw[2])};
+    GridIndex gin{in_bitmap, in_prefix, in_perm, B, in_dhw[0], in_dhw[1], in_dhw[2], dz_cells_pad(in_dhw[0], in_dhw[1], in_dhw[2]), in_cap};
     int blocks_out = max(1, min(dz_cdiv(out_cap, 256), DZ_NUM_SMS * 8));
     TableOut to = table_out(nbr, tab, sched_ws, out_cap);
     if (sched_ws) DZ_CUDA(cudaMemsetAsync(sched_ws, 0, sched_zero_bytes(out_cap), st));

@@ -15,6 +15,8 @@
 // reciprocal multiply or an FMA contraction: see SURVEY.md Appendix A.1.
 #include "common.cuh"
 
+#include <cub/device/device_radix_sort.cuh>
+
 #define SENTINEL 0x7f7f7f7f
 #define INVALID_CELL 0xffffffffu
 
@@ -610,45 +612,84 @@ __global__ void __launch_bounds__(VOX_THREADS) k_dyn_mark(const float* __restric
     cell_out[i] = cell;
 }
 
-__global__ void __launch_bounds__(VOX_THREADS) k_dyn_accum(const float* __restrict__ points, int n, int stride, int c, DynGeom g,
-                                                           const long long* __restrict__ cell_in, const uint32_t* __restrict__ bitmap,
-                                                           const uint32_t* __restrict__ prefix, int cap, float* __restrict__ feats,
-                                                           int* __restrict__ cnt, int32_t* __restrict__ coords) {
+// sort key of every point: its voxel's rank (ranks ascend with the b,x,y,z key), n for a dropped point
+__global__ void __launch_bounds__(VOX_THREADS) k_dyn_key(const long long* __restrict__ cell_in, int n,
+                                                         const uint32_t* __restrict__ bitmap, const uint32_t* __restrict__ prefix,
+                                                         uint32_t* __restrict__ key, int* __restrict__ idx) {
     int i = blockIdx.x * VOX_THREADS + threadIdx.x;
     if (i >= n) return;
     long long cell = cell_in[i];
-    if (cell < 0) return;
-    size_t w = (size_t)(cell >> 5);
-    uint32_t bit = (uint32_t)cell & 31u;
-    int rank = (int)(prefix[w] + __popc(bitmap[w] & ((1u << bit) - 1u)));
-    if (rank >= cap) return;
-    const float* row = points + (size_t)i * stride + 1;
-    for (int k = 0; k < c; ++k) atomicAdd(feats + (size_t)rank * c + k, __ldg(row + k));
-    int old = atomicAdd(cnt + rank, 1);
-    if (old == 0) {
+    uint32_t k = (uint32_t)n;
+    if (cell >= 0) {
+        size_t w = (size_t)(cell >> 5);
+        uint32_t bit = (uint32_t)cell & 31u;
+        k = prefix[w] + __popc(bitmap[w] & ((1u << bit) - 1u));
+    }
+    key[i] = k;
+    idx[i] = i;
+}
+
+// after the stable sort by rank: every voxel's points form one run [beg, end) in ascending point index
+__global__ void __launch_bounds__(VOX_THREADS) k_dyn_runs(const uint32_t* __restrict__ key, const int* __restrict__ idx, int n,
+                                                          const long long* __restrict__ cell_in, DynGeom g, const int* __restrict__ d_m,
+                                                          int cap, int* __restrict__ beg, int* __restrict__ end,
+                                                          int32_t* __restrict__ coords) {
+    int j = blockIdx.x * VOX_THREADS + threadIdx.x;
+    if (j >= n) return;
+    uint32_t k = key[j];
+    if (k >= (uint32_t)min(*d_m, cap)) return;                  // dropped point, or a voxel beyond the caller's capacity
+    if (j == 0 || key[j - 1] != k) {
+        beg[k] = j;
+        long long cell = cell_in[idx[j]];
         long long b = cell / g.cells_pad, r = cell % g.cells_pad;
         int cz = (int)(r % g.grid[2]); r /= g.grid[2];
         int cy = (int)(r % g.grid[1]);
         int cx = (int)(r / g.grid[1]);
-        reinterpret_cast<int4*>(coords)[rank] = make_int4((int)b, cz, cy, cx);   // [b,z,y,x], vfe.py:143
+        reinterpret_cast<int4*>(coords)[k] = make_int4((int)b, cz, cy, cx);     // [b,z,y,x], vfe.py:143
+    }
+    if (j == n - 1 || key[j + 1] != k) end[k] = j + 1;
+}
+
+// mean of every voxel column: one fp32 sum in ascending point index, then an IEEE divide by the count (torch_scatter's
+// scatter_mean on the CPU).  Rows m..cap-1 are zeroed.
+__global__ void k_dyn_mean(const float* __restrict__ points, int stride, int c, const int* __restrict__ idx,
+                           const int* __restrict__ beg, const int* __restrict__ end, const int* __restrict__ d_m, int cap,
+                           float* __restrict__ feats) {
+    int m = min(*d_m, cap);
+    for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < (long long)cap * c; t += (long long)gridDim.x * blockDim.x) {
+        int r = (int)(t / c), k = (int)(t % c);
+        float s = 0.f;
+        if (r < m) {
+            int j0 = beg[r], j1 = end[r];
+#pragma unroll 4
+            for (int j = j0; j < j1; ++j) s = __fadd_rn(s, __ldg(points + (size_t)__ldg(idx + j) * stride + 1 + k));
+            s = __fdiv_rn(s, (float)(j1 - j0));
+        }
+        feats[t] = s;
     }
 }
 
-__global__ void k_dyn_finish(float* __restrict__ feats, const int* __restrict__ cnt, const int* __restrict__ d_m, int cap, int c) {
-    int m = min(*d_m, cap);
-    for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < (long long)m * c; t += (long long)gridDim.x * blockDim.x) {
-        int r = (int)(t / c);
-        feats[t] = __fdiv_rn(feats[t], (float)cnt[r]);
-    }
+static int dyn_key_bits(int n) { return n > 0 ? 32 - __builtin_clz((unsigned)n) : 1; }   // keys are 0..n
+
+static size_t dyn_sort_bytes(int n) {
+    size_t bytes = 0;
+    if (cub::DeviceRadixSort::SortPairs(nullptr, bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const int*)nullptr, (int*)nullptr,
+                                        n, 0, dyn_key_bits(n)) != cudaSuccess)
+        return 0;
+    return bytes;
 }
 
 extern "C" size_t dz_voxelize_dynamic_ws_bytes(int n_points, int cap, int B, int X, int Y, int Z) {
     size_t words = (size_t)((long long)B * dz_cells_pad(X, Y, Z) / 32);
     size_t n = (size_t)(n_points > 0 ? n_points : 1);
-    return dz_align_up(words * 4, 256) * 2 + dz_align_up(n * 8, 256) + dz_align_up((size_t)cap * 4, 256) +
+    return dz_align_up(words * 4, 256) * 2 + dz_align_up(n * 8, 256) + dz_align_up(n * 4, 256) * 4 +
+           dz_align_up((size_t)cap * 4, 256) * 2 + dz_align_up(dyn_sort_bytes(n_points > 0 ? n_points : 0), 256) +
            dz_scan_ws_bytes(words) + 256;
 }
 
+// Every voxel's mean is summed in ascending point index, so the result does not depend on launch timing: the same frame gives
+// the same bits on every run and under CUDA-graph replay, equal to the reference's sequential scatter on the CPU.  Points are
+// stable-sorted by voxel rank (CUB radix sort over the bits of 0..n), then one thread per voxel column walks its run.
 extern "C" int dz_voxelize_dynamic_mean(const float* points, int n, int c, int B, const float* range6, const float* vsize3,
                                         const int* grid_xyz3, float* feats, int32_t* coords, int cap, int* d_m,
                                         void* ws, size_t ws_bytes, dz_stream_t stream) {
@@ -662,22 +703,31 @@ extern "C" int dz_voxelize_dynamic_mean(const float* points, int n, int c, int B
     g.cells_pad = dz_cells_pad(g.grid[0], g.grid[1], g.grid[2]);
     size_t words = (size_t)((long long)B * g.cells_pad / 32);
     size_t nn = (size_t)(n > 0 ? n : 1);
+    size_t sort_bytes = dyn_sort_bytes(n);
     DzWs w(ws, ws_bytes);
     uint32_t* bitmap = w.take<uint32_t>(words);
     uint32_t* prefix = w.take<uint32_t>(words);
     long long* cell = w.take<long long>(nn);
-    int* cnt = w.take<int>(cap);
+    uint32_t* key = w.take<uint32_t>(nn);
+    uint32_t* key_sorted = w.take<uint32_t>(nn);
+    int* idx = w.take<int>(nn);
+    int* idx_sorted = w.take<int>(nn);
+    int* beg = w.take<int>(cap);
+    int* end = w.take<int>(cap);
+    void* sort_tmp = w.take<char>(sort_bytes > 0 ? sort_bytes : 1);
     int* sums = (int*)w.take<char>(dz_scan_ws_bytes(words));
     if (!sums) { dz_set_error("dz_voxelize_dynamic_mean: workspace carve failed"); return DZ_ERR_WORKSPACE; }
     DZ_CUDA(cudaMemsetAsync(bitmap, 0, words * 4, st));
-    DZ_CUDA(cudaMemsetAsync(cnt, 0, (size_t)cap * 4, st));
-    DZ_CUDA(cudaMemsetAsync(feats, 0, (size_t)cap * c * 4, st));
     int pblocks = max(1, dz_cdiv(n, VOX_THREADS));
     k_dyn_mark<<<pblocks, VOX_THREADS, 0, st>>>(points, n, 1 + c, g, B, bitmap, cell);
     int rc = scan_launch(bitmap, prefix, words, nullptr, d_m, sums, st);
     if (rc) return rc;
-    k_dyn_accum<<<pblocks, VOX_THREADS, 0, st>>>(points, n, 1 + c, c, g, cell, bitmap, prefix, cap, feats, cnt, coords);
-    k_dyn_finish<<<DZ_NUM_SMS * 4, 256, 0, st>>>(feats, cnt, d_m, cap, c);
+    if (n > 0) {
+        k_dyn_key<<<pblocks, VOX_THREADS, 0, st>>>(cell, n, bitmap, prefix, key, idx);
+        DZ_CUDA(cub::DeviceRadixSort::SortPairs(sort_tmp, sort_bytes, key, key_sorted, idx, idx_sorted, n, 0, dyn_key_bits(n), st));
+        k_dyn_runs<<<pblocks, VOX_THREADS, 0, st>>>(key_sorted, idx_sorted, n, cell, g, d_m, cap, beg, end, coords);
+    }
+    k_dyn_mean<<<DZ_NUM_SMS * 4, 256, 0, st>>>(points, 1 + c, c, idx_sorted, beg, end, d_m, cap, feats);
     DZ_LAUNCH_CHECK();
     return DZ_OK;
 }

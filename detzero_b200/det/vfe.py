@@ -75,20 +75,36 @@ class DynamicMeanVFE(nn.Module):
         self.grid_size = [int(g) for g in grid_size]              # x,y,z
         self.voxel_size = [float(v) for v in voxel_size]
         self.point_cloud_range = [float(v) for v in point_cloud_range]
-        self.max_voxels = int(model_cfg.get('MAX_NUMBER_OF_VOXELS', 400000)) if hasattr(model_cfg, 'get') else 400000
 
     def get_output_feature_dim(self):
         return self.num_point_features
+
+    #: capacity over the largest voxel count seen so far (the count is read back by CenterPoint.post_processing)
+    CAP_HEADROOM = 1.3
 
     @torch.no_grad()
     def forward(self, batch_dict, **kwargs):
         points = batch_dict['points'].float().contiguous()       # (b, x, y, z, i, e, ...)
         B = int(batch_dict['batch_size'])
         c = points.shape[1] - 1
-        cap = min(points.shape[0], self.max_voxels * B)
+        # like the reference, a frame has no voxel limit: every voxel holds at least one point, so one row per point always holds
+        # every voxel.  Once a count has been read back, the capacity follows it (smaller level-1 buffers and launch grids); a
+        # frame with more voxels is reported as an overflow (never truncated silently), the hint grows and the frame is re-run.
+        cap = points.shape[0]
+        hint = getattr(self, '_cap_hint', None)
+        if hint is not None:
+            cap = min(cap, (int(hint * self.CAP_HEADROOM) + 127) // 128 * 128)
+        cap = max(cap, 1)
         feats, coords, d_m = ops.voxelize_dynamic_mean(points, c, B, self.point_cloud_range, self.voxel_size,
-                                                       self.grid_size, max(cap, 1))
+                                                       self.grid_size, cap)
         batch_dict['voxel_features'] = feats
         batch_dict['voxel_coords'] = coords
         batch_dict['voxel_count'] = d_m
+        batch_dict['voxel_wanted'] = (d_m, cap, self)            # checked in CenterPoint.post_processing
         return batch_dict
+
+    def note_count(self, wanted, cap):
+        """feed the read-back voxel count into the capacity hint; raises if the capacity truncated the frame"""
+        self._cap_hint = max(int(wanted), int(getattr(self, '_cap_hint', 0) or 0))
+        if wanted > cap:
+            raise RuntimeError('voxel capacity overflow: %d voxels > capacity %d (hint raised; re-run the frame)' % (wanted, cap))

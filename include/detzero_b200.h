@@ -88,7 +88,8 @@ int dz_mean_vfe(const float* voxels, const int32_t* num_per_voxel, int M, int P,
 /* Dynamic mean voxelization of a collated batch: DynamicMeanVFE.forward (vfe.py:110-147): floor((p-lo)/vs),
  * in-range mask, key b*XYZ + x*YZ + y*Z + z, unique (sorted), scatter_mean of all c columns.
  *   points (n, 1+c) [b,x,y,z,...] ; out feats (cap,c), coords (cap,4) [b,z,y,x] ordered by ascending key ;
- *   *d_m = number of voxels.  bitmap_xyz: B*round_up(X*Y*Z,32)/32 words, zero on entry. */
+ *   *d_m = number of voxels (voxels of rank >= cap are not written).  Each mean is one fp32 sum in ascending point
+ *   index followed by an IEEE divide by the count: deterministic, and bit-equal to a sequential scatter on the CPU. */
 size_t dz_voxelize_dynamic_ws_bytes(int n_points, int cap, int B, int X, int Y, int Z);
 int dz_voxelize_dynamic_mean(const float* points, int n, int c, int B,
                              const float* range_xyz6_host, const float* vsize_xyz3_host,

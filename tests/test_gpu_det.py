@@ -84,7 +84,7 @@ def test_dynamic_mean_vfe(cuda):
     m = int(d_m.item())
     assert m == coords_ref.shape[0]
     assert torch.equal(coords[:m].cpu(), coords_ref)                       # order = ascending (b,x,y,z) key
-    assert util.rel_err(feats[:m].cpu(), mean_ref) < 1e-5                  # atomics: sum order differs
+    assert np.array_equal(feats[:m].cpu().numpy().view(np.uint32), mean_ref.numpy().view(np.uint32))
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -115,6 +115,39 @@ def test_rulebook_set_exact(cuda, ks, stride, pad):
         assert odhw == ref_shape and m == ref_idx.shape[0]
         assert np.array_equal(oc[:m].cpu().numpy(), ref_idx)                # sorted (b,z,y,x): bit-exact site list
         assert _pairs_from_nbr(nbr, m) == _pairs_from_oracle(ref_pairs)
+
+
+def test_rulebooks_on_an_overflowed_level_stay_inside_its_capacity(cuda):
+    """a strided conv whose output capacity is below its site count keeps the first `cap` sites (ascending order) and reports the
+    full count; the rulebooks built on that level (submanifold, and the next strided conv) must only name rows < cap: the sites
+    past the capacity are in the level's grid index but have no row.  Otherwise the conv gathers outside the feature buffer."""
+    from detzero_b200 import ops
+    from detzero_b200.spconv.pytorch import SparseConvTensor
+    shape, B = [11, 40, 36], 2
+    idx, f = _sparse_input(cuda, 23, B, shape, 0.08, 16)
+    t = SparseConvTensor(f.to(cuda), torch.from_numpy(idx).to(cuda), shape, B)
+    ref_idx, ref_shape, _ = spconv_ref.rulebook_conv(idx, shape, 3, 2, 1)
+    m = ref_idx.shape[0]
+    cap = m // 2
+    for layout in ('k', 'row'):
+        oc, d_n, oi, tab, odhw = ops.rulebook_conv(t._idx, t._count, t._cap, t.grid_index(), [3, 3, 3], [2, 2, 2], [1, 1, 1],
+                                                   out_cap=cap, layout=layout)
+        assert int(d_n.item()) == m                                          # the overflow stays visible
+        assert np.array_equal(oc.cpu().numpy(), ref_idx[:cap])
+        # submanifold rulebook on the truncated level: the oracle's pairs among its first `cap` sites, nothing else
+        nbr = ops.rulebook_subm(oc, d_n, cap, oi, [3, 3, 3], layout=layout)
+        k_major = nbr if layout == 'k' else nbr[:, :27].t()
+        want = {(k, i, o) for k, i, o in _pairs_from_oracle(spconv_ref.rulebook_subm(ref_idx, ref_shape, 3)) if i < cap and o < cap}
+        assert int(k_major.max().item()) < cap
+        assert _pairs_from_nbr(k_major.contiguous(), cap) == want, layout
+        # the next strided conv reads the truncated level through the same index
+        oc2, d_n2, _, nbr2, _ = ops.rulebook_conv(oc, d_n, cap, oi, [3, 3, 3], [2, 2, 2], [1, 1, 1], out_cap=4 * m, layout=layout)
+        m2 = int(d_n2.item())
+        k2 = nbr2[:, :m2] if layout == 'k' else nbr2[:m2, :27].t()
+        ref2_idx, _, ref2_pairs = spconv_ref.rulebook_conv(ref_idx[:cap], ref_shape, 3, 2, 1)
+        assert np.array_equal(oc2[:m2].cpu().numpy(), ref2_idx)
+        assert int(k2.max().item()) < cap
+        assert _pairs_from_nbr(k2.contiguous(), m2) == _pairs_from_oracle(ref2_pairs), layout
 
 
 @pytest.mark.parametrize('cin,cout', [(5, 16), (16, 16), (16, 32), (32, 32), (32, 64), (64, 64), (64, 128), (128, 128)])
