@@ -299,7 +299,7 @@ k_conv2d_tf32(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
                 for (int w = 1; w < CT_CONSUMERS; ++w) cm = fmaxf(cm, red[w * BN + threadIdx.x]);
                 const int grp = (p.grow0 + ty0 * p.Wo + tx0) / p.gmax_rows;
                 float* addr = p.gmax + (size_t)grp * p.cout + n0 + threadIdx.x;
-                if (cm >= 0.f) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(cm));
+                if (__float_as_int(cm) >= 0) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(cm));      // sign bit: -0.0 takes atomicMin
                 else atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(cm));
             }
             tc::named_sync(1, 32 * CT_CONSUMERS);                            // red is rewritten by the next tile

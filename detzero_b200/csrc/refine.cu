@@ -147,8 +147,10 @@ __global__ void k_group_max(const float* __restrict__ x, int G, int group, int C
 // few groups x many rows (PRM memory encoder: 16 tracks x 9600 keys; GRM: 4096 points): the one-thread-per-(group, channel) kernel
 // above runs on G*C/256 CTAs (16!) and took 2.1 ms of an 8 ms refiner step.  Split every group's rows over many CTAs; the max is
 // order-independent, so an atomic max (sign-aware integer compare of the float bits, y pre-set to -inf) gives the identical result.
+// The branch tests the sign BIT: -0.0 >= 0.f holds, but as a signed int -0.0 is INT_MIN, below every negative float, so a float
+// compare would send it to atomicMax and a group whose maximum is -0.0 would keep the -inf fill.
 __device__ __forceinline__ void atomic_max_float(float* addr, float v) {
-    if (v >= 0.f) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
+    if (__float_as_int(v) >= 0) atomicMax(reinterpret_cast<int*>(addr), __float_as_int(v));
     else atomicMin(reinterpret_cast<unsigned int*>(addr), __float_as_uint(v));
 }
 __global__ void k_fill_f32(float* __restrict__ y, long long n, float v) {

@@ -54,19 +54,23 @@ def make_conv_layers(cfg, c_in, c_out, output_use_norm=False):
     return nn.Sequential(*layers)
 
 
-def _w2d(m, mode=_lib.DZ_F32):
-    """weight of Linear / Conv1d(k=1) / Conv2d(k=1) as (N, K); rounded to TF32 (RN) once for the tensor-core mode.
+def _w2d(m, mode=_lib.DZ_F32, name='weight', rows=None):
+    """weight of Linear / Conv1d(k=1) / Conv2d(k=1) (or the parameter `name` of m, rows [lo, hi) if given) as (N, K); rounded to
+    TF32 (RN) once for the tensor-core mode: the tensor core truncates the fp32 container, and a weight it truncates biases every
+    output toward zero.
     Cached on the module itself (not in a global keyed by id(): ids / addresses are recycled after a model is freed)."""
-    w = m.weight
+    w = getattr(m, name)
     ver = (w._version, w.data_ptr(), w.device)
     cache = m.__dict__.setdefault('_dz_w2d', {})
-    hit = cache.get(mode)
+    key = (mode, name, rows)
+    hit = cache.get(key)
     if hit is not None and hit[0] == ver:
         return hit[1]
-    w2 = w.detach().reshape(w.shape[0], -1).contiguous().float()
+    w2 = w.detach() if rows is None else w.detach()[rows[0]:rows[1]]
+    w2 = w2.reshape(w2.shape[0], -1).contiguous().float()
     if mode == _lib.DZ_TF32:
         w2 = ops.round_tf32(w2)
-    cache[mode] = (ver, w2)
+    cache[key] = (ver, w2)
     return w2
 
 
@@ -165,10 +169,10 @@ class MultiheadAttention(nn.Module):
         self.out_proj = nn.Linear(embed_dim, embed_dim, bias=bias)
         nn.init.xavier_uniform_(self.in_proj_weight)
 
-    def _scaled(self, lo, hi, scale_q):
+    def _scaled(self, lo, hi, scale_q, mode):
         """(W[lo:hi], scale, shift) with the query scaling folded in for the first E rows (multi_head_attention.py:207)"""
         E = self.embed_dim
-        w = self.in_proj_weight.detach()[lo:hi].contiguous().float()
+        w = _w2d(self, mode, 'in_proj_weight', (lo, hi))
         b = self.in_proj_bias.detach()[lo:hi].float() if self.in_proj_bias is not None else torch.zeros(hi - lo, device=w.device)
         s = torch.ones(hi - lo, device=w.device)
         if scale_q and lo == 0:
@@ -181,17 +185,17 @@ class MultiheadAttention(nn.Module):
         B, Pq, E = query.shape
         Pk = key.shape[1]
         if self_attention:
-            w, s, b = self._scaled(0, 3 * E, True)
+            w, s, b = self._scaled(0, 3 * E, True, mode)
             qkv = ops.linear(query.reshape(B * Pq, E), w, s, b, False, mode=mode).view(B, Pq, 3 * E)
             q, k, v = qkv[:, :, :E], qkv[:, :, E:2 * E], qkv[:, :, 2 * E:]
         else:
-            w, s, b = self._scaled(0, E, True)
+            w, s, b = self._scaled(0, E, True, mode)
             q = ops.linear(query.reshape(B * Pq, E), w, s, b, False, mode=mode).view(B, Pq, E)
-            w, s, b = self._scaled(E, 3 * E, False)
+            w, s, b = self._scaled(E, 3 * E, False, mode)
             kv = ops.linear(key.reshape(B * Pk, E), w, None, b, False, mode=mode).view(B, Pk, 2 * E)
             k, v = kv[:, :, :E], kv[:, :, E:]
         att = ops.attention(q, k, v, key_padding_mask, self.num_heads, mode=mode)
-        out = ops.linear(att.view(B * Pq, E), self.out_proj.weight.detach().float().contiguous(), None,
+        out = ops.linear(att.view(B * Pq, E), _w2d(self.out_proj, mode), None,
                          None if self.out_proj.bias is None else self.out_proj.bias.detach().float(), False, mode=mode)
         return out.view(B, Pq, E)
 
@@ -235,8 +239,8 @@ class TransformerDecoderLayer(nn.Module):
         kin = ops.add(key, kpe) if kpe is not None else key
         q2 = self.multihead_attn.forward_tokens(qin, kin, ca_mask, mode, False)
         x = self._ln(self.norm2, x, q2.reshape(B * Pq, E))
-        h = ops.linear(x, self.linear1.weight.detach().float(), None, self.linear1.bias.detach().float(), True, mode=mode)
-        h = ops.linear(h, self.linear2.weight.detach().float(), None, self.linear2.bias.detach().float(), False, mode=mode)
+        h = ops.linear(x, _w2d(self.linear1, mode), None, self.linear1.bias.detach().float(), True, mode=mode)
+        h = ops.linear(h, _w2d(self.linear2, mode), None, self.linear2.bias.detach().float(), False, mode=mode)
         x = self._ln(self.norm3, x, h)
         return x.view(B, Pq, E)
 
