@@ -1,5 +1,6 @@
 // boxgeom.cuh -- rotated-BEV box geometry shared by the NMS / IoU kernels (head.cu), the tracker / crop kernels (track.cu) and the
-// weighted box fusion of test-time augmentation (tta.cu).
+// weighted box fusion of test-time augmentation (tta.cu); the point-in-box test is shared by the object crop (track.cu) and the
+// refiner input builder (refine_data.cu).
 // Same polygon-clip algorithm as the reference (utils/detzero_utils/ops/iou3d_nms/src/iou3d_nms_kernel.cu:42-335): the keep set of
 // the NMS and the tracker's association matrix depend on its 1e-2 in-box margin and atan2 ordering, so it is re-expressed, not changed.
 #pragma once
@@ -93,4 +94,13 @@ __device__ __forceinline__ float iou3d(const float* a, const float* b) {
     const float oh = fmaxf(fminf(a_max, b_max) - fmaxf(a_min, b_min), 0.f);
     const float o3 = bev_overlap(a, b) * oh;
     return o3 / fmaxf(a[3] * a[4] * a[5] + b[3] * b[4] * b[5] - o3, 1e-6f);
+}
+
+// roiaware_pool3d_kernel.cu:16-36 (check_pt_in_box3d, GPU margin 1e-5; the z test has no margin)
+__device__ __forceinline__ bool pt_in_box3d(float x, float y, float z, const float* b) {
+    if (fabsf(z - b[2]) > b[5] / 2.0f) return false;
+    const float sx = x - b[0], sy = y - b[1];
+    const float cosa = cosf(-b[6]), sina = sinf(-b[6]);
+    const float lx = sx * cosa + sy * (-sina), ly = sx * sina + sy * cosa;
+    return (fabsf(lx) < b[3] / 2.0f + 1e-5f) & (fabsf(ly) < b[4] / 2.0f + 1e-5f);
 }

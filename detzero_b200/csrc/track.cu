@@ -51,15 +51,6 @@ extern "C" int dz_boxes_pairwise(const float* boxes_a, int na, int lda, const fl
 }
 
 // ---- object crop ----------------------------------------------------------------------------------------------------------
-// roiaware_pool3d_kernel.cu:16-36 (check_pt_in_box3d, GPU margin 1e-5; the z test has no margin)
-__device__ __forceinline__ bool pt_in_box3d(float x, float y, float z, const float* b) {
-    if (fabsf(z - b[2]) > b[5] / 2.0f) return false;
-    const float sx = x - b[0], sy = y - b[1];
-    const float cosa = cosf(-b[6]), sina = sinf(-b[6]);
-    const float lx = sx * cosa + sy * (-sina), ly = sx * sina + sy * cosa;
-    return (fabsf(lx) < b[3] / 2.0f + 1e-5f) & (fabsf(ly) < b[4] / 2.0f + 1e-5f);
-}
-
 static constexpr int CROP_CHUNK = 2048;            // points per block
 
 // pass 1 (write_idx == 0): counts[t][chunk] = points of the chunk inside box t;  pass 2: ordered indices, starting at the

@@ -143,3 +143,90 @@ def grm_inputs(seed, B=2, mem=4096, q=3, qpts=256):
 def crm_inputs(seed, B=2, boxes=200, pts=256, dims=32):
     g = np.random.default_rng(seed)
     return {'conf_points': torch.from_numpy(g.normal(0, 1, (B, boxes, pts, dims)).astype(np.float32))}
+
+
+# ---- a tracked sequence for the refiner input builder (detzero_b200/refine/data.py)
+def _rz(a):
+    c, s = np.cos(a), np.sin(a)
+    return np.array([[c, -s, 0.0], [s, c, 0.0], [0.0, 0.0, 1.0]])
+
+
+def synthetic_sequence(seed, frames=20, tracks=8, L=200, n_background=20000, max_pts=3000, origin=(5000.0, -3000.0, 50.0),
+                       min_len=1, enlarge=1.1, margin=1e-3, ego_step=1.0, max_speed=0.4, lengths=None, cls=None):
+    """A seeded tracked sequence: ego poses with world translations around ``origin`` (about 5 km) and yaw wrapping through +-pi,
+    objects moving on smooth paths (headings wrapping too), 0..~max_pts points on and inside each box over a synth_waymo_cloud
+    background, and no point within ``margin`` of any enlarged box face, so crop membership is unambiguous.
+    Returns a dict: frames (N, 6) f32 collated rows [b=frame, x, y, z, tanh(i), elongation] in the lidar frame, frame_offsets (F+1),
+    poses (F, 4, 4) f64, and the TrackBatch fields as numpy arrays (boxes (B, L, 7) f64 world, frame_of_box, scores, box_num, cls,
+    track_uid).  ``lengths`` / ``cls`` fix the box count / class of each track (default: random)."""
+    from .det.dataset import synth_waymo_cloud
+    g = np.random.default_rng([int(seed), 0x5E9])
+    F = int(frames)
+    yaw0 = np.pi - 0.4
+    ego_yaw = yaw0 + 0.8 * np.arange(F) / max(F - 1, 1)
+    ego_xy = np.cumsum(np.stack([np.cos(ego_yaw), np.sin(ego_yaw)], 1) * ego_step, 0)
+    poses = np.zeros((F, 4, 4))
+    for f in range(F):
+        tilt = np.array([[1, 0, 0], [0, np.cos(0.004), -np.sin(0.004)], [0, np.sin(0.004), np.cos(0.004)]])
+        poses[f, :3, :3] = _rz(ego_yaw[f]) @ tilt
+        poses[f, :3, 3] = np.asarray(origin) + [ego_xy[f, 0], ego_xy[f, 1], 0.01 * f]
+        poses[f, 3, 3] = 1
+    B = int(tracks)
+    boxes = np.zeros((B, L, 7))
+    fob = np.zeros((B, L), np.int32)
+    scores = np.zeros((B, L), np.float32)
+    box_num = np.zeros(B, np.int32)
+    cls = (g.integers(1, 4, B) if cls is None else np.asarray(cls)).astype(np.int32)
+    dims_by_cls = np.array([[4.7, 2.0, 1.6], [0.9, 0.9, 1.8], [1.9, 0.8, 1.7]])
+    obj_pts = [[] for _ in range(F)]
+    frame_boxes = [[] for _ in range(F)]
+    for b in range(B):
+        n = int(g.integers(min(min_len, F), min(L, F) + 1)) if lengths is None else int(lengths[b])
+        start = int(g.integers(0, F - n + 1))
+        box_num[b] = n
+        dims = dims_by_cls[cls[b] - 1] * g.uniform(0.9, 1.1, 3)
+        r0, a0 = g.uniform(6, 45), g.uniform(-np.pi, np.pi)
+        c0 = poses[start, :3, 3] + [r0 * np.cos(a0), r0 * np.sin(a0), -1.2]
+        h0, speed, turn = g.uniform(-np.pi, np.pi), g.uniform(0, max_speed), g.uniform(-0.05, 0.05)
+        pts_n = np.where(g.random(n) < 0.1, 0, np.exp(g.uniform(0, np.log(max_pts), n)).astype(int))
+        for j in range(n):
+            f = start + j
+            h = h0 + turn * j
+            c = c0 + speed * j * np.array([np.cos(h), np.sin(h), 0.0]) + poses[f, :3, 3] - poses[start, :3, 3]
+            boxes[b, j] = [c[0], c[1], c[2], dims[0], dims[1], dims[2], h]
+            fob[b, j] = f
+            scores[b, j] = np.float32(g.uniform(0.05, 0.95))
+            u = g.uniform(-0.48, 0.48, (pts_n[j], 3)) * dims                       # inside the (unenlarged) box
+            u[: pts_n[j] // 3, 2] = -dims[2] / 2 + 0.02                            # some on the bottom face
+            w = u @ _rz(h).T + c
+            obj_pts[f].append(np.concatenate([w, g.uniform(0, 1, (len(w), 1))], 1))
+            frame_boxes[f].append(boxes[b, j])
+    rows, offsets = [], [0]
+    from scipy.spatial import cKDTree
+    for f in range(F):
+        bg = synth_waymo_cloud(seed=int(seed) * 1000 + f, n_target=n_background)
+        P = poses[f]
+        bgw = np.concatenate([bg[:, :3].astype(np.float64) @ P[:3, :3].T + P[:3, 3], bg[:, 3:4]], 1)
+        pw = np.concatenate([bgw] + obj_pts[f], 0) if obj_pts[f] else bgw
+        keep = np.ones(len(pw), bool)
+        if frame_boxes[f]:
+            fb = np.array(frame_boxes[f])
+            tree = cKDTree(pw[:, :2])
+            for bx, idx in zip(fb, tree.query_ball_point(fb[:, :2], np.linalg.norm(fb[:, 3:5] * enlarge, axis=1) / 2 + 0.1)):
+                idx = np.asarray(idx, np.int64)
+                if not len(idx):
+                    continue
+                rel = (pw[idx, :3] - bx[:3]) @ _rz(bx[6])                          # box frame
+                half = bx[3:6] * enlarge / 2
+                d = np.abs(rel) - half
+                outside = np.max(d, 1)
+                keep[idx[np.abs(outside) < margin * 3]] = False                   # within a few margins of an enlarged face
+        pw = pw[keep]
+        loc = ((pw[:, :3] - P[:3, 3]) @ P[:3, :3]).astype(np.float32)
+        r = np.zeros((len(pw), 6), np.float32)
+        r[:, 0], r[:, 1:4], r[:, 4], r[:, 5] = f, loc, np.tanh(pw[:, 3]), 0.0
+        rows.append(r)
+        offsets.append(offsets[-1] + len(r))
+    return {'frames': np.concatenate(rows, 0), 'frame_offsets': np.asarray(offsets, np.int64), 'poses': poses, 'boxes': boxes,
+            'frame_of_box': fob, 'scores': scores, 'box_num': box_num, 'cls': cls,
+            'track_uid': (np.arange(B, dtype=np.int64) * 7919 + int(seed) * 104729 + 1)}

@@ -240,6 +240,38 @@ int dz_crop_points_in_boxes(const float* points, int n_pts, int pt_stride, const
 int dz_points_in_boxes_mask(const float* points, int n_pts, int pt_stride, const float* boxes, int n_boxes, int ldb,
                             int32_t* mask, dz_stream_t stream);
 
+/* ---- refiner inputs (SURVEY.md 8f row 2), csrc/refine_data.cu -------------------------------------------------------------- */
+/* Builds the eval inputs of the refiner modules for B tracks of up to L box slots straight from the collated frames, in one call per
+ * kind: PRM (kind 0) = WaymoPositionDataset.extract_track_feature (refining/detzero_refine/datasets/waymo/waymo_position_dataset.py:31-184),
+ * CRM (kind 1) = WaymoConfidenceDataset.extract_track_feature (waymo_confidence_dataset.py:59-162), GRM (kind 2) =
+ * WaymoGeometryDataset.extract_track_feature (waymo_geometry_dataset.py:26-154), fused with the object crop of
+ * daemon/prepare_object_data.py:241-327 (enlarged boxes, roiaware_pool3d_kernel.cu:23-36 test) and sample_points
+ * (refining/detzero_refine/utils/data_utils.py:12-30).  The sampling is keyed and deterministic and the geometry float64: see the
+ * header of csrc/refine_data.cu for the exact key function and the other deliberate deviations.
+ *   points (rows of pt_stride >= 5 floats [b, x, y, z, tanh(i), ...], lidar frame) with frame_offsets (n_frames + 1); max_frame_points
+ *   (host) >= the largest frame.  poses (n_frames, 4, 4) f64 lidar -> world.  Tracks: boxes (B, L, 7) f64 world, frame_of_box (B, L),
+ *   scores (B, L) f32, box_num (B) (1..L), cls (B) (1-based, the cyclist one-hot), track_uid (B) i64.
+ *   crop = 0: every point of the box's frame belongs to the box (per-object point sets packed one frame per box).
+ *   kq / km / nq: query points, memory points, GRM query boxes (QUERY_POINTS_NUM, MEMORY_POINTS_NUM, QUERY_NUM).
+ * Outputs (f32 unless noted), PRM: q_pts (B, L, kq, C) pos_query_points, m_pts (B, L, km, C) pos_memory_points, C = 32 (+3 with_class),
+ *   traj (B, L, 7) pos_trajectory, box_f (B, L) padding_mask, track_f (B, 7) pos_init_box.  CRM: q_pts (B, L, kq, 32) conf_points,
+ *   box_f (B, L) conf_score (-1 padded).  GRM: q_pts (B, q_out, kq, 4) geo_query_points, m_pts (B, km, 11) geo_memory_points,
+ *   traj (B, L, 7) world boxes, box_f (B, q_out, 7) geo_query_boxes, query_num (B) int32 geo_query_num.
+ *   counts (B, L) int32 crop counts and sel (the sorted selected ranks: PRM (B, L, kq + km), CRM (B, L, kq), GRM (B, nq * kq + km))
+ *   are optional outputs (NULL: kept in the workspace). */
+size_t dz_refine_inputs_ws_bytes(int kind, int B, int L, int max_frame_points, int kq, int km, int nq);
+int dz_refine_inputs(int kind, const float* points, int pt_stride, const int32_t* frame_offsets, int n_frames, int max_frame_points,
+                     const double* poses, const double* boxes, const int32_t* frame_of_box, const float* scores,
+                     const int32_t* box_num, const int32_t* cls, const int64_t* track_uid, int B, int L, int kq, int km, int nq,
+                     int q_out, int with_class, double enlarge_scale, int crop_on_bev, int crop, unsigned long long seed,
+                     float* q_pts, float* m_pts, float* traj, float* box_f, float* track_f, int32_t* query_num, int32_t* counts,
+                     int32_t* sel, void* ws, size_t ws_bytes, dz_stream_t stream);
+/* revert_to_each_frame: PRM (kind 0) pred (B, L, 7) in the init-box frame -> world (box_coords_transform, data_utils.py) -> lidar
+ * (world_to_lidar) (waymo_position_dataset.py:257-286); GRM (kind 2) pred (B, 7): its size written into each world box -> lidar
+ * (waymo_geometry_dataset.py:160-186).  lidar, world (B, L, 7) f64, rows past box_num zero. */
+int dz_refine_revert(int kind, const float* pred, const double* poses, int n_frames, const double* boxes, const int32_t* frame_of_box,
+                     const int32_t* box_num, int B, int L, double* lidar, double* world, dz_stream_t stream);
+
 /* ---- test-time augmentation (CenterPoint TTA) ------------------------------------------------------------- */
 /* A view is 4 host floats [op, p1, p2, p3]: DZ_TTA_ORIGINAL; DZ_TTA_FLIP_X (y = -y); DZ_TTA_FLIP_Y (x = -x); DZ_TTA_FLIP_XY;
  * DZ_TTA_ROT with p1, p2 = cos, sin of the float32 angle (float32 torch on the CPU, as the reference computes them) and, for
