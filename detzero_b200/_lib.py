@@ -44,6 +44,7 @@ _SIGS = {
     'dz_rulebook_schedule_ws_bytes': (sz, [ci]),
     'dz_rulebook_schedule': (ci, [vp, ci, vp, vp, vp, sz, ci, vp, vp]),
     'dz_spconv_fwd': (ci, [vp, ci, ci, vp, ci, ci, vp, vp, ci, vp, vp, vp, vp, ci, vp, ci, ci, vp]),
+    'dz_round_tf32': (ci, [vp, vp, ci, ci, vp, vp]),
     'dz_rulebook_transpose': (ci, [vp, ci, ci, vp, vp, ci, vp]),
     'dz_spconv_wgrad': (ci, [vp, ci, vp, ci, ci, vp, ci, vp, ci, vp, vp]),
     'dz_spconv_fwd_planes': (ci, [vp, ci, ci, vp, ci, ci, vp, vp, ci, vp, vp, vp, vp, ci, vp, ci, ci, vp, vp]),

@@ -38,7 +38,8 @@ struct StCfg {
     static constexpr int PLANES = SPLIT ? 2 : 1;               // operand pieces: [A_hi | A_lo] and [W_hi | W_lo] under SPLIT
     static constexpr int W_BYTES = COUT * 128;
     static constexpr int STAGE_BYTES = PLANES * (ST_A_BYTES + W_BYTES);
-    // Cout = 128 only occurs with K = 3 (conv_out): few k-steps, so a shallow ring suffices
+    // Cout = 128: the 128 x 128 B tile is the largest stage; VoxelBackBone8x runs it only as conv_out (K = 3), VoxelResBackBone8x
+    // also as spconv4 (cin = 64) and the res4 blocks (K = 27, with a residual).  Three stages still cover one step's MMAs
     static constexpr int STAGES = SPLIT ? 3 : (COUT >= 128 ? 3 : 4);
     // PW producer warps per stage: warp w gathers its 128/PW rows of the steps it = s, s+STAGES, ... into stage s = (w-8) % STAGES
     // (one warp alone cannot keep enough cp.async gathers in flight; the register gather of SPLIT keeps 8 loads per lane in
@@ -343,4 +344,22 @@ int dz_spconv_fwd_tc(const float* in, int cin, int in_rows, const int32_t* nbr, 
 #undef DZ_ST
     dz_set_error("dz_spconv_fwd(%s): (cin=%d, cout=%d) not instantiated", name, cin, cout);
     return DZ_ERR_UNSUPPORTED;
+}
+
+// RN_tf32 (ties to even) of the first min(*d_n, cap) rows: the same bits as ops.round_tf32, non-finite values kept
+__global__ void __launch_bounds__(256) k_round_tf32(const float* __restrict__ x, const int* __restrict__ d_n, int cap, int c, float* __restrict__ out) {
+    const int n = d_n ? min(*d_n, cap) : cap;
+    const long long total = (long long)n * c;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const uint32_t u = __float_as_uint(x[i]);
+        out[i] = (u & 0x7f800000u) == 0x7f800000u ? __uint_as_float(u) : __uint_as_float((u + 0xfffu + ((u >> 13) & 1u)) & ~0x1fffu);
+    }
+}
+
+extern "C" int dz_round_tf32(const float* x, const int* d_n, int cap, int c, float* out, dz_stream_t stream) {
+    DZ_CHECK_ARG(x && out && cap >= 1 && c >= 1);
+    const int blocks = max(1, min(dz_cdiv((long long)cap * c, 256), DZ_NUM_SMS * 8));
+    k_round_tf32<<<blocks, 256, 0, (cudaStream_t)stream>>>(x, d_n, cap, c, out);
+    DZ_LAUNCH_CHECK();
+    return DZ_OK;
 }

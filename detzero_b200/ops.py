@@ -261,6 +261,18 @@ def round_tf32(t):
     return ((i + 0xFFF + lsb) & ~0x1FFF).view(torch.float32)
 
 
+def round_tf32_rows(x, d_n):
+    """RN_tf32 of the first *d_n rows of an fp32 (rows, c) tensor on the device (the bits of round_tf32); rows beyond are left
+    uninitialised"""
+    _need_cuda(x)
+    rows, c = x.shape
+    out = torch.empty((rows, c), dtype=torch.float32, device=x.device)
+    if rows:
+        check(lib().dz_round_tf32(_p(_f32c(x)), _p(d_n), rows, c, _p(out), _stream()), 'round_tf32')
+        _count(1)
+    return out
+
+
 def spconv_fwd(feats, nbr, d_n_out, out_cap, weight_packed, scale, shift, residual, relu, mode=_lib.DZ_F32, out=None,
                d_n_in=None, kshape=None, row_order=None, layout=None, tab_tiles=None):
     """feats (in_cap, cin); weight_packed per pack_spconv_weight; kshape = (K, cin, cout).

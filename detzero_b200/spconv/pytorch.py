@@ -47,6 +47,7 @@ class SparseConvTensor:
         self._n = n_host
         self._index = index
         self._planes = 0            # 0: fp32 (rows, C) features; 1 / 2: bf16 operand planes (rows, planes*C), csrc/spconv_bf16.cu
+        self._tf32 = False          # fp32 features known to be TF32-representable (written by a DZ_TF32 layer's rounding epilogue)
 
     # ---- spconv-visible surface ---------------------------------------------------------------------------
     def num(self):
@@ -89,6 +90,8 @@ class SparseConvTensor:
             t._count = torch.full((1,), t._cap, dtype=torch.int32, device=new_features.device)
         t._feat = new_features
         t._planes = 0
+        t._tf32 = False
+        t.__dict__.pop('_tf32_cache', None)
         return t
 
     def dense(self, channels_first=True):
@@ -106,12 +109,26 @@ class SparseConvTensor:
                                                      self.spatial_shape, with_perm=True)
         return self._index
 
-    def _like(self, feat, planes=0):
+    def _like(self, feat, planes=0, tf32=False):
         t = SparseConvTensor.__new__(SparseConvTensor)
         t.__dict__.update(self.__dict__)
         t._feat = feat
         t._planes = planes
+        t._tf32 = tf32
+        t.__dict__.pop('_tf32_cache', None)
         return t
+
+    def _as_tf32(self):
+        """this tensor's fp32 features RN-rounded to TF32 (rounded once per tensor): a DZ_TF32 layer reads its input operand by
+        truncation, which would bias every unrounded input toward zero.  The output of a DZ_TF32 layer is rounded by its epilogue
+        and passes through as it is; so does everything else in a TF32 backbone but its input, the VFE's voxel means"""
+        if getattr(self, '_tf32', False):
+            return self._feat
+        hit = self.__dict__.get('_tf32_cache')
+        if hit is None or hit[0] is not self._feat:
+            hit = (self._feat, ops.round_tf32_rows(self._feat, self._count))
+            self._tf32_cache = hit
+        return hit[1]
 
     def _as_planes(self, planes, c_pad):
         """this tensor's features as bf16 operand planes (converted once per tensor if they are fp32)"""
@@ -319,16 +336,19 @@ class _SparseConv(SparseModule):
         else:
             if x._planes or (residual is not None and residual._planes):
                 raise RuntimeError('a bf16-plane tensor cannot feed a %s layer: use one COMPUTE_MODE per backbone' % self.mode)
-            feat, res = x._feat, (None if residual is None else residual._feat)
+            feat = x._as_tf32() if mode == _lib.DZ_TF32 else x._feat
+            res = None if residual is None else residual._feat           # added in fp32 by the epilogue: no rounding
+        tf32 = mode == _lib.DZ_TF32                      # the TF32 epilogue rounds its output
         if self.subm:
             out = ops.spconv_fwd(feat, nbr, x._count, x._cap, self.packed_weight(mode), scale, shift, res, relu, mode,
                                  kshape=self.kshape, row_order=order, layout=lay, tab_tiles=rule.tab_tiles)
-            return x._like(out, planes)
+            return x._like(out, planes, tf32)
         out = ops.spconv_fwd(feat, nbr, rule.d_n_out, rule.out_cap, self.packed_weight(mode), scale, shift, None,
                              relu, mode, d_n_in=x._count, kshape=self.kshape, row_order=order, layout=lay, tab_tiles=rule.tab_tiles)
         t = SparseConvTensor(out, rule.out_idx, rule.out_dhw, x.batch_size, indice_dict=x.indice_dict,
                              count=rule.d_n_out, n_host=None, index=rule.out_index)
         t._planes = planes
+        t._tf32 = tf32
         t._producer = self
         return t
 

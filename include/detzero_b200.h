@@ -143,6 +143,10 @@ int dz_spconv_fwd(const float* in, int cin, int in_rows, const int32_t* nbr, int
                   const int32_t* row_order, const int* d_n_out,
                   int out_cap, const float* weight, const float* scale, const float* shift,
                   const float* residual, int relu, float* out, int cout, int mode, dz_stream_t stream);
+/* out[r, :] = RN_tf32(x[r, :]) (round to nearest, ties to even, 10 explicit mantissa bits) for r < min(*d_n, cap); rows beyond
+ * are left alone.  DZ_TF32 reads its input operand by truncation, so an fp32 tensor that enters a DZ_TF32 layer without having
+ * come out of one (whose epilogue rounds) is rounded once with this first.  in == out is allowed. */
+int dz_round_tf32(const float* x, const int* d_n, int cap, int c, float* out, dz_stream_t stream);
 
 /* Backward of dz_spconv_fwd on the same k-major table (exact fp32; SURVEY.md 8f row 1; the reference trains through spconv's
  * autograd, detection/tools/train_utils.py:59-68).  dz_rulebook_transpose: nbrT (K, cap_in), nbrT[k][j] = o for every pair

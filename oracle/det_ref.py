@@ -211,7 +211,9 @@ def decode_bbox_from_heatmap(maps, pc_range, voxel_size, fmap_stride, K, score_t
     rc = _transpose_and_gather_feat(rot_cos, inds).view(B, Kk, 1)
     cz = _transpose_and_gather_feat(maps['center_z'], inds).view(B, Kk, 1)
     dm = _transpose_and_gather_feat(dim, inds).view(B, Kk, 3)
-    angle = torch.atan2(rs, rc)
+    # float32 atan2 rounded once from float64: the correctly rounded heading, on every CPU.  torch's float32 atan2 kernels differ
+    # by an ulp between its scalar and vectorised code paths, so a float32 call would tie the oracle to the CPU it runs on
+    angle = torch.atan2(rs.double(), rc.double()).float()
     xs = xs.view(B, Kk, 1) + center[:, :, 0:1]
     ys = ys.view(B, Kk, 1) + center[:, :, 1:2]
     xs = xs * fmap_stride * voxel_size[0] + pc_range[0]

@@ -13,7 +13,7 @@ import pytest
 import torch
 
 from oracle import det_ref, spconv_ref
-from tests import util
+from tests import spconv_arith, util
 from tests.test_gpu_bench_config import POST, _check_against_oracle, _settle
 from detzero_b200 import _lib
 
@@ -236,8 +236,9 @@ def _crop(coords, n):
 @pytest.mark.gpu
 @pytest.mark.parametrize('layer', LAYERS, ids=[l[0] for l in LAYERS])
 def test_plane_kernel_layer_at_scale(cuda, frames, layer):
-    """module path (forward_fused, scheduled, tile-major table) in bf16x2 and bf16 against a float64 restatement on the same input;
-    scheduled, unscheduled and tile-major launches give the same bits; capacity rows beyond the count are untouched"""
+    """module path (forward_fused, scheduled; tile-major table in the bf16 modes) in every compute mode against a float64
+    restatement on the same input, element by element within the bounds of tests/spconv_arith.py; in the bf16 modes scheduled,
+    unscheduled and tile-major launches give the same bits and capacity rows beyond the count are untouched"""
     from detzero_b200 import ops
     from detzero_b200.spconv import pytorch as spconv
     name, cin, cout, subm, ks, stride, pad, res = layer
@@ -261,20 +262,36 @@ def test_plane_kernel_layer_at_scale(cuda, frames, layer):
     scale = torch.from_numpy(g.uniform(0.5, 1.5, cout).astype(np.float32))
     shift = torch.from_numpy(g.normal(0, 0.1, cout).astype(np.float32))
     r = torch.from_numpy(g.normal(0, 1, (n_out, cout)).astype(np.float32)) if res else None
-    want = spconv_ref.sparse_conv_native(f.double(), w.double(), pairs, n_out) * scale.double() + shift.double()
-    if res:
-        want = want + r.double()
-    want = torch.relu(want)
+    K = int(np.prod(kshape))
+    native = {}
+
+    def reference(mode):
+        """float64 x . w epilogue of the layer's input and residual as the mode stores them (bf16: the planes, summed; tf32: the
+        input RN-rounded once) and sum |x| |w|"""
+        kind = mode if mode in ('bf16x2', 'bf16', 'tf32') else 'fp32'
+        if kind not in native:
+            if kind in spconv_arith.PLANES:
+                fs = torch.stack(spconv_arith.split_bf16(f)[:spconv_arith.PLANES[kind]]).double().sum(0)
+            else:
+                fs = (spconv_arith.rn_tf32(f) if kind == 'tf32' else f).double()
+            native[kind] = (spconv_ref.sparse_conv_native(fs, w.double(), pairs, n_out),
+                            spconv_ref.sparse_conv_native(fs.abs(), w.double().abs(), pairs, n_out))
+        y, A = native[kind]
+        rs = None
+        if res:
+            rs = sum(p.double() for p in spconv_arith.residual_pieces(mode, r))
+        want = y * scale.double() + shift.double() + (0 if rs is None else rs)
+        return torch.relu(want), A, (None if rs is None else rs.abs())
     cap = n_in + (SPARE if subm else 0)
     fc = torch.full((cap, cin), 1e3)
     fc[:n_in] = f
     ic = torch.zeros((cap, 4), dtype=torch.int32)
     ic[:n_in] = torch.from_numpy(idx)
     d_n = torch.tensor([n_in], dtype=torch.int32, device=cuda)
-    for mode, tol in (('bf16x2', 2e-5), ('bf16', 1e-2)):
+    for mode in spconv_arith.MODES:
         if mode not in _lib.MODES:
             pytest.skip('mode %s not built' % mode)
-        P = _lib.PLANES[_lib.MODES[mode]]
+        P = _lib.PLANES.get(_lib.MODES[mode], 0)
         x = spconv.SparseConvTensor(fc.to(cuda), ic.to(cuda), SPARSE_SHAPE, 1, count=d_n, n_host=n_in)
         if subm:
             conv = spconv.SubMConv3d(cin, cout, ks, bias=False, indice_key='k', mode=mode)
@@ -292,15 +309,20 @@ def test_plane_kernel_layer_at_scale(cuda, frames, layer):
         with torch.no_grad():
             y = conv.forward_fused(x, sc, sh, resid, True)
         rule = x.indice_dict['k']
-        assert rule.order is not None and rule.tab_tiles is not None, name       # the module ran the scheduled tile-major path
+        if mode != 'fp32':                                                       # the module ran the scheduled (tile-major) path
+            assert rule.order is not None and (rule.tab_tiles is not None or not P), name
         d_out = x._count if subm else rule.d_n_out
         out_cap = x._cap if subm else rule.out_cap
         assert int(d_out.item()) == n_out
         if not subm:
             assert np.array_equal(rule.out_idx[:n_out].cpu().numpy(), out_idx), name
-        got = y.features
+        got = y.features.cpu()
         assert got.shape == (n_out, cout)
-        assert util.rel_err(got.cpu(), want) < tol, (name, mode, util.rel_err(got.cpu(), want))
+        want, A, r_abs = reference(mode)
+        util.assert_within(got, want, spconv_arith.bound(mode, K, cin, A, scale, shift, r_abs, got.double().abs()),
+                           '%s %s' % (name, mode))
+        if not P:
+            continue
         # the same launch unscheduled, scheduled, and scheduled from the tile-major table: bit for bit, spare rows untouched
         fp = x._as_planes(P, 8 if cin <= 8 else cin)
         rp = None if resid is None else resid._as_planes(P, cout)

@@ -46,3 +46,33 @@ from detzero_b200.synthetic import model_cfg, CLASS_NAMES    # noqa: E402,F401  
 def rel_err(a, b):
     a, b = torch.as_tensor(a).double(), torch.as_tensor(b).double()
     return ((a - b).abs().max() / b.abs().max().clamp_min(1e-30)).item()
+
+
+def assert_within(got, ref, bound, what):
+    """|got - ref| <= bound element-wise; NaN exactly where ref is NaN.  Returns the largest err / bound; a failure reports it and
+    where it occurs"""
+    got = got.to(torch.float64)
+    ref, bound = ref.to(got.device), bound.to(got.device)
+    gn, rn = torch.isnan(got), torch.isnan(ref)
+    if not torch.equal(gn, rn):
+        i = np.unravel_index(int((gn != rn).to(torch.uint8).argmax()), tuple(got.shape))
+        raise AssertionError('%s: NaN pattern differs from torch at %s (got %r, ref %r)' % (what, i, got[i].item(), ref[i].item()))
+    err = torch.where(rn, torch.zeros_like(got), (got - ref).abs())
+    bound = torch.where(rn, torch.zeros_like(bound), bound)
+    ratio = torch.where(err == 0, torch.zeros_like(err), err / bound)      # bound == 0 and err > 0: inf
+    ratio = torch.nan_to_num(ratio, nan=float('inf'))
+    worst = float(ratio.max()) if ratio.numel() else 0.0
+    if not worst <= 1.0:
+        i = np.unravel_index(int(ratio.argmax()), tuple(got.shape))
+        raise AssertionError('%s: largest err/bound %.3g at %s (err %.3g, bound %.3g, got %r, ref %r)'
+                             % (what, worst, i, err[i].item(), bound[i].item(), got[i].item(), ref[i].item()))
+    return worst
+
+
+def assert_equal_signed(got, ref, what):
+    """bit-level agreement up to NaN payloads: equal values and the same sign of zero"""
+    got, ref = got.cpu(), ref.cpu().to(got.dtype)
+    same = (got == ref) & (torch.signbit(got) == torch.signbit(ref))
+    if not bool(same.all()):
+        i = np.unravel_index(int((~same).to(torch.uint8).argmax()), tuple(got.shape))
+        raise AssertionError('%s: first difference at %s (got %r, torch %r)' % (what, i, got[i].item(), ref[i].item()))
