@@ -66,6 +66,8 @@ _SIGS = {
     'dz_crop_points_ws_bytes': (sz, [ci, ci]),
     'dz_crop_points_in_boxes': (ci, [vp, ci, ci, vp, ci, ci, vp, ci, vp, vp, sz, vp]),
     'dz_points_in_boxes_mask': (ci, [vp, ci, ci, vp, ci, ci, vp, vp]),
+    'dz_track_sequences_ws_bytes': (sz, [ci, ci, ci, ci, ci]),
+    'dz_track_sequences': (ci, [vp, vp, vp, vp, ci, ci, ci, vp, ci, ci, vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]),
     'dz_refine_inputs_ws_bytes': (sz, [ci, ci, ci, ci, ci, ci, ci]),
     'dz_refine_inputs': (ci, [ci, vp, ci, vp, ci, ci, vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, ctypes.c_double, ci, ci,
                               ctypes.c_uint64, vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]),

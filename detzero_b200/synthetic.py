@@ -230,3 +230,68 @@ def synthetic_sequence(seed, frames=20, tracks=8, L=200, n_background=20000, max
     return {'frames': np.concatenate(rows, 0), 'frame_offsets': np.asarray(offsets, np.int64), 'poses': poses, 'boxes': boxes,
             'frame_of_box': fob, 'scores': scores, 'box_num': box_num, 'cls': cls,
             'track_uid': (np.arange(B, dtype=np.int64) * 7919 + int(seed) * 104729 + 1)}
+
+
+def synthetic_detections(seed, frames=199, objects=300, false_positives=40, K=500, miss=0.1, chain=0, origin=(5000.0, -3000.0, 50.0)):
+    """Seeded gathered detections of one sequence for the tracker, laid out so that no association, merge or overlap-filter decision
+    sits near its threshold: objects drive in lanes 12 m apart (one class and speed per lane: parked, slow and fast vehicles,
+    pedestrians, cyclists), 30 / 10 / 5 m apart within a lane, each alive over a random run of frames, detected with 3 cm / 0.01 rad
+    jitter, dropped with probability ``miss``, and with one low-score stretch (score < 0.1) each; ``false_positives`` boxes per frame
+    far from every lane, one in ten above the score threshold; ``chain`` static pedestrians 0.73 m apart without jitter, so that
+    each detection overlaps three tracks (one large association component).  The ego drives through the scene.
+    Returns boxes (F, K, 9) f32 lidar rows [x, y, z, dx, dy, dz, heading, score, label], counts (F), poses (F, 4, 4) and the ground
+    truth gt_id (F, K) (-1 for a false positive)."""
+    g = np.random.default_rng([int(seed), 0x7AC])
+    F = int(frames)
+    yaw = 0.3 + 0.2 * np.arange(F) / max(F - 1, 1)
+    poses = np.zeros((F, 4, 4))
+    for f in range(F):
+        poses[f, :3, :3] = _rz(yaw[f])
+        poses[f, :3, 3] = np.asarray(origin) + [2.0 * f, 0.5 * f, 0.0]
+        poses[f, 3, 3] = 1
+    kinds = [(1, 0.0, 30.), (1, 1.0, 30.), (1, 10.0, 30.), (2, 1.2, 5.), (3, 4.0, 10.)]     # class, speed, spacing
+    dims_by_cls = np.array([[4.7, 2.0, 1.6], [0.9, 0.6, 1.8], [1.9, 0.8, 1.7]])
+    dets = [[] for _ in range(F)]
+    lane, placed = 0, 0
+    while placed < objects:
+        cls, speed, gap = kinds[lane % len(kinds)]
+        direction = 1.0 if lane % 2 == 0 else -1.0
+        for k in range(min(8, objects - placed)):
+            start = int(g.integers(0, max(F - 8, 1)))
+            end = int(g.integers(min(start + 8, F), F + 1))
+            dims = dims_by_cls[cls - 1] * g.uniform(0.95, 1.05, 3)
+            low0 = int(g.integers(start, end))
+            low1 = low0 + int(g.integers(1, 4))
+            x0 = k * gap * 1.2 + g.uniform(0, 0.2 * gap) - 120.
+            for f in range(start, end):
+                if g.random() < miss:
+                    continue
+                c = np.array([x0 + direction * speed * 0.1 * f, 12.0 * lane - 60., -1.0]) + g.normal(0, 0.03, 3)
+                h = (0.0 if direction > 0 else np.pi - 1e-3) + g.normal(0, 0.01)
+                sc = g.uniform(0.02, 0.09) if low0 <= f < low1 else g.uniform(0.3, 0.95)
+                dets[f].append((c, dims * (1 + g.normal(0, 0.005, 3)), h, sc, cls, placed + k))
+        placed += min(8, objects - placed)
+        lane += 1
+    for k in range(chain):
+        for f in range(F):
+            dets[f].append((np.array([-150. + 0.73 * k, -90., -1.0]), dims_by_cls[1], 0.0, 0.8, 2, objects + k))
+    for f in range(F):
+        for _ in range(int(false_positives)):
+            c = np.array([g.uniform(-600, 600), g.uniform(300, 900), -1.0])
+            cls = int(g.integers(1, 4))
+            sc = g.uniform(0.1, 0.3) if g.random() < 0.1 else g.uniform(0.01, 0.09)
+            dets[f].append((c, dims_by_cls[cls - 1], g.uniform(-np.pi, np.pi), sc, cls, -1))
+    boxes = np.zeros((F, K, 9), np.float32)
+    gt_id = np.full((F, K), -1, np.int64)
+    counts = np.zeros(F, np.int32)
+    for f in range(F):
+        order = g.permutation(len(dets[f]))[:K]
+        R, t = poses[f, :3, :3], poses[f, :3, 3]
+        for i, j in enumerate(order):
+            c, d, h, sc, cls, gid = dets[f][j]
+            lw = (np.asarray(origin) + c - t) @ R                               # c is relative to the origin
+            hl = h - yaw[f]
+            boxes[f, i] = [*lw, *d, np.arctan2(np.sin(hl), np.cos(hl)), sc, cls]
+            gt_id[f, i] = gid
+        counts[f] = len(order)
+    return {'boxes': boxes, 'counts': counts, 'poses': poses, 'gt_id': gt_id}

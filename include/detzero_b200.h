@@ -244,6 +244,21 @@ int dz_crop_points_in_boxes(const float* points, int n_pts, int pt_stride, const
 int dz_points_in_boxes_mask(const float* points, int n_pts, int pt_stride, const float* boxes, int n_boxes, int ldb,
                             int32_t* mask, dz_stream_t stream);
 
+/* ---- the DetZero tracker (csrc/tracker.cu) ------------------------------------------------------------------------------ */
+/* S sequences of the gathered detection form: boxes (S, F, K, 9) float32 lidar rows [x, y, z, dx, dy, dz, heading, score,
+ * label 1..3], counts (S, F), num_frames (S), poses (S, F, 4, 4) float64 lidar -> world.  K <= 512.
+ * params (23 doubles): overlap-filter thresholds [3], first-stage IoU [3], second-stage IoU [3], merge [3], score [3] (per class
+ * Vehicle, Pedestrian, Cyclist), P[2], Q[2], R, DELTA_T, LEAST_AGE, HEADER_LENGTH.
+ * Outputs per sequence s: trk (S, max_tracks, 6) int32 rows [track id, class, first frame, entry count, dynamic, entry offset] of the
+ * n_tracks[s] post-processed tracks in id order; ent_box (S, max_entries, 9) float64 world boxes, ent_score, ent_hit (0 / 1 / 2),
+ * ent_frame of each entry; kept (S, F, K) u8 the overlap filter's keep flags; overflow[s] != 0 when a capacity was exceeded (the
+ * sequence's outputs are then invalid).  One block per sequence, no host synchronisation. */
+size_t dz_track_sequences_ws_bytes(int S, int F, int K, int max_tracks, int max_entries);
+int dz_track_sequences(const float* boxes, const int* counts, const int* num_frames, const double* poses, int S, int F, int K,
+                       const double* params, int max_tracks, int max_entries, int* trk, int* n_tracks, double* ent_box,
+                       float* ent_score, int* ent_hit, int* ent_frame, unsigned char* kept, int* overflow, void* ws,
+                       size_t ws_bytes, dz_stream_t stream);
+
 /* ---- refiner inputs (SURVEY.md 8f row 2), csrc/refine_data.cu -------------------------------------------------------------- */
 /* Builds the eval inputs of the refiner modules for B tracks of up to L box slots straight from the collated frames, in one call per
  * kind: PRM (kind 0) = WaymoPositionDataset.extract_track_feature (refining/detzero_refine/datasets/waymo/waymo_position_dataset.py:31-184),
