@@ -72,6 +72,8 @@ _SIGS = {
     'dz_refine_inputs': (ci, [ci, vp, ci, vp, ci, ci, vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, ctypes.c_double, ci, ci,
                               ctypes.c_uint64, vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]),
     'dz_refine_revert': (ci, [ci, vp, vp, ci, vp, vp, vp, ci, ci, vp, vp, vp]),
+    'dz_combine_frames_ws_bytes': (sz, [ci, ci, ci]),
+    'dz_combine_frames': (ci, [vp, vp, vp, vp, vp, vp, vp, ci, ci, vp, vp, vp, ci, ci, ci, vp, vp, vp, vp, vp, sz, vp]),
     'dz_tta_expand': (ci, [vp, ci, vp, ci, vp, ci, vp, vp]),
     'dz_tta_unaugment': (ci, [vp, vp, ci, ci, vp, ci, vp, vp]),
     'dz_wbf_3d_ws_bytes': (sz, [ci, ci, ci, ci]),

@@ -6,6 +6,8 @@ revert_to_each_frame (refining/detzero_refine/datasets/waymo/), together with th
 daemon/prepare_object_data.py:241-327.  Each builder returns the dict the modules of detzero_b200.refine consume, with the
 reference's keys, shapes and float32 dtype.  Sampling is keyed on (seed, track_uid) and deterministic; see csrc/refine_data.cu for
 that function and the other deliberate deviations (float64 geometry, per-track GRM query count, the crop's coordinates).
+``combine_frames`` puts the refined tracks of a sequence together into per-frame result rows (csrc/combine.cu), replacing
+daemon/combine_output.py's convert_frame_format and combine_det.
 """
 import zlib
 
@@ -193,6 +195,66 @@ def revert_position_boxes(pred_boxes, poses, tracks):
 def revert_geometry_boxes(pred_boxes, poses, tracks):
     """WaymoGeometryDataset.revert_to_each_frame: the GRM size (B, 7) written into every world box -> (lidar, world) (B, L, 7)"""
     return _revert(GRM, pred_boxes, poses, tracks)
+
+
+def combine_frames(prm_lidar, grm_pred, scores, frame_of_box, box_num, cls, track_id, num_frames, drop=None, max_rows=1024):
+    """convert_frame_format + combine_det (daemon/combine_output.py) on the device (csrc/combine.cu): the refined tracks of one
+    sequence -> per-frame result rows.  Tables of the B tracks in output order (combine_final's: class by class, ids ascending):
+    prm_lidar (B, L, 7) f64 (revert_position_boxes' lidar boxes), grm_pred (B, 7) (the GRM prediction; only its size is used),
+    scores (B, L) f32 (the CRM pred_score, or the tracker's per-box score), frame_of_box (B, L) sequence frame indices 0..num_frames-1
+    (a caller whose frame_of_box is not one, e.g. after tracks_from_object_infos, passes the sequence frame index here), box_num (B),
+    cls (B) 1..3, track_id (B) in 0..2**31-1, unique.  drop: None, or the tracker's dropped detections of the sequence as
+    (det (>= num_frames, K, 9) f32 gathered rows, counts, kept (.., K) bool), e.g. (res.boxes[s], res.counts[s], res.kept[s]) of a
+    TrackResult.
+    Returns rows (F, R, 9) f32 [x, y, z, dx, dy, dz, heading, score, label], obj_id (F, R) int32 (-1: a dropped detection) and
+    count (F) int32, R = max_rows; rows past count[f] are zero with obj_id -1.  A frame's rows are its track boxes (PRM box with
+    the GRM size, by track then box order), then its dropped detections in input order with det_drop's heading wrap.  A frame
+    without a track box has no row at all.  Raises if a frame needs more than max_rows rows.
+    Deviations from combine_final: one call combines every class given (the reference writes one accumulating file per class), and a
+    frame with tracks but no detections has no dropped row (combine_det raises KeyError there)."""
+    dev = prm_lidar.device
+    B, L = int(prm_lidar.shape[0]), int(prm_lidar.shape[1])
+    F, R = int(num_frames), int(max_rows)
+    if F < 1 or R < 1:
+        raise ValueError('num_frames and max_rows must be positive')
+    i32 = dict(dtype=torch.int32, device=dev)
+    prm = prm_lidar.to(dtype=torch.float64).contiguous()
+    assert prm.shape == (B, L, 7), prm.shape
+    grm = torch.as_tensor(grm_pred).to(device=dev, dtype=torch.float32).reshape(B, 7).contiguous()
+    sc = torch.as_tensor(scores).to(device=dev, dtype=torch.float32).reshape(B, L).contiguous()
+    fob = torch.as_tensor(frame_of_box).to(**i32).reshape(B, L).contiguous()
+    bn = torch.as_tensor(box_num).to(**i32).reshape(B).contiguous()
+    cl = torch.as_tensor(cls).to(**i32).reshape(B).contiguous()
+    tid = torch.as_tensor(track_id).to(device=dev, dtype=torch.int64).reshape(B)
+    if B:
+        lo, hi = torch.stack([tid.min(), tid.max()]).tolist()
+        if lo < 0 or hi >= 1 << 31:
+            raise ValueError('track ids must lie in 0..2**31-1 (got %d..%d)' % (lo, hi))
+    tid = tid.to(torch.int32).contiguous()
+    det = cnt = kept = None
+    K = 0
+    if drop is not None:
+        det, cnt, kept = drop
+        assert det.dim() == 3 and det.shape[0] >= F and det.shape[2] == 9, det.shape
+        K = int(det.shape[1])
+        det = det[:F].to(device=dev, dtype=torch.float32).contiguous()
+        cnt = torch.as_tensor(cnt)[:F].to(**i32).contiguous()
+        kept = torch.as_tensor(kept)[:F].to(device=dev, dtype=torch.uint8).reshape(F, K).contiguous()
+    rows = torch.zeros((F, R, 9), dtype=torch.float32, device=dev)
+    obj_id = torch.full((F, R), -1, **i32)
+    count = torch.empty((F,), **i32)
+    overflow = torch.zeros((1,), **i32)
+    ws = ops.workspace(lib().dz_combine_frames_ws_bytes(B, L, F), dev, 'combine')
+    check(lib().dz_combine_frames(ops._p(prm), ops._p(grm), ops._p(sc), ops._p(fob), ops._p(bn), ops._p(cl), ops._p(tid), B, L,
+                                  ops._p(det), ops._p(cnt), ops._p(kept), K, F, R, ops._p(rows), ops._p(obj_id), ops._p(count),
+                                  ops._p(overflow), ops._p(ws), ws.numel(), ops._stream()), 'combine_frames')
+    ops._count(3)
+    ov = int(overflow.item())
+    if ov & 2:
+        raise ValueError('combine_frames: a frame_of_box entry lies outside 0..%d' % (F - 1))
+    if ov & 1:
+        raise RuntimeError('combine_frames: a frame needs more than max_rows=%d rows' % R)
+    return rows, obj_id, count
 
 
 def tracks_from_object_infos(obj_infos, L=200, track_uid=None, device='cuda'):

@@ -119,6 +119,23 @@ def crm_cfg():
     return AttrDict({'NAME': 'ConfidencePointnet', 'ENCODER_MLP': [128, 128], 'REGRESSION_MLP': [512], 'SCORE_THRESH': [0.35, 0.7]})
 
 
+def refine_models(seed, mode='fp32', classes=CLASS_NAMES, device='cuda'):
+    """{class: {'PRM', 'GRM', 'CRM': refine.RefineTemplate}} of the shipped REGRESSION configs with seeded weights (distinct per class
+    and kind), as offboard.refine_sequence takes them"""
+    from .refine import RefineTemplate
+    out = {}
+    for i, c in enumerate(classes):
+        out[c] = {}
+        for j, (kind, name, cfg, qd, md) in enumerate((('PRM', 'PositionRefineModel', prm_cfg(), 32, 32),
+                                                       ('GRM', 'GeometryRefineModel', grm_cfg(), 11, 4),
+                                                       ('CRM', 'ConfidenceRefineModel', crm_cfg(), 32, 32))):
+            cfg.COMPUTE_MODE = mode
+            m = RefineTemplate(AttrDict({'NAME': name, 'QUERY_POINT_DIMS': qd, 'MEMORY_POINT_DIMS': md, 'REGRESSION': cfg})).eval()
+            load_seeded(m, int(seed) * 16 + 3 * i + j)
+            out[c][kind] = m.to(device)
+    return out
+
+
 def prm_inputs(seed, B=2, boxes=200, qpts=256, mpts=48, dims=32):
     g = np.random.default_rng(seed)
     box_num = g.integers(20, boxes + 1, B)
@@ -152,13 +169,15 @@ def _rz(a):
 
 
 def synthetic_sequence(seed, frames=20, tracks=8, L=200, n_background=20000, max_pts=3000, origin=(5000.0, -3000.0, 50.0),
-                       min_len=1, enlarge=1.1, margin=1e-3, ego_step=1.0, max_speed=0.4, lengths=None, cls=None):
+                       min_len=1, enlarge=1.1, margin=1e-3, ego_step=1.0, max_speed=0.4, lengths=None, cls=None,
+                       radius=45.0):
     """A seeded tracked sequence: ego poses with world translations around ``origin`` (about 5 km) and yaw wrapping through +-pi,
     objects moving on smooth paths (headings wrapping too), 0..~max_pts points on and inside each box over a synth_waymo_cloud
     background, and no point within ``margin`` of any enlarged box face, so crop membership is unambiguous.
     Returns a dict: frames (N, 6) f32 collated rows [b=frame, x, y, z, tanh(i), elongation] in the lidar frame, frame_offsets (F+1),
     poses (F, 4, 4) f64, and the TrackBatch fields as numpy arrays (boxes (B, L, 7) f64 world, frame_of_box, scores, box_num, cls,
-    track_uid).  ``lengths`` / ``cls`` fix the box count / class of each track (default: random)."""
+    track_uid).  ``lengths`` / ``cls`` fix the box count / class of each track (default: random); each track starts 6 m to
+    ``radius`` m from the ego."""
     from .det.dataset import synth_waymo_cloud
     g = np.random.default_rng([int(seed), 0x5E9])
     F = int(frames)
@@ -185,7 +204,7 @@ def synthetic_sequence(seed, frames=20, tracks=8, L=200, n_background=20000, max
         start = int(g.integers(0, F - n + 1))
         box_num[b] = n
         dims = dims_by_cls[cls[b] - 1] * g.uniform(0.9, 1.1, 3)
-        r0, a0 = g.uniform(6, 45), g.uniform(-np.pi, np.pi)
+        r0, a0 = g.uniform(6, radius), g.uniform(-np.pi, np.pi)
         c0 = poses[start, :3, 3] + [r0 * np.cos(a0), r0 * np.sin(a0), -1.2]
         h0, speed, turn = g.uniform(-np.pi, np.pi), g.uniform(0, max_speed), g.uniform(-0.05, 0.05)
         pts_n = np.where(g.random(n) < 0.1, 0, np.exp(g.uniform(0, np.log(max_pts), n)).astype(int))
@@ -230,6 +249,39 @@ def synthetic_sequence(seed, frames=20, tracks=8, L=200, n_background=20000, max
     return {'frames': np.concatenate(rows, 0), 'frame_offsets': np.asarray(offsets, np.int64), 'poses': poses, 'boxes': boxes,
             'frame_of_box': fob, 'scores': scores, 'box_num': box_num, 'cls': cls,
             'track_uid': (np.arange(B, dtype=np.int64) * 7919 + int(seed) * 104729 + 1)}
+
+
+def detections_from_sequence(s, seed, miss=0.1, fp=10, K=500):
+    """Gathered lidar detections (F, K, 9) of a synthetic_sequence's ground-truth boxes, for the tracker: 3 cm / 0.01 rad / 0.5 %
+    jitter, about ``miss`` of the boxes missed (never the first or last two of a track), ``fp`` far false positives per frame, rows
+    shuffled.  Returns boxes, counts (F), gt (F, K) (the ground-truth track of each row, -1 for a false positive)."""
+    g = np.random.default_rng([int(seed), 0xC0B])
+    F = len(s['poses'])
+    dims = [[4.7, 2.0, 1.6], [0.9, 0.9, 1.8], [1.9, 0.8, 1.7]]
+    rows = [[] for _ in range(F)]
+    for b in range(len(s['box_num'])):
+        n = int(s['box_num'][b])
+        for j in range(n):
+            if 2 <= j < n - 2 and g.random() < miss:
+                continue
+            f = int(s['frame_of_box'][b, j])
+            P, w = s['poses'][f], s['boxes'][b, j]
+            loc = (w[:3] + g.normal(0, 0.03, 3) - P[:3, 3]) @ P[:3, :3]
+            h = w[6] + g.normal(0, 0.01) - np.arctan2(P[1, 0], P[0, 0])
+            rows[f].append(([*loc, *(w[3:6] * (1 + g.normal(0, 0.005, 3))), np.arctan2(np.sin(h), np.cos(h)),
+                             g.uniform(0.3, 0.95), s['cls'][b]], b))
+    for f in range(F):
+        for _ in range(fp):
+            a, r, c = g.uniform(-np.pi, np.pi), g.uniform(300, 500), int(g.integers(1, 4))
+            rows[f].append(([r * np.cos(a), r * np.sin(a), -1.0, *dims[c - 1], g.uniform(-np.pi, np.pi), g.uniform(0.02, 0.3), c], -1))
+    boxes, gt, counts = np.zeros((F, K, 9), np.float32), np.full((F, K), -1), np.zeros(F, np.int32)
+    for f in range(F):
+        if len(rows[f]) > K:
+            raise ValueError('frame %d has %d detections (K = %d)' % (f, len(rows[f]), K))
+        for i, k in enumerate(g.permutation(len(rows[f]))):
+            boxes[f, i], gt[f, i] = rows[f][k]
+        counts[f] = len(rows[f])
+    return boxes, counts, gt
 
 
 def synthetic_detections(seed, frames=199, objects=300, false_positives=40, K=500, miss=0.1, chain=0, origin=(5000.0, -3000.0, 50.0)):

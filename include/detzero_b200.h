@@ -291,6 +291,26 @@ int dz_refine_inputs(int kind, const float* points, int pt_stride, const int32_t
 int dz_refine_revert(int kind, const float* pred, const double* poses, int n_frames, const double* boxes, const int32_t* frame_of_box,
                      const int32_t* box_num, int B, int L, double* lidar, double* world, dz_stream_t stream);
 
+/* ---- combine: refined tracks -> per-frame result rows (csrc/combine.cu) ------------------------------------------------------- */
+/* convert_frame_format + combine_det as combine_final drives them (daemon/combine_output.py:27-41,44-99,102-167), for the B tracks
+ * of one sequence in output order: prm_lidar (B, L, 7) f64 (revert_position_boxes' lidar boxes), grm_pred (B, 7) f32 (only its size
+ * is read; the reference reads the same bits from the GRM's reverted boxes), score (B, L) f32 (CRM pred_score, or the tracker's
+ * per-box score), frame_of_box (B, L) (0..F-1), box_num (B) (0..L), cls (B) (label), track_id (B) (>= 0).  Optional (det NULL: none)
+ * the tracker's dropped detections: det (F, K, 9) f32 gathered rows, det_count (F), kept (F, K) u8 (TrackResult.kept).
+ * Outputs: rows (F, R, 9) f32 [x, y, z, dx, dy, dz, heading, score, label], obj_id (F, R) (-1 for a dropped detection), count (F);
+ * rows of a frame: its track boxes by track then box order, then its dropped rows in input order with det_drop's heading wrap.
+ * A frame without a track box gets no row (combine_det only extends frames convert_frame_format emitted).  Rows past count[f] are
+ * not written.  overflow (zeroed by the caller): bit 1 = a frame needed more than R rows (count clamped, nothing written past R),
+ * bit 2 = a frame index outside 0..F-1 (box skipped).  Deterministic (no atomic places a row), enqueue only.
+ * Deviations from combine_final: the reference writes one file per class and its class loop accumulates (each file holds every
+ * class processed so far; the last one omits sequences without a track of the last class); here one call combines the given tracks,
+ * every class at once.  combine_det raises KeyError for a frame with tracks but no drop entry; here that frame has no dropped row. */
+size_t dz_combine_frames_ws_bytes(int B, int L, int F);
+int dz_combine_frames(const double* prm_lidar, const float* grm_pred, const float* score, const int32_t* frame_of_box,
+                      const int32_t* box_num, const int32_t* cls, const int32_t* track_id, int B, int L, const float* det,
+                      const int32_t* det_count, const unsigned char* kept, int K, int F, int R, float* rows, int32_t* obj_id,
+                      int32_t* count, int32_t* overflow, void* ws, size_t ws_bytes, dz_stream_t stream);
+
 /* ---- test-time augmentation (CenterPoint TTA) ------------------------------------------------------------- */
 /* A view is 4 host floats [op, p1, p2, p3]: DZ_TTA_ORIGINAL; DZ_TTA_FLIP_X (y = -y); DZ_TTA_FLIP_Y (x = -x); DZ_TTA_FLIP_XY;
  * DZ_TTA_ROT with p1, p2 = cos, sin of the float32 angle (float32 torch on the CPU, as the reference computes them) and, for
