@@ -138,11 +138,18 @@ static int conv2d_f32_launch(const Conv2dParams& p, cudaStream_t st) {
 
 int dz_conv2d_fwd_tc(const Conv2dParams& p, int mode, cudaStream_t st);
 
+// the fp32 kernel reads the input as float4 (and the TMA unit needs a 16-byte aligned base), the tensor-core per-thread epilogue
+// writes float2: a view at an odd storage offset is refused rather than faulting on a misaligned vector access
+static bool vector_aligned(const float* in, const float* out) {
+    return (reinterpret_cast<uintptr_t>(in) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0;
+}
+
 extern "C" int dz_conv2d_fwd(const float* in, int B, int H, int W, int cin, int in_cstride, const float* weight, int KH,
                              int KW, int stride, int pad, const float* scale, const float* shift, int relu, float* out,
                              int Ho, int Wo, int cout, int out_coff, int out_cstride, int mode, dz_stream_t stream) {
     DZ_CHECK_ARG(in && weight && out && B >= 1 && cin % C2_BK == 0 && in_cstride % 4 == 0 && cout % 4 == 0);
     DZ_CHECK_ARG(Ho == (H + 2 * pad - KH) / stride + 1 && Wo == (W + 2 * pad - KW) / stride + 1);
+    DZ_CHECK_ARG(vector_aligned(in, out));
     Conv2dParams p{in, weight, scale, shift, out, B, H, W, cin, in_cstride, KH, KW, stride, pad, Ho, Wo, cout,
                    Ho, Wo, 1, 0, 0, out_coff, out_cstride, relu};
     if (mode == DZ_F32) return conv2d_f32_launch(p, (cudaStream_t)stream);
@@ -153,6 +160,7 @@ extern "C" int dz_deconv2d_fwd(const float* in, int B, int H, int W, int cin, co
                                const float* scale, const float* shift, int relu, float* out, int cout, int out_coff,
                                int out_cstride, int mode, dz_stream_t stream) {
     DZ_CHECK_ARG(in && weight && out && s >= 1 && cin % C2_BK == 0 && cout % 4 == 0);
+    DZ_CHECK_ARG(vector_aligned(in, out));
     if (mode != DZ_F32) {
         // tensor cores: one GEMM with N = s * s * cout over the input pixels (weights (dy, dx, cout, cin))
         Conv2dParams p{in, weight, scale, shift, out, B, H, W, cin, cin, 1, 1, 1, 0, H, W, cout, H * s, W * s, s, 0, 0,

@@ -182,7 +182,8 @@ int dz_sparse_to_bev_planes(const void* feats, const int32_t* coords, const int*
 /* NHWC conv2d (cross-correlation) with fused per-channel affine (folded BatchNorm2d / bias) and ReLU; output
  * written at channel offset into a tensor with out_cstride channels (fused torch.cat, backbone2d.py:107-108).
  * weight packed (KH, KW, cin, cout).  Replaces nn.Conv2d(+ZeroPad2d)+BatchNorm2d+ReLU stacks at
- * backbone2d.py:34-48 and center_head.py:25-31,81-88. */
+ * backbone2d.py:34-48 and center_head.py:25-31,81-88.  in must be 16-byte and out 8-byte aligned (DZ_ERR_ARG otherwise),
+ * here and in dz_deconv2d_fwd. */
 int dz_conv2d_fwd(const float* in, int B, int H, int W, int cin, int in_cstride, const float* weight, int KH, int KW,
                   int stride, int pad, const float* scale, const float* shift, int relu,
                   float* out, int Ho, int Wo, int cout, int out_coff, int out_cstride, int mode,

@@ -40,6 +40,13 @@ def trunc_tf32(t):
     return (t.float().contiguous().view(torch.int32) & ~0x1FFF).view(torch.float32)
 
 
+def trunc32(v64):
+    """float64 -> float32 rounded toward zero (a truncating fp32 add)"""
+    f = v64.float()
+    over = f.to(F64).abs() > v64.abs()
+    return torch.where(over, torch.nextafter(f, torch.zeros_like(f)), f)
+
+
 def split_bf16(t):
     """(p0, p1) = (RN_bf16(t), RN_bf16(t - p0)) as float32 (ops.to_planes, pack_spconv_weight)"""
     t = t.float()
@@ -125,10 +132,12 @@ def epilogue_exact(mode, y64, scale, shift, res, relu):
     return o
 
 
-def output_bits(mode, o32):
-    """what the kernel stores for the fp32 epilogue value o32: float32 (rows, cout) or bf16 planes (rows, P * cout)"""
+def output_bits(mode, o32, relu=True):
+    """what the kernel stores for the fp32 epilogue value o32: float32 (rows, cout) or bf16 planes (rows, P * cout).  The sparse
+    convs round every tf32 output; the dense tf32 convs round only a ReLU output (it feeds another TF32 conv), so relu=False
+    stores the fp32 value as it is"""
     if mode == 'tf32':
-        return rna_tf32(o32)
+        return rna_tf32(o32) if relu else o32
     if mode in PLANES:
         p0, p1 = split_bf16(o32)
         return (torch.cat([p0, p1], 1) if mode == 'bf16x2' else p0).to(torch.bfloat16)
@@ -228,8 +237,11 @@ def operand_coef(mode, x_tf32_exact=True):
     return 2.0 ** -8
 
 
-def output_coef(mode):
-    """relative error of the output rounding: RNA to TF32 (2^-11), two bf16 planes (2^-16), one (2^-8)"""
+def output_coef(mode, relu=True):
+    """relative error of the output rounding: RNA to TF32 (2^-11; none for a dense conv without ReLU, see output_bits), two bf16
+    planes (2^-16), one (2^-8)"""
+    if mode == 'tf32' and not relu:
+        return 0.0
     return {'fp32': 0.0, 'tf32x3': 0.0, 'tf32': 2.0 ** -11, 'bf16x2': 2.0 ** -16 * (1 + 2.0 ** -15), 'bf16': 2.0 ** -8}[mode]
 
 
@@ -239,11 +251,115 @@ def single_pass_coef(mode):
     return {'tf32x3': 2.0 ** -11 + 2.0 ** -11, 'bf16x2': 2.0 ** -8}[mode]
 
 
-def bound(mode, K, cin, A, scale, shift, res_abs, got_abs, x_tf32_exact=True):
+def bound(mode, K, cin, A, scale, shift, res_abs, got_abs, x_tf32_exact=True, relu=True):
     """element-wise bound on |stored output - float64 x . w epilogue|.
     y = sum x w errs by (operand + accumulation) A; the epilogue multiplies that by |scale| and adds <= 3 roundings
     (u each) of |y scale|, + |shift|, + |residual|; ReLU is 1-Lipschitz; the output rounding adds output_coef |got|."""
     c = operand_coef(mode, x_tf32_exact) + accumulation_coef(mode, K, cin)
     sa = A * scale.abs().to(F64)
     b = c * sa + 3 * U * ((1 + c) * sa + shift.abs().to(F64) + (0 if res_abs is None else res_abs))
-    return b + output_coef(mode) * got_abs
+    return b + output_coef(mode, relu) * got_abs
+
+
+# ---- dense conv2d / ConvTranspose2d (csrc/conv2d_tc.cu, csrc/bev.cu) ------------------------------------------------------------
+# The dense convs follow the contract above with K = KH KW taps and no residual: tf32 is sum T(x) RN(w) (RN = pack_conv_weight /
+# pack_deconv_weight) in 4 wgmma k-steps per 32-channel slice per tap, then __fmul_rn(., scale), __fadd_rn(., shift), fmaxf(., 0),
+# and cvt.rna.tf32 only when ReLU is on; fp32 is one FMA chain over KH KW cin, then * scale, + shift (possibly contracted into
+# one FMA: bound() allows three roundings) and ReLU, stored unrounded.  A ConvTranspose2d with kernel == stride has one tap per
+# output (K = 1).  Tensors are NHWC: x (B, H, W, cin), outputs (B, Ho, Wo, cout); weights in torch layout, (cout, cin, KH, KW) or,
+# transposed, (cin, cout, s, s).
+def exact_dense(g, mode, B, H, W, cin, cout, KH, KW, transposed=False):
+    """exact_operands in dense layout: x (B, H, W, cin), w (cout, cin, KH, KW) -- transposed: (cin, cout, KH, KW), KH = KW = s --,
+    scale, shift (cout); tap k = r KW + s carries the split weight values of offset k"""
+    x, w, scale, shift, _ = exact_operands(g, mode, B * H * W, cin, cout, KH * KW, 1)
+    w = w.view(KH, KW, cin, cout)
+    w = w.permute(2, 3, 0, 1) if transposed else w.permute(3, 2, 0, 1)
+    return x.view(B, H, W, cin), w.contiguous(), scale, shift
+
+
+def conv2d64(x, w, stride=1, pad=0, transposed=False):
+    """float64 NHWC conv2d (or ConvTranspose2d with kernel == stride) of x and w, on their device"""
+    x64, w64 = x.to(F64).permute(0, 3, 1, 2), w.to(F64)
+    if transposed:
+        y = torch.nn.functional.conv_transpose2d(x64, w64, stride=w.shape[2])
+    else:
+        y = torch.nn.functional.conv2d(x64, w64, stride=stride, padding=pad)
+    return y.permute(0, 2, 3, 1)
+
+
+def dense_contract64(mode, x, w, stride=1, pad=0, transposed=False):
+    """(float64 contract sum, A = the sum of the magnitudes of its products) of a dense conv in mode fp32 / tf32"""
+    y = A = None
+    for a, b in pieces(mode, x, w):
+        t = conv2d64(a, b, stride, pad, transposed)
+        s = conv2d64(a.abs(), b.abs(), stride, pad, transposed)
+        y, A = (t, s) if y is None else (y + t, A + s)
+    return y, A
+
+
+def _grid_bits(t, cdim):
+    """per channel c (dimension cdim of t): (f, bits) with every t[c] an integer multiple of 2^-f and max |t[c]| 2^f < 2^bits"""
+    t = t.to(F64).movedim(cdim, 0).reshape(t.shape[cdim], -1)
+    f = torch.full((t.shape[0],), 99, dtype=torch.int64, device=t.device)
+    for e in range(-30, 64):
+        s = t * 2.0 ** e
+        f[(s == s.round()).all(1) & (f == 99)] = e
+    assert bool((f < 99).all())
+    m = t.abs().amax(1) * torch.pow(2.0, f.to(F64))
+    return f, torch.ceil(torch.log2(m + 1)).to(torch.int64)
+
+
+def assert_exact_dense(mode, x, w, stride=1, pad=0, transposed=False):
+    """the exactness budget of exact_operands at a dense shape, re-derived from the operands themselves rather than from the generator's
+    argument: per input channel, the bits of the input piece plus the bits of the weight piece fit in 24 (every product is exact in
+    fp32), and the largest sum of product magnitudes of an output stays below 2^24 units of the finest product bit (every partial
+    sum in any order, rounded or truncated, is exact).  With the generator's values (channel 0: x in +-[1.25, 1.75] on 2^-10 (tf32)
+    / 2^-12 (fp32), w in +-[1.25, 1.5] on 2^-2 after RN_tf32 (tf32) / channel 1 on 2^-12 (fp32); every other value 0 or +-0.25) an
+    output sums at most K (1.76 * 1.5 + 0.25 * 1.51 + (cin - 2) / 16) < 9 * 35 = 315 at cin = 512, K = 9: below 2^9, on a grid of
+    2^-12 (tf32) / 2^-14 (fp32), so below 2^21 / 2^23 units.  Returns the largest A"""
+    wdim = 0 if transposed else 1
+    f, A = None, None
+    for a, b in pieces(mode, x, w):
+        fa, ba = _grid_bits(a, a.dim() - 1)
+        fb, bb = _grid_bits(b, wdim)
+        assert int((ba + bb).max()) <= 24, 'a contract product is not exact in fp32'
+        fab = int((fa + fb).max())
+        f = fab if f is None else max(f, fab)
+        s = conv2d64(a.abs(), b.abs(), stride, pad, transposed)
+        A = s if A is None else A + s
+    amax = float(A.max())
+    assert amax * 2.0 ** f < 2.0 ** 24, ('partial sums may round', amax, f)
+    return amax
+
+
+def tf32_exact(t):
+    """t is TF32-representable (the tensor core's truncating read of it is exact)"""
+    return torch.equal(t, trunc_tf32(t))
+
+
+def assert_conv2d(got, x, w, stride, pad, scale, shift, relu, mode, what, transposed=False):
+    """element-wise check of a dense conv output got (B, Ho, Wo, cout) against the float64 conv of its input x as stored and its fp32
+    weights w (torch layout), with bound(); x_tf32_exact is read off x itself.  One frame at a time on the device, so that the
+    float64 operands of a 188 x 188 x 512 map stay small.  Returns the largest err / bound"""
+    from tests.util import assert_within
+    cout = got.shape[3]
+    K = 1 if transposed else w.shape[2] * w.shape[3]
+    cin = w.shape[0] if transposed else w.shape[1]
+    dev = got.device
+    one = torch.ones(cout, dtype=torch.float32, device=dev)
+    scale = one if scale is None else scale.to(dev)
+    shift = torch.zeros_like(one) if shift is None else shift.to(dev)
+    exact = mode == 'tf32' and tf32_exact(x)
+    w = w.to(dev)
+    worst = 0.0
+    for b in range(x.shape[0]):
+        xb = x[b:b + 1].to(dev)
+        y = conv2d64(xb, w, stride, pad, transposed)
+        A = conv2d64(xb.abs(), w.abs(), stride, pad, transposed)
+        ref = y * scale.to(F64) + shift.to(F64)
+        if relu:
+            ref = ref.clamp_min(0)
+        gb = got[b:b + 1]
+        bnd = bound(mode, K, cin, A, scale, shift, None, gb.to(F64).abs(), x_tf32_exact=exact, relu=relu)
+        worst = max(worst, assert_within(gb, ref, bnd, '%s frame %d' % (what, b)))
+    return worst

@@ -4,7 +4,7 @@ per-thread stores."""
 import pytest
 import torch
 
-from tests import util
+from tests import spconv_arith as sa
 from detzero_b200 import _lib
 
 pytestmark = pytest.mark.gpu
@@ -17,11 +17,11 @@ def test_deconv2d_tf32_one_gemm(cuda, B, cin, cout, H, W, coff, ctot):
     x = torch.randn(B, cin, H, W, generator=g)
     w = torch.randn(cin, cout, 2, 2, generator=g) * 0.05
     scale, shift = torch.rand(cout, generator=g) + 0.5, torch.randn(cout, generator=g) * 0.1
-    ref = torch.relu(torch.nn.functional.conv_transpose2d(x, w, None, stride=2) * scale.view(1, -1, 1, 1) + shift.view(1, -1, 1, 1))
     out = torch.full((B, 2 * H, 2 * W, ctot), -3.0, device=cuda)
     n0 = ops.launch_count()
-    ops.deconv2d(x.permute(0, 2, 3, 1).contiguous().to(cuda), ops.pack_deconv_weight(w, _lib.DZ_TF32).to(cuda), (2, cin, cout), scale.to(cuda),
+    xh = x.permute(0, 2, 3, 1).contiguous().to(cuda)
+    ops.deconv2d(xh, ops.pack_deconv_weight(w, _lib.DZ_TF32).to(cuda), (2, cin, cout), scale.to(cuda),
                  shift.to(cuda), True, out=out, out_coff=coff, mode=_lib.DZ_TF32)
     assert ops.launch_count() - n0 == 1
-    assert util.rel_err(out[..., coff:coff + cout].permute(0, 3, 1, 2).cpu(), ref) < 2e-3
+    sa.assert_conv2d(out[..., coff:coff + cout], xh, w, 1, 0, scale, shift, True, 'tf32', 'deconv', transposed=True)
     assert torch.all(out[..., :coff] == -3.0) and torch.all(out[..., coff + cout:] == -3.0)

@@ -1,16 +1,19 @@
-"""The N=256 halo conv2d kernel (3x3 stride-1, output channels on the wgmma M side, 256-pixel patches on N) against torch fp32:
+"""The N=256 halo conv2d kernel (3x3 stride-1, output channels on the wgmma M side, 256-pixel patches on N) element by element
+against float64 (spconv_arith.assert_conv2d):
 every channel-tile width it takes, ragged image edges and channel tiles, output at a channel offset of a wider tensor, and frame
 independence of a batch."""
 import pytest
 import torch
-from torch.profiler import ProfilerActivity, profile
 
+from tests import spconv_arith as sa
 from tests import util
 from detzero_b200 import _lib, ops
 
 pytestmark = pytest.mark.gpu
 
-KERNEL = 'k_conv2d_tf32_halo_n256'
+
+def _nhwc(cuda, x):
+    return x.permute(0, 2, 3, 1).contiguous().to(cuda)
 
 
 def _inputs(seed, B, cin, cout, H, W):
@@ -22,7 +25,7 @@ def _inputs(seed, B, cin, cout, H, W):
 
 
 def _conv(cuda, x, w, scale, shift, cin, cout, out=None, coff=0):
-    return ops.conv2d(x.permute(0, 2, 3, 1).contiguous().to(cuda), ops.pack_conv_weight(w, _lib.DZ_TF32).to(cuda), (3, 3, cin, cout), 1, 1,
+    return ops.conv2d(_nhwc(cuda, x), ops.pack_conv_weight(w, _lib.DZ_TF32).to(cuda), (3, 3, cin, cout), 1, 1,
                       scale.to(cuda), shift.to(cuda), True, out=out, out_coff=coff, mode=_lib.DZ_TF32)
 
 
@@ -33,14 +36,10 @@ def _conv(cuda, x, w, scale, shift, cin, cout, out=None, coff=0):
                                                           (64, 384, 95, 93, 4, 32, 448)])
 def test_conv2d_halo_n256(cuda, cin, cout, H, W, B, coff, cstride):
     x, w, scale, shift = _inputs(17, B, cin, cout, H, W)
-    ref = torch.relu(torch.nn.functional.conv2d(x, w, None, 1, 1) * scale.view(1, -1, 1, 1) + shift.view(1, -1, 1, 1))
     out = torch.full((B, H, W, cstride), -3.0, device=cuda)
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        _conv(cuda, x, w, scale, shift, cin, cout, out=out, coff=coff)
-        torch.cuda.synchronize()
-    assert any(KERNEL in e.key for e in prof.key_averages()), 'the shape did not select the N=256 halo kernel'
-    got = out[..., coff:coff + cout].permute(0, 3, 1, 2).cpu()
-    assert util.rel_err(got, ref) < 2e-3
+    _, seen = util.conv2d_kernels(lambda: _conv(cuda, x, w, scale, shift, cin, cout, out=out, coff=coff))
+    assert seen == {'k_conv2d_tf32_halo_n256<%d>' % (128 if cout > 64 else 64)}, ('the shape did not select the N=256 halo kernel', seen)
+    sa.assert_conv2d(out[..., coff:coff + cout], _nhwc(cuda, x), w, 1, 1, scale, shift, True, 'tf32', 'halo n256')
     assert torch.all(out[..., :coff] == -3.0) and torch.all(out[..., coff + cout:] == -3.0)
 
 

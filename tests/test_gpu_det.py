@@ -6,6 +6,7 @@ import torch
 
 import oracle
 from oracle import det_ref, spconv_ref, weights
+from tests import spconv_arith as sa
 from tests import util
 from detzero_b200 import _lib
 
@@ -332,13 +333,14 @@ def test_conv2d_fp32(cuda, cin, cout, k, stride, pad, H, W):
     x = torch.randn(2, cin, H, W, generator=g)
     w = torch.randn(cout, cin, k, k, generator=g) * 0.05
     scale, shift = torch.rand(cout, generator=g) + 0.5, torch.randn(cout, generator=g) * 0.1
-    ref = torch.relu(torch.nn.functional.conv2d(x, w, None, stride, pad) * scale.view(1, -1, 1, 1) + shift.view(1, -1, 1, 1))
-    for mode, tol in ((_lib.DZ_F32, 1e-5), (_lib.DZ_TF32, 2e-3)):
-        if mode == _lib.DZ_TF32 and cin % 32:
+    xh = x.permute(0, 2, 3, 1).contiguous().to(cuda)
+    for mode in ('fp32', 'tf32'):
+        if mode == 'tf32' and cin % 32:
             continue
-        out = ops.conv2d(x.permute(0, 2, 3, 1).contiguous().to(cuda), ops.pack_conv_weight(w, mode).to(cuda), (k, k, cin, cout),
-                         stride, pad, scale.to(cuda), shift.to(cuda), True, mode=mode)
-        assert util.rel_err(out.permute(0, 3, 1, 2).cpu(), ref) < tol, mode
+        m = _lib.MODES[mode]
+        out = ops.conv2d(xh, ops.pack_conv_weight(w, m).to(cuda), (k, k, cin, cout), stride, pad, scale.to(cuda), shift.to(cuda), True,
+                         mode=m)
+        sa.assert_conv2d(out, xh, w, stride, pad, scale, shift, True, mode, mode)
 
 
 @pytest.mark.parametrize('cin,cout,H,W,coff,cstride', [(128, 128, 136, 184, 0, 128), (64, 64, 152, 168, 32, 160), (256, 256, 94, 94, 0, 256)])
@@ -351,12 +353,11 @@ def test_conv2d_tf32_many_tiles(cuda, cin, cout, H, W, coff, cstride):
     x = torch.randn(1, cin, H, W, generator=g)
     w = torch.randn(cout, cin, 3, 3, generator=g) * 0.05
     scale, shift = torch.rand(cout, generator=g) + 0.5, torch.randn(cout, generator=g) * 0.1
-    ref = torch.relu(torch.nn.functional.conv2d(x, w, None, 1, 1) * scale.view(1, -1, 1, 1) + shift.view(1, -1, 1, 1))
+    xh = x.permute(0, 2, 3, 1).contiguous().to(cuda)
     out = torch.full((1, H, W, cstride), -3.0, device=cuda)
-    ops.conv2d(x.permute(0, 2, 3, 1).contiguous().to(cuda), ops.pack_conv_weight(w, _lib.DZ_TF32).to(cuda), (3, 3, cin, cout), 1, 1,
+    ops.conv2d(xh, ops.pack_conv_weight(w, _lib.DZ_TF32).to(cuda), (3, 3, cin, cout), 1, 1,
                scale.to(cuda), shift.to(cuda), True, out=out, out_coff=coff, mode=_lib.DZ_TF32)
-    got = out[..., coff:coff + cout].permute(0, 3, 1, 2).cpu()
-    assert util.rel_err(got, ref) < 2e-3
+    sa.assert_conv2d(out[..., coff:coff + cout], xh, w, 1, 1, scale, shift, True, 'tf32', 'many tiles')
     assert torch.all(out[..., :coff] == -3.0) and torch.all(out[..., coff + cout:] == -3.0)
 
 
@@ -366,12 +367,12 @@ def test_deconv2d_fp32_concat(cuda, s):
     g = torch.Generator().manual_seed(4)
     x = torch.randn(2, 64, 7, 9, generator=g)
     w = torch.randn(64, 32, s, s, generator=g) * 0.1
-    ref = torch.nn.functional.conv_transpose2d(x, w, None, stride=s)
-    for mode, tol in ((_lib.DZ_F32, 1e-5), (_lib.DZ_TF32, 2e-3)):
+    xh = x.permute(0, 2, 3, 1).contiguous().to(cuda)
+    for mode in ('fp32', 'tf32'):
         out = torch.zeros(2, 7 * s, 9 * s, 48, device=cuda)
-        ops.deconv2d(x.permute(0, 2, 3, 1).contiguous().to(cuda), ops.pack_deconv_weight(w, mode).to(cuda), (s, 64, 32), None, None,
-                     False, out=out, out_coff=16, mode=mode)
-        assert util.rel_err(out[..., 16:].permute(0, 3, 1, 2).cpu(), ref) < tol, mode
+        ops.deconv2d(xh, ops.pack_deconv_weight(w, _lib.MODES[mode]).to(cuda), (s, 64, 32), None, None,
+                     False, out=out, out_coff=16, mode=_lib.MODES[mode])
+        sa.assert_conv2d(out[..., 16:], xh, w, 1, 0, None, None, False, mode, mode, transposed=True)
         assert out[..., :16].abs().max().item() == 0
 
 
@@ -385,11 +386,11 @@ def test_deconv2d_tf32_strided_tma_store(cuda, B, cin, cout, H, W, coff, ctot):
     x = torch.randn(B, cin, H, W, generator=g)
     w = torch.randn(cin, cout, 2, 2, generator=g) * 0.05
     scale, shift = torch.rand(cout, generator=g) + 0.5, torch.randn(cout, generator=g) * 0.1
-    ref = torch.relu(torch.nn.functional.conv_transpose2d(x, w, None, stride=2) * scale.view(1, -1, 1, 1) + shift.view(1, -1, 1, 1))
+    xh = x.permute(0, 2, 3, 1).contiguous().to(cuda)
     out = torch.full((B, 2 * H, 2 * W, ctot), -3.0, device=cuda)
-    ops.deconv2d(x.permute(0, 2, 3, 1).contiguous().to(cuda), ops.pack_deconv_weight(w, _lib.DZ_TF32).to(cuda), (2, cin, cout), scale.to(cuda),
+    ops.deconv2d(xh, ops.pack_deconv_weight(w, _lib.DZ_TF32).to(cuda), (2, cin, cout), scale.to(cuda),
                  shift.to(cuda), True, out=out, out_coff=coff, mode=_lib.DZ_TF32)
-    assert util.rel_err(out[..., coff:coff + cout].permute(0, 3, 1, 2).cpu(), ref) < 2e-3
+    sa.assert_conv2d(out[..., coff:coff + cout], xh, w, 1, 0, scale, shift, True, 'tf32', 'strided store', transposed=True)
     assert torch.all(out[..., :coff] == -3.0) and torch.all(out[..., coff + cout:] == -3.0)
 
 
@@ -673,7 +674,7 @@ def test_batched_frames_equal_single_frames(cuda):
                                                                       # (fused head stage 2), 3 x 128 (fused head stage 1), ragged image edges
                                                                       (512, 64, 3, 1, 1, 188, 188, 2, 0, 64), (384, 12, 3, 1, 1, 100, 90, 4, 0, 12),
                                                                       (64, 384, 3, 1, 1, 95, 93, 4, 0, 384), (128, 128, 3, 1, 1, 61, 67, 8, 128, 384)])
-def test_conv2d_tf32_cta_pair_kernel(cuda, cin, cout, k, stride, pad, H, W, B, coff, cstride):
+def test_conv2d_tf32_halo_and_generic_kernels(cuda, cin, cout, k, stride, pad, H, W, B, coff, cstride):
     """the BEV-backbone and head shapes at batch sizes that give several tiles per SM: Cout = 256 (two 128-wide weight tiles per
     patch), odd tile counts, ragged edges, stride 2, 1x1, channel-offset (concat) output; the 3x3 stride-1 shapes run through the
     HALO variant (one (16+2) x (8+2) activation tile per 32-channel slice, nine shifted wgmma descriptors) at every tile width"""
@@ -682,11 +683,10 @@ def test_conv2d_tf32_cta_pair_kernel(cuda, cin, cout, k, stride, pad, H, W, B, c
     x = torch.randn(B, cin, H, W, generator=g)
     w = torch.randn(cout, cin, k, k, generator=g) * 0.05
     scale, shift = torch.rand(cout, generator=g) + 0.5, torch.randn(cout, generator=g) * 0.1
-    ref = torch.relu(torch.nn.functional.conv2d(x, w, None, stride, pad) * scale.view(1, -1, 1, 1) + shift.view(1, -1, 1, 1))
-    Ho, Wo = ref.shape[2], ref.shape[3]
+    Ho, Wo = (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1
+    xh = x.permute(0, 2, 3, 1).contiguous().to(cuda)
     out = torch.full((B, Ho, Wo, cstride), -3.0, device=cuda)
-    ops.conv2d(x.permute(0, 2, 3, 1).contiguous().to(cuda), ops.pack_conv_weight(w, _lib.DZ_TF32).to(cuda), (k, k, cin, cout), stride, pad,
+    ops.conv2d(xh, ops.pack_conv_weight(w, _lib.DZ_TF32).to(cuda), (k, k, cin, cout), stride, pad,
                scale.to(cuda), shift.to(cuda), True, out=out, out_coff=coff, mode=_lib.DZ_TF32)
-    got = out[..., coff:coff + cout].permute(0, 3, 1, 2).cpu()
-    assert util.rel_err(got, ref) < 2e-3
+    sa.assert_conv2d(out[..., coff:coff + cout], xh, w, stride, pad, scale, shift, True, 'tf32', 'conv2d')
     assert torch.all(out[..., :coff] == -3.0) and torch.all(out[..., coff + cout:] == -3.0)

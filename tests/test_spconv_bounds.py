@@ -33,13 +33,6 @@ def _products(mode, nbr, x, w, x_is_planes=False):
     return torch.cat(cols, 2)
 
 
-def _trunc32(v64):
-    """float64 -> float32 rounded toward zero"""
-    f = v64.float()
-    over = f.to(F64).abs() > v64.abs()
-    return torch.where(over, torch.nextafter(f, torch.zeros_like(f)), f)
-
-
 def _sum32(p, order, trunc=False):
     if order == 'pairwise':
         t = p.float()
@@ -52,7 +45,7 @@ def _sum32(p, order, trunc=False):
     acc = torch.zeros(p.shape[:-1], dtype=torch.float32)
     for i in idx:
         s = acc.to(F64) + p[..., i]
-        acc = _trunc32(s) if trunc else s.float()
+        acc = sa.trunc32(s) if trunc else s.float()
     return acc
 
 
@@ -119,7 +112,7 @@ def _emulate(mode, nbr, x, w, scale, shift, res, relu, x_is_planes=False, drop_p
             steps = steps[:-1]
         for s in steps:
             for ga, wb in gathered:
-                acc = _trunc32(acc.to(F64) + ga[:, s:s + ch] @ wb[s:s + ch])
+                acc = sa.trunc32(acc.to(F64) + ga[:, s:s + ch] @ wb[s:s + ch])
     if mode in sa.PLANES:
         o = (acc.to(F64) * scale.to(F64) + shift.to(F64)).float()                # fma
     else:

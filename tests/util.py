@@ -1,4 +1,6 @@
 """shared builders for the parity tests"""
+import re
+
 import numpy as np
 import torch
 
@@ -76,3 +78,30 @@ def assert_equal_signed(got, ref, what):
     if not bool(same.all()):
         i = np.unravel_index(int((~same).to(torch.uint8).argmax()), tuple(got.shape))
         raise AssertionError('%s: first difference at %s (got %r, torch %r)' % (what, i, got[i].item(), ref[i].item()))
+
+
+def _conv2d_kernel_names(prof):
+    seen = set()
+    for e in prof.key_averages():
+        m = re.search(r'(k_conv2d_tf32_halo_n256|k_conv2d_tf32|k_conv2d_f32)<([^>]*)>', e.key)
+        if m:
+            args = [re.sub(r'\((?:int|bool)\)', '', a).strip() for a in m.group(2).split(',')]
+            if m.group(1) == 'k_conv2d_tf32':
+                args[1] = {'0': 'false', '1': 'true'}.get(args[1], args[1])
+            seen.add('%s<%s>' % (m.group(1), ', '.join(args)))
+    return seen
+
+
+def conv2d_kernels(run, tries=3):
+    """(run(), the dense conv2d kernels it launched as 'name<args>' with the demangler's (int) / (bool) casts removed), from
+    torch.profiler.  A profiler session now and then records none of its kernels; run (idempotent) is then profiled again, so a
+    lost record is not taken for a wrong kernel, while a wrong kernel still shows as one"""
+    from torch.profiler import ProfilerActivity, profile
+    for _ in range(tries):
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            out = run()
+            torch.cuda.synchronize()
+        seen = _conv2d_kernel_names(prof)
+        if seen:
+            break
+    return out, seen
