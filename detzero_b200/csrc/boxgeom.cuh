@@ -82,6 +82,14 @@ static __device__ float bev_overlap(const float* a, const float* b) {
     return fabsf(area) / 2.f;
 }
 
+// centre distance beyond the sum of half-diagonals plus 0.05 m: the BEV overlap of the two boxes is exactly 0 (no corner lies
+// within the 1e-2 in-box margin, no edges cross); the tracker and the ground-truth scoring skip such pairs before bev_overlap
+__device__ __forceinline__ bool far_pair(const float* a, const float* b) {
+    const float dx = a[0] - b[0], dy = a[1] - b[1];
+    const float r = 0.5f * (sqrtf(a[3] * a[3] + a[4] * a[4]) + sqrtf(b[3] * b[3] + b[4] * b[4])) + 0.05f;
+    return dx * dx + dy * dy > r * r;
+}
+
 __device__ __forceinline__ float bev_iou(const float* a, const float* b) {
     float sa = a[3] * a[4], sb = b[3] * b[4];
     float so = bev_overlap(a, b);

@@ -16,7 +16,7 @@
 // through bev_iou of boxgeom.cuh.  The reference's cost (1 - affinity, 5000 where cost >= 1, scipy linear_sum_assignment) makes
 // the optimum a maximum-cardinality matching of the valid edges with the least total cost; that objective separates over the
 // connected components of the valid-edge graph.  The components are labelled by min-hooking union-find; each one is solved
-// exactly (Hungarian with potentials, float64 costs (double)(1.f - iou)).  A component of at most SMALL_EDGES edges (nearly all:
+// exactly (Hungarian with potentials of assign.cuh, float64 costs (double)(1.f - iou)).  A component of at most SMALL_EDGES edges (nearly all:
 // one detection and its track) is solved by one thread on its edges sorted by (row, column); a larger one (a chain of pedestrians,
 // a crowd) by the whole block, one component at a time, with the same arithmetic and tie rule.  The dense cost matrix of a
 // component lives in the per-sequence assignment scratch (SCR_CAP doubles, e.g. a 700 x 700 component).
@@ -38,6 +38,7 @@
 #include <limits.h>
 #include "common.cuh"
 #include "boxgeom.cuh"
+#include "assign.cuh"
 
 namespace {
 
@@ -45,7 +46,6 @@ constexpr int NT = 512, NW = NT / 32;
 constexpr int EDGE_CAP = 32768;            // association edges per call
 constexpr int MEDGE_CAP = 32768;           // merge edges per call
 constexpr int SCR_CAP = 1 << 19;           // float64 assignment scratch per sequence
-constexpr float FAR_SLACK = 0.05f;
 constexpr int SMALL_EDGES = 32;            // components with more edges are solved by the whole block
 
 struct Seq {
@@ -72,8 +72,8 @@ struct Seq {
 struct Shared {
     int n_live, n_rlive, next_id, n_edges, n_medges, changed, overflow, f_used, r_used, scr_used, n_rows, n_cols, n_tmp, n_births;
     int warp[NW + 1];
-    double wval[NW], hdelta;                // block-wide Hungarian: per-warp minima, the step's delta and column
-    int widx[NW], hj1, n_big;
+    int n_big;
+    HungShared<NT> hs;                      // block-wide Hungarian
 };
 
 __device__ __forceinline__ float yawf(float y) {                      // transform_utils.yaw_filter, ndarray branch, float32
@@ -90,13 +90,6 @@ __device__ __forceinline__ double yawd(double y) {
     if (y > pi) y -= pi2;
     if (y <= -pi) y += pi2;
     return y;
-}
-
-// centre distance beyond the sum of half-diagonals (+ slack): the BEV overlap of the two boxes is exactly 0
-__device__ __forceinline__ bool far_pair(const float* a, const float* b) {
-    const float dx = a[0] - b[0], dy = a[1] - b[1];
-    const float r = 0.5f * (sqrtf(a[3] * a[3] + a[4] * a[4]) + sqrtf(b[3] * b[3] + b[4] * b[4])) + FAR_SLACK;
-    return dx * dx + dy * dy > r * r;
 }
 
 // ordered block-wide compaction: out positions of the items i < n with pred(i) true, in index order; returns the count
@@ -118,100 +111,6 @@ __device__ int block_compact(int n, Pred pred, Emit emit, Shared& sh) {
         __syncthreads();
     }
     return total;
-}
-
-__device__ __forceinline__ int uf_find(volatile int* lab, int x) {
-    int p = lab[x];
-    while (p != x) { x = p; p = lab[x]; }
-    return x;
-}
-
-// exact rectangular assignment (Hungarian with potentials, rows <= cols), a row-major n x m; p[j] = row (1-based) of column j
-__device__ void hungarian(const double* a, int n, int m, double* u, double* v, double* minv, int* p, int* way, unsigned char* used) {
-    for (int j = 0; j <= m; ++j) { v[j] = 0.; p[j] = 0; way[j] = 0; }
-    for (int i = 0; i <= n; ++i) u[i] = 0.;
-    for (int i = 1; i <= n; ++i) {
-        p[0] = i;
-        int j0 = 0;
-        for (int j = 0; j <= m; ++j) { minv[j] = DBL_MAX; used[j] = 0; }
-        do {
-            used[j0] = 1;
-            const int i0 = p[j0];
-            double delta = DBL_MAX;
-            int j1 = 0;
-            for (int j = 1; j <= m; ++j)
-                if (!used[j]) {
-                    const double cur = a[(size_t)(i0 - 1) * m + (j - 1)] - u[i0] - v[j];
-                    if (cur < minv[j]) { minv[j] = cur; way[j] = j0; }
-                    if (minv[j] < delta) { delta = minv[j]; j1 = j; }
-                }
-            for (int j = 0; j <= m; ++j)
-                if (used[j]) { u[p[j]] += delta; v[j] -= delta; } else minv[j] -= delta;
-            j0 = j1;
-        } while (p[j0] != 0);
-        do { const int j1 = way[j0]; p[j0] = p[j1]; j0 = j1; } while (j0);
-    }
-}
-
-// (value, index) minimum over the block, the smaller index on a tie -> sh.hdelta, sh.hj1 (the first minimum of an ascending scan)
-__device__ void block_argmin(double val, int idx, Shared& sh) {
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-#pragma unroll
-    for (int off = 16; off; off >>= 1) {
-        const double ov = __shfl_down_sync(0xffffffffu, val, off);
-        const int oi = __shfl_down_sync(0xffffffffu, idx, off);
-        if (ov < val || (ov == val && oi < idx)) { val = ov; idx = oi; }
-    }
-    if (lane == 0) { sh.wval[w] = val; sh.widx[w] = idx; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double bv = sh.wval[0];
-        int bi = sh.widx[0];
-        for (int k = 1; k < NW; ++k)
-            if (sh.wval[k] < bv || (sh.wval[k] == bv && sh.widx[k] < bi)) { bv = sh.wval[k]; bi = sh.widx[k]; }
-        sh.hdelta = bv; sh.hj1 = bi;
-    }
-    __syncthreads();
-}
-
-// hungarian() with every column loop spread over the block: the same arithmetic on every element and the same (first) minimum,
-// so the result is that of the one-thread solver.  Each augmentation step costs two block reductions.
-__device__ void hungarian_block(const double* a, int n, int m, double* u, double* v, double* minv, int* p, int* way,
-                                unsigned char* used, Shared& sh) {
-    for (int j = threadIdx.x; j <= m; j += NT) { v[j] = 0.; p[j] = 0; way[j] = 0; }
-    for (int i = threadIdx.x; i <= n; i += NT) u[i] = 0.;
-    __syncthreads();
-    for (int i = 1; i <= n; ++i) {
-        for (int j = threadIdx.x; j <= m; j += NT) { minv[j] = DBL_MAX; used[j] = 0; }
-        if (threadIdx.x == 0) p[0] = i;
-        __syncthreads();
-        int j0 = 0;
-        while (true) {
-            if (threadIdx.x == 0) used[j0] = 1;
-            __syncthreads();
-            const int i0 = p[j0];
-            const double ui0 = u[i0];
-            double best = DBL_MAX;
-            int bj = INT_MAX;
-            for (int j = 1 + threadIdx.x; j <= m; j += NT)
-                if (!used[j]) {
-                    const double cur = a[(size_t)(i0 - 1) * m + (j - 1)] - ui0 - v[j];
-                    if (cur < minv[j]) { minv[j] = cur; way[j] = j0; }
-                    if (minv[j] < best) { best = minv[j]; bj = j; }
-                }
-            block_argmin(best, bj, sh);
-            const double delta = sh.hdelta;
-            const int j1 = sh.hj1;
-            for (int j = threadIdx.x; j <= m; j += NT)
-                if (used[j]) { u[p[j]] += delta; v[j] -= delta; } else minv[j] -= delta;
-            __syncthreads();
-            j0 = j1;
-            if (p[j0] == 0) break;
-        }
-        if (threadIdx.x == 0)
-            do { const int j1 = way[j0]; p[j0] = p[j1]; j0 = j1; } while (j0);
-        __syncthreads();
-    }
 }
 
 struct Frame {                      // one frame's detections in shared memory
@@ -434,7 +333,7 @@ __device__ void associate(Frame& fr, Seq& sq, Shared& sh, int n_rows, int n_cols
         int* p = (int*)(minv + hm + 1);
         int* way = p + hm + 1;
         unsigned char* used = (unsigned char*)(way + hm + 1);
-        hungarian_block(A, hn, hm, u, v, minv, p, way, used, sh);
+        hungarian_block<NT>(A, hn, hm, u, v, minv, p, way, used, sh.hs);
         for (int j = 1 + threadIdx.x; j <= hm; j += NT) {
             if (!p[j]) continue;
             const int hi = p[j] - 1, hj = j - 1;

@@ -175,8 +175,8 @@ def synthetic_sequence(seed, frames=20, tracks=8, L=200, n_background=20000, max
     objects moving on smooth paths (headings wrapping too), 0..~max_pts points on and inside each box over a synth_waymo_cloud
     background, and no point within ``margin`` of any enlarged box face, so crop membership is unambiguous.
     Returns a dict: frames (N, 6) f32 collated rows [b=frame, x, y, z, tanh(i), elongation] in the lidar frame, frame_offsets (F+1),
-    poses (F, 4, 4) f64, and the TrackBatch fields as numpy arrays (boxes (B, L, 7) f64 world, frame_of_box, scores, box_num, cls,
-    track_uid).  ``lengths`` / ``cls`` fix the box count / class of each track (default: random); each track starts 6 m to
+    poses (F, 4, 4) f64, the TrackBatch fields as numpy arrays (boxes (B, L, 7) f64 world, frame_of_box, scores, box_num, cls,
+    track_uid) and points_per_box (B, L), the object points put in each box.  ``lengths`` / ``cls`` fix the box count / class of each track (default: random); each track starts 6 m to
     ``radius`` m from the ego."""
     from .det.dataset import synth_waymo_cloud
     g = np.random.default_rng([int(seed), 0x5E9])
@@ -194,6 +194,7 @@ def synthetic_sequence(seed, frames=20, tracks=8, L=200, n_background=20000, max
     boxes = np.zeros((B, L, 7))
     fob = np.zeros((B, L), np.int32)
     scores = np.zeros((B, L), np.float32)
+    npts = np.zeros((B, L), np.int32)
     box_num = np.zeros(B, np.int32)
     cls = (g.integers(1, 4, B) if cls is None else np.asarray(cls)).astype(np.int32)
     dims_by_cls = np.array([[4.7, 2.0, 1.6], [0.9, 0.9, 1.8], [1.9, 0.8, 1.7]])
@@ -208,6 +209,7 @@ def synthetic_sequence(seed, frames=20, tracks=8, L=200, n_background=20000, max
         c0 = poses[start, :3, 3] + [r0 * np.cos(a0), r0 * np.sin(a0), -1.2]
         h0, speed, turn = g.uniform(-np.pi, np.pi), g.uniform(0, max_speed), g.uniform(-0.05, 0.05)
         pts_n = np.where(g.random(n) < 0.1, 0, np.exp(g.uniform(0, np.log(max_pts), n)).astype(int))
+        npts[b, :n] = pts_n
         for j in range(n):
             f = start + j
             h = h0 + turn * j
@@ -247,8 +249,43 @@ def synthetic_sequence(seed, frames=20, tracks=8, L=200, n_background=20000, max
         rows.append(r)
         offsets.append(offsets[-1] + len(r))
     return {'frames': np.concatenate(rows, 0), 'frame_offsets': np.asarray(offsets, np.int64), 'poses': poses, 'boxes': boxes,
-            'frame_of_box': fob, 'scores': scores, 'box_num': box_num, 'cls': cls,
+            'frame_of_box': fob, 'scores': scores, 'box_num': box_num, 'cls': cls, 'points_per_box': npts,
             'track_uid': (np.arange(B, dtype=np.int64) * 7919 + int(seed) * 104729 + 1)}
+
+
+def synthetic_ground_truth(s, seed, name='seq', difficulty=None):
+    """The ground truth of a synthetic_sequence ``s`` as the frame dicts of waymo_infos_<split>.pkl (detzero_b200.track.
+    ground_truth_from_infos reads them): per frame 'sequence_name', 'sample_idx' (the frame index), 'frame_id', 'pose' and 'annos'
+    with one row per box in track order: 'name', 'obj_ids' (seeded strings), 'gt_boxes_lidar' (7), 'gt_boxes_global' (9, the
+    velocity as the finite difference of the centres), 'difficulty' (0, or difficulty[b][j] where given) and 'num_points_in_gt' (the
+    object points the sequence put in the box)."""
+    g = np.random.default_rng([int(seed), 0x6D7])
+    F, B = len(s['poses']), len(s['box_num'])
+    ids = ['%s_%08x' % (name, int(v)) for v in g.integers(0, 1 << 32, B)]
+    rows = [[] for _ in range(F)]
+    for b in range(B):
+        n = int(s['box_num'][b])
+        for j in range(n):
+            f = int(s['frame_of_box'][b, j])
+            w = s['boxes'][b, j]
+            nxt = s['boxes'][b, j + 1] if j + 1 < n else w
+            prv = s['boxes'][b, j - 1] if j + 1 == n and n > 1 else w
+            vel = ((nxt[:2] - w[:2]) if j + 1 < n else (w[:2] - prv[:2])) * 10.
+            P = s['poses'][f]
+            lid = np.concatenate([(w[:3] - P[:3, 3]) @ P[:3, :3], w[3:6],
+                                  [np.arctan2(np.sin(w[6] - np.arctan2(P[1, 0], P[0, 0])), np.cos(w[6] - np.arctan2(P[1, 0], P[0, 0])))]])
+            d = 0 if difficulty is None else int(difficulty[b][j])
+            rows[f].append((CLASS_NAMES[int(s['cls'][b]) - 1], ids[b], lid, np.concatenate([w, vel]), d, int(s['points_per_box'][b, j])))
+    infos = []
+    for f in range(F):
+        r = rows[f]
+        infos.append({'sequence_name': name, 'sample_idx': f, 'frame_id': f, 'pose': s['poses'][f].copy(),
+                      'annos': {'name': np.array([x[0] for x in r], dtype='<U10'), 'obj_ids': np.array([x[1] for x in r], dtype='<U32'),
+                                'gt_boxes_lidar': np.array([x[2] for x in r], np.float32).reshape(-1, 7),
+                                'gt_boxes_global': np.array([x[3] for x in r], np.float64).reshape(-1, 9),
+                                'difficulty': np.array([x[4] for x in r], np.int32),
+                                'num_points_in_gt': np.array([x[5] for x in r], np.int32)}})
+    return infos
 
 
 def detections_from_sequence(s, seed, miss=0.1, fp=10, K=500):

@@ -260,6 +260,27 @@ int dz_track_sequences(const float* boxes, const int* counts, const int* num_fra
                        float* ent_score, int* ent_hit, int* ent_frame, unsigned char* kept, int* overflow, void* ws,
                        size_t ws_bytes, dz_stream_t stream);
 
+/* ---- tracks against ground truth (csrc/track_gt.cu) ------------------------------------------------------------------------ */
+/* The trajectory scoring of DetZero's training-target assignment (target_assign.assign_track_target,
+ * tracking/detzero_track/models/tracking_modules/target_assign.py:8-139; recall = 0, BEV IoU) and of its tracklet recall
+ * (TrackRecall.eval_single_seq, tracking/detzero_track/utils/track_recall.py:153-262 with get_trajectory_similarity of
+ * utils/track_calculation.py:84-123; recall = 1, 3-D IoU when iou_3d), for S sequences in one launch.
+ * Ground truth: gt_box (S, F, G, 7) float32 lidar boxes, gt_world (S, F, G, 9) float64 world boxes, gt_cls (S, F, G) class 1..3 or 0
+ * (never scored), gt_obj the per-sequence object index (0 .. n_obj[s] - 1, -1 for a class-0 row), gt_diff / gt_npts difficulty and
+ * num_points_in_gt, gt_cnt (S, F) rows per frame, gt_num_frames (S).  Tracks: the dz_track_sequences outputs trk (S, max_tracks, 6),
+ * n_tracks, ent_box (S, max_entries, 9), ent_frame, and poses (S, F, 4, 4) lidar -> world of the same frames.
+ * thresholds (3 doubles): the IoU threshold per class; class_mask: bit c set when class c is scored.
+ * Outputs: obj_rec (S, max_objects, 5) int32 [matched track or -1, match count, trajectory length, bucket 1 (L1) / 2 (L2), class];
+ * trk_rec (S, max_tracks, 4) int32 [matched object or -1, class, entry count, dynamic]; ent_iou (S, max_entries) float32 the BEV IoU
+ * of each entry with its track's matched object in that frame (0 where absent); overflow[s] != 0 when the max_pairs pair table or the
+ * assignment scratch overflowed (the sequence's outputs are then invalid).  One block per sequence, no host synchronisation. */
+size_t dz_track_gt_ws_bytes(int S, int F, int max_objects, int max_tracks, int max_entries, int max_pairs);
+int dz_track_gt(const float* gt_box, const double* gt_world, const int* gt_cls, const int* gt_obj, const int* gt_diff, const int* gt_npts,
+                const int* gt_cnt, const int* gt_num_frames, const int* n_obj, int S, int F, int G, int max_objects, const int* trk,
+                const int* n_tracks, const double* ent_box, const int* ent_frame, const double* poses, int max_tracks,
+                int max_entries, const double* thresholds, int class_mask, int recall, int iou_3d, int max_pairs, int* obj_rec,
+                int* trk_rec, float* ent_iou, int* overflow, void* ws, size_t ws_bytes, dz_stream_t stream);
+
 /* ---- refiner inputs (SURVEY.md 8f row 2), csrc/refine_data.cu -------------------------------------------------------------- */
 /* Builds the eval inputs of the refiner modules for B tracks of up to L box slots straight from the collated frames, in one call per
  * kind: PRM (kind 0) = WaymoPositionDataset.extract_track_feature (refining/detzero_refine/datasets/waymo/waymo_position_dataset.py:31-184),
