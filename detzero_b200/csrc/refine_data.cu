@@ -34,6 +34,7 @@
 //      float32 test), where the reference tests float32 world points: only points within ~1e-3 m of an enlarged face can differ.
 #include "common.cuh"
 #include "boxgeom.cuh"
+#include "refine_frame.cuh"
 
 enum { RD_PRM = 0, RD_CRM = 1, RD_GRM = 2 };
 enum { ST_PRM_Q = 0, ST_PRM_M = 1, ST_CRM = 2, ST_GRM_Q = 3, ST_GRM_M = 4 };
@@ -67,14 +68,6 @@ __host__ __device__ __forceinline__ unsigned long long mix64(unsigned long long 
 
 __device__ __forceinline__ unsigned long long key_base(unsigned long long seed, long long uid, int slot, int stream) {
     return mix64(mix64(mix64(seed) ^ (unsigned long long)uid) ^ (((unsigned long long)slot << 8) | (unsigned long long)stream));
-}
-
-// data_utils.limit_heading_range: into [-pi, pi)
-__device__ __forceinline__ double wrap_pi(double a) {
-    const double PI = 3.14159265358979323846;
-    while (a >= PI) a -= 2 * PI;
-    while (a < -PI) a += 2 * PI;
-    return a;
 }
 
 __device__ __forceinline__ int track_len(const RdParams& P, int b) { return min(max(P.box_num[b], 0), P.L); }
@@ -125,10 +118,11 @@ __global__ void k_rd_prep(RdParams P) {
     }
     // init_coords_transform: init box = traj[L // 2] (heading wrapped); trajectory into its frame
     const double* bi = P.boxes + ((size_t)b * P.L + L / 2) * 7;
-    const double yi = wrap_pi(bi[6]), c = cos(yi), s = sin(yi);
+    const InitFrame fr = init_frame(bi);
+    const double yi = fr.yaw, c = fr.c, s = fr.s;
     o.E[0] = c; o.E[1] = s; o.E[4] = -s; o.E[5] = c; o.E[10] = 1.0;
-    const double dx = bw[0] - bi[0], dy = bw[1] - bi[1], dz = bw[2] - bi[2];
-    double loc[7] = {c * dx + s * dy, -s * dx + c * dy, dz, bw[3], bw[4], bw[5], wrap_pi(wrap_pi(bw[6]) - yi)};
+    double loc[7];
+    to_init_frame(fr, bi, bw, loc);
     o.E[3] = loc[0]; o.E[7] = loc[1]; o.E[11] = loc[2];
     const double ch = cos(loc[6]), sh = sin(loc[6]);
     for (int k = 0; k < 8; ++k) {                                         // box_utils.boxes_to_corners_3d

@@ -8,6 +8,7 @@ import numpy as np
 import torch
 
 from .refine import data as rdata
+from .refine import score as rscore
 from .track import CLASS_NAMES
 
 
@@ -15,10 +16,13 @@ class OffboardResult:
     """Final boxes of one sequence: rows (F, R, 9) f32 [x, y, z, dx, dy, dz, heading, score, label], obj_id (F, R) int32 (-1: a
     dropped detection), count (F) int32 (see refine.data.combine_frames), and the per-track tables they came from, in output order:
     tables['prm_lidar'] (B, L, 7) f64, 'grm_pred' (B, 7) f32, 'scores' (B, L) f32, 'frame_of_box' (B, L), 'box_num' (B), 'cls' (B),
-    'track_id' (B) int64; poses (F, 4, 4) f64."""
+    'track_id' (B) int64; poses (F, 4, 4) f64.  When the sequence was scored against ground truth (refine_sequence(assign=...)):
+    recall {class: {'PRM', 'GRM', 'CRM': the refine.score record}} and tables['refine_iou'] (B, L) f32 (the CRM's IoU labels, -1
+    past box_num), tables['matched'] (B, L) uint8; recall is None otherwise."""
 
-    def __init__(self, tables, poses, rows, obj_id, count):
+    def __init__(self, tables, poses, rows, obj_id, count, recall=None):
         self.tables, self.poses, self.rows, self.obj_id, self.count = tables, poses, rows, obj_id, count
+        self.recall = recall
 
     def frame_order(self):
         """the sequence frame indices that have rows, in order of first appearance over the tracks (convert_frame_format's order)"""
@@ -74,7 +78,7 @@ class _Stages:
 
 
 def refine_sequence(frames, frame_offsets, poses, track_result, models, sequence=0, class_names=CLASS_NAMES, combine_conf_res=True,
-                    combine_drop=True, chunk=16, seed=0, max_rows=1024, timings=None):
+                    combine_drop=True, chunk=16, seed=0, max_rows=1024, timings=None, assign=None, recall_thresholds=None):
     """DetZero's refine and combine stages over one tracked sequence (refining/tools/test.py per class, then combine_final).
     frames / frame_offsets / poses: the sequence's collated points, as refine.data.position_inputs takes them (frame f of the tracker
     is frame f here).  track_result: track.TrackResult, sequence ``sequence`` of it.  models: {class name: {'PRM', 'GRM', 'CRM':
@@ -85,6 +89,11 @@ def refine_sequence(frames, frame_offsets, poses, track_result, models, sequence
     combine_drop, the tracker's dropped detections of every class.  Tracks of unlisted classes are left out.
     timings: an optional dict that receives the device milliseconds of each stage (inputs, forwards, revert, combine; one extra
     synchronisation).  Returns an OffboardResult.
+    assign: a track.AssignResult of ``track_result`` (track.assign_track_target); each chunk then also gets its ground truth
+    (refine.data.track_targets, stage 'targets') and is scored (refine.score: the PRM, GRM and, with combine_conf_res, CRM records
+    and the IoU labels, stage 'score'; one device-to-host copy per record and chunk), and the chunks' records are added up per
+    class into OffboardResult.recall.  recall_thresholds: {class: list}, by default refine.score.RECALL_THRESH_LIST.  Without
+    ``assign`` none of this runs.
     Deviations from combine_final: the reference writes one file per class and its class loop accumulates, so each file holds every
     class processed so far, and its last file omits sequences without a track of the last class; here one call gives all listed
     classes of its sequence.  combine_det raises KeyError for a frame with tracks but no drop entry; here that frame has no
@@ -96,6 +105,8 @@ def refine_sequence(frames, frame_offsets, poses, track_result, models, sequence
         missing = [k for k in need if k not in models.get(c, {})]
         if missing:
             raise KeyError('models[%r] lacks %s' % (c, ', '.join(missing)))
+    thresholds = dict(rscore.RECALL_THRESH_LIST)
+    thresholds.update(recall_thresholds or {})
     chunk = int(chunk)
     if chunk < 1:
         raise ValueError('chunk must be positive')
@@ -106,11 +117,19 @@ def refine_sequence(frames, frame_offsets, poses, track_result, models, sequence
     poses = torch.as_tensor(poses).to(device=dev, dtype=torch.float64).contiguous()
     st = _Stages(timings)
     parts = {k: [] for k in ('prm_lidar', 'grm_pred', 'scores', 'frame_of_box', 'box_num', 'cls', 'track_id')}
+    recall = None
+    if assign is not None:
+        parts['refine_iou'], parts['matched'] = [], []
+        recall = {c: {k: rscore.empty_record(thresholds[c], k == 'CRM') for k in (('PRM', 'GRM', 'CRM') if combine_conf_res
+                                                                                  else ('PRM', 'GRM'))} for c in class_names}
     for c in class_names:
         tb = track_result.track_batch(c, sequence=sequence)
         m = models[c]
         for c0 in range(0, len(tb), chunk):
             sub = tb.select(slice(c0, c0 + chunk))
+            if assign is not None:
+                st.mark('targets')
+                tg = rdata.track_targets(assign, sub, sequence)
             st.mark('position_inputs')
             pin = rdata.position_inputs(frames, frame_offsets, poses, sub, seed=seed)
             st.mark('prm_forward')
@@ -127,7 +146,18 @@ def refine_sequence(frames, frame_offsets, poses, track_result, models, sequence
             else:
                 score = sub.scores
             st.mark('revert')
-            lidar, _ = rdata.revert_position_boxes(pred, poses, sub)
+            lidar, world = rdata.revert_position_boxes(pred, poses, sub)
+            if assign is not None:
+                st.mark('score')
+                th, size7 = thresholds[c], size.float().reshape(len(sub), 7)
+                iou = rscore.refine_iou_labels(world, size7, sub, tg)
+                new = {'PRM': rscore.position_recall(world, sub, tg, th), 'GRM': rscore.geometry_recall(size7, sub, tg, th)}
+                if combine_conf_res:
+                    new['CRM'] = rscore.confidence_recall(sub.scores, score, iou, sub, tg, th)
+                for k, r in new.items():
+                    recall[c][k] = rscore.accumulate(recall[c][k], r)
+                parts['refine_iou'].append(iou)
+                parts['matched'].append(tg.matched)
             st.mark(None)
             parts['prm_lidar'].append(lidar)
             parts['grm_pred'].append(size.float().reshape(len(sub), 7))
@@ -138,8 +168,9 @@ def refine_sequence(frames, frame_offsets, poses, track_result, models, sequence
             parts['track_id'].append(sub.track_uid)
     L = 200 if not parts['prm_lidar'] else parts['prm_lidar'][0].shape[1]
     empty = {'prm_lidar': (0, L, 7), 'grm_pred': (0, 7), 'scores': (0, L), 'frame_of_box': (0, L), 'box_num': (0,), 'cls': (0,),
-             'track_id': (0,)}
-    dtypes = {'prm_lidar': torch.float64, 'grm_pred': torch.float32, 'scores': torch.float32, 'track_id': torch.int64}
+             'track_id': (0,), 'refine_iou': (0, L), 'matched': (0, L)}
+    dtypes = {'prm_lidar': torch.float64, 'grm_pred': torch.float32, 'scores': torch.float32, 'track_id': torch.int64,
+              'refine_iou': torch.float32, 'matched': torch.uint8}
     tables = {k: torch.cat(v) if v else torch.zeros(empty[k], dtype=dtypes.get(k, torch.int32), device=dev) for k, v in parts.items()}
     drop = (track_result.boxes[sequence], track_result.counts[sequence], track_result.kept[sequence]) if combine_drop else None
     st.mark('combine')
@@ -147,4 +178,4 @@ def refine_sequence(frames, frame_offsets, poses, track_result, models, sequence
                                                tables['box_num'], tables['cls'], tables['track_id'], F, drop=drop, max_rows=max_rows)
     st.mark(None)
     st.finish()
-    return OffboardResult(tables, poses, rows, obj_id, count)
+    return OffboardResult(tables, poses, rows, obj_id, count, recall)

@@ -7,7 +7,8 @@ daemon/prepare_object_data.py:241-327.  Each builder returns the dict the module
 reference's keys, shapes and float32 dtype.  Sampling is keyed on (seed, track_uid) and deterministic; see csrc/refine_data.cu for
 that function and the other deliberate deviations (float64 geometry, per-track GRM query count, the crop's coordinates).
 ``combine_frames`` puts the refined tracks of a sequence together into per-frame result rows (csrc/combine.cu), replacing
-daemon/combine_output.py's convert_frame_format and combine_det.
+daemon/combine_output.py's convert_frame_format and combine_det.  ``track_targets`` attaches the ground truth of an assignment
+(track.assign_track_target) to a TrackBatch (csrc/refine_gt.cu); refine.score turns it into the recall records and IoU labels.
 """
 import zlib
 
@@ -80,6 +81,77 @@ class TrackBatch:
         """the tracks idx (a slice or an index list) as a TrackBatch"""
         return TrackBatch(self.boxes[idx], self.frame_of_box[idx], self.scores[idx], self.box_num[idx], self.cls[idx],
                           self.track_uid[idx], self.boxes.device)
+
+
+class TrackTargets:
+    """Ground truth of the B tracks of a TrackBatch (device tensors), as daemon/prepare_object_data.py:64-190 attaches it to each
+    track box: gt_boxes (B, L, 7) float64 world (zeros where the matched object has no row in the slot's frame, for an unmatched
+    track and past box_num), matched (B, L) uint8 (1 where the object is present; 1 on every valid slot of an unmatched track, as
+    the reference has it), matched_tracklet (B) uint8, state (B) int32 (1 dynamic: the object's for a matched track, the tracker's
+    otherwise), gt_traj (B, L, 7) float32 (the dataset's gt_pos_trajectory: gt_boxes in the track's init-box frame) and obj (B)
+    int32, the matched object's index in the GroundTruth tables or -1."""
+
+    def __init__(self, gt_boxes, matched, matched_tracklet, state, gt_traj, obj):
+        self.gt_boxes, self.matched, self.matched_tracklet, self.state = gt_boxes, matched, matched_tracklet, state
+        self.gt_traj, self.obj = gt_traj, obj
+
+    def __len__(self):
+        return self.obj.shape[0]
+
+    def select(self, idx):
+        """the tracks idx (a slice or an index list) as a TrackTargets"""
+        return TrackTargets(self.gt_boxes[idx], self.matched[idx], self.matched_tracklet[idx], self.state[idx], self.gt_traj[idx],
+                            self.obj[idx])
+
+
+def refine_targets(gt_world, gt_obj, gt_cnt, trk_obj, obj_state, trk_state, tracks):
+    """dz_refine_targets on raw tables: gt_world (F, G, 9) f64, gt_obj (F, G), gt_cnt (F) of one sequence; trk_obj, obj_state,
+    trk_state (B) per track of ``tracks`` (a TrackBatch) -> TrackTargets.  Enqueue only."""
+    dev = tracks.boxes.device
+    B, L = len(tracks), tracks.L
+    i32 = lambda t: torch.as_tensor(t).to(device=dev, dtype=torch.int32).contiguous()
+    gt_world = torch.as_tensor(gt_world).to(device=dev, dtype=torch.float64).contiguous()
+    F, G = int(gt_world.shape[0]), int(gt_world.shape[1])
+    assert gt_world.shape == (F, G, 9), gt_world.shape
+    gt_obj, gt_cnt, trk_obj, obj_state, trk_state = i32(gt_obj), i32(gt_cnt), i32(trk_obj), i32(obj_state), i32(trk_state)
+    assert gt_obj.shape == (F, G) and gt_cnt.shape == (F,) and trk_obj.shape == obj_state.shape == trk_state.shape == (B,)
+    out = TrackTargets(torch.zeros((B, L, 7), dtype=torch.float64, device=dev), torch.zeros((B, L), dtype=torch.uint8, device=dev),
+                       torch.zeros((B,), dtype=torch.uint8, device=dev), torch.zeros((B,), dtype=torch.int32, device=dev),
+                       torch.zeros((B, L, 7), dtype=torch.float32, device=dev), trk_obj)
+    if B and F and G:
+        check(lib().dz_refine_targets(ops._p(gt_world), ops._p(gt_obj), ops._p(gt_cnt), F, G, ops._p(trk_obj), ops._p(obj_state),
+                                      ops._p(trk_state), ops._p(tracks.boxes), ops._p(tracks.frame_of_box), ops._p(tracks.box_num),
+                                      B, L, ops._p(out.gt_boxes), ops._p(out.matched), ops._p(out.matched_tracklet),
+                                      ops._p(out.state), ops._p(out.gt_traj), ops._stream()), 'refine_targets')
+        ops._count(1)
+    return out
+
+
+def track_targets(assign_result, tracks, sequence=0):
+    """The ground truth of every track of ``tracks`` (a TrackBatch of sequence ``sequence`` of the TrackResult that
+    ``assign_result``, a track.AssignResult, scored; frame_of_box indexes the sequence's frames) -> TrackTargets
+    (csrc/refine_gt.cu).  Replaces the ground-truth half of daemon/prepare_object_data.py:64-190 and the gt_pos_trajectory of
+    WaymoPositionDataset.extract_track_feature.  The batch's track_uid are looked up among the sequence's track ids on the device;
+    one flag is read back to reject a track_uid the sequence does not have."""
+    tr, gt = assign_result.track_result, assign_result.gt
+    s = int(sequence)
+    n = int(tr.n_tracks[s])
+    dev = tracks.boxes.device
+    B = len(tracks)
+    trk = tr.trk[s, :n]
+    if B and n:
+        ids, order = torch.sort(trk[:, 0].long())
+        pos = torch.searchsorted(ids, tracks.track_uid).clamp_(max=n - 1)
+        if not bool((ids[pos] == tracks.track_uid).all()):
+            raise ValueError('a track_uid of the batch is not a track id of sequence %d' % s)
+        row = order[pos]
+        rec = assign_result.trk_rec[s, :n][row]
+        trk_obj, obj_state, trk_state = rec[:, 0], rec[:, 3], trk[row, 4]
+    elif B:
+        raise ValueError('sequence %d has no tracks' % s)
+    else:
+        trk_obj = obj_state = trk_state = torch.zeros((0,), dtype=torch.int32, device=dev)
+    return refine_targets(gt.world[s], gt.obj[s], gt.counts[s], trk_obj, obj_state, trk_state, tracks)
 
 
 def _frames_args(frames, frame_offsets, poses):

@@ -333,6 +333,45 @@ int dz_combine_frames(const double* prm_lidar, const float* grm_pred, const floa
                       const int32_t* det_count, const unsigned char* kept, int K, int F, int R, float* rows, int32_t* obj_id,
                       int32_t* count, int32_t* overflow, void* ws, size_t ws_bytes, dz_stream_t stream);
 
+/* ---- the refiners against ground truth (csrc/refine_gt.cu) --------------------------------------------------------------------- */
+/* Ground truth per track slot, for B tracks of one sequence with L box slots (daemon/prepare_object_data.py:64-190, which attaches
+ * gt_boxes_global / matched / matched_tracklet / state to each track box on the host, and the gt_pos_trajectory of
+ * refining/detzero_refine/datasets/waymo/waymo_position_dataset.py:41-42,76-80,159-160).  gt_world (F, G, 9) f64, gt_obj (F, G),
+ * gt_cnt (F): one sequence of the dz_track_gt ground-truth tables.  trk_obj (B): the object matched to each track (dz_track_gt's
+ * trk_rec[.., 0]) or -1; obj_state / trk_state (B): the matched object's state (trk_rec[.., 3]) and the tracker's own (trk[.., 4]).
+ * boxes (B, L, 7) f64 world, frame_of_box (B, L), box_num (B): the track tables of dz_refine_inputs.
+ * Outputs: gt_boxes (B, L, 7) f64 world, the matched object's box in the slot's frame (its first row there), zeros where it has none,
+ * for an unmatched track and past box_num; matched (B, L) u8: 1 where the object is present, and 1 on every valid slot of an
+ * unmatched track (prepare_object_data.py:184-188); matched_tracklet (B) u8; state (B) (1 dynamic): the object's for a matched
+ * track, the tracker's otherwise; gt_traj (B, L, 7) f32: gt_boxes in the frame of the track's init box (slot box_num / 2), by the
+ * float64 transform dz_refine_inputs kind 0 applies to pos_trajectory (zero boxes included, as init_coords_transform does), rows
+ * past box_num zero. */
+int dz_refine_targets(const double* gt_world, const int32_t* gt_obj, const int32_t* gt_cnt, int F, int G, const int32_t* trk_obj,
+                      const int32_t* obj_state, const int32_t* trk_state, const double* boxes, const int32_t* frame_of_box,
+                      const int32_t* box_num, int B, int L, double* gt_boxes, unsigned char* matched,
+                      unsigned char* matched_tracklet, int32_t* state, float* gt_traj, dz_stream_t stream);
+/* out[i] = 3-D IoU of boxes_a[i] and boxes_b[i] (rows of >= 7 floats, row strides lda / ldb): the diagonal of dz_boxes_pairwise
+ * kind 2, bit for bit.  Replaces iou3d_nms_utils.boxes_iou3d_gpu(a, b).diag(), which computes n x n rotated clips to keep n. */
+int dz_boxes_iou3d_aligned(const float* boxes_a, int lda, const float* boxes_b, int ldb, int n, float* out, dz_stream_t stream);
+/* The per-box IoUs and per-track counts of generate_recall_record (refining/detzero_refine/models/position_refine_model.py:100-133,
+ * geometry_refine_model.py:98-141), one block per track, one launch: in_boxes / out_boxes / gt_boxes (B, L, 7) f64 world (the box
+ * before and after refinement, and dz_refine_targets' gt_boxes), size (B, 7) f32 or NULL: when given, the refined box takes its
+ * dx, dy, dz from size[b][3:6] (the GRM's prediction, geometry_refine_model.py:105-108).  Every pair is re-centred on its ground-truth
+ * centre in float64, rounded to float32 and clipped as dz_boxes_pairwise kind 2 does.  A slot is scored when matched_tracklet[b] and
+ * matched[b][j] and j < box_num[b].  thresholds: n_thresholds <= 8 host doubles, compared as float32 (iou > th).
+ * Outputs: iou_in, iou_out (B, L) f32 (0 on the slots not scored); rec (B, 1 + 2 n) int32 [scored slots, count(iou_in > th_k)..,
+ * count(iou_out > th_k)..].  A ground-truth box without volume gives 0.
+ * out_boxes == NULL is label mode, generate_refine_boxes_iou (daemon/generate_iou_gt.py:36-53): every slot below box_num is scored,
+ * in_boxes (with size, when given) against gt_boxes; only iou_in (and rec, when not NULL) is written. */
+int dz_refine_score(const double* in_boxes, const double* out_boxes, const float* size, const double* gt_boxes,
+                    const unsigned char* matched, const unsigned char* matched_tracklet, const int32_t* box_num, int B, int L,
+                    const double* thresholds, int n_thresholds, float* iou_in, float* iou_out, int32_t* rec, dz_stream_t stream);
+/* The CRM counters (confidence_refine_model.py:81-104) per track over its box_num slots, from conf_score, pred_score, iou (B, L) f32:
+ * rec (B, 5) int32 [matched_up, matched_down, unmatched_up, unmatched_down, box_num] with gt_label = iou >= 0.7 (float32) and
+ * up = pred_score >= conf_score. */
+int dz_confidence_score(const float* conf_score, const float* pred_score, const float* iou, const int32_t* box_num, int B, int L,
+                        int32_t* rec, dz_stream_t stream);
+
 /* ---- test-time augmentation (CenterPoint TTA) ------------------------------------------------------------- */
 /* A view is 4 host floats [op, p1, p2, p3]: DZ_TTA_ORIGINAL; DZ_TTA_FLIP_X (y = -y); DZ_TTA_FLIP_Y (x = -x); DZ_TTA_FLIP_XY;
  * DZ_TTA_ROT with p1, p2 = cos, sin of the float32 angle (float32 torch on the CPU, as the reference computes them) and, for

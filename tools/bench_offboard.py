@@ -8,7 +8,10 @@ chunks of 16 tracks per class, revert, combine_frames with the dropped detection
   * sequences/s of the whole chain (track + refine_sequence, CUDA events around both, including the host stalls between kernels);
   * the combine_frames call on its own, best of --reps (memset, three kernels and its two host reads).
 
-    python tools/bench_offboard.py [--tracks 300] [--frames 199] [--background 180000] [--chunk 16] [--reps 5]
+With --assign the tracks are also assigned to the sequence's ground truth (track.assign_track_target, outside the timed chain) and
+every chunk is scored (refine.data.track_targets, refine.score): the stages 'targets' and 'score' then appear with their share.
+
+    python tools/bench_offboard.py [--tracks 300] [--frames 199] [--background 180000] [--chunk 16] [--reps 5] [--assign]
 """
 import argparse
 import json
@@ -23,7 +26,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from detzero_b200 import offboard, synthetic              # noqa: E402
 from detzero_b200.refine import data as D                 # noqa: E402
-from detzero_b200.track import track_sequences            # noqa: E402
+from detzero_b200.track import assign_track_target, ground_truth_from_infos, track_sequences            # noqa: E402
 
 
 def _card():
@@ -46,6 +49,7 @@ def main():
     ap.add_argument('--mode', default='fp32', help='refiner COMPUTE_MODE')
     ap.add_argument('--reps', type=int, default=5)
     ap.add_argument('--seed', type=int, default=1)
+    ap.add_argument('--assign', action='store_true', help='score the refiners against the ground truth of the sequence')
     a = ap.parse_args()
     assert torch.cuda.is_available(), 'bench_offboard needs a GPU'
     dev = torch.device('cuda:0')
@@ -59,16 +63,20 @@ def main():
     frames, poses = torch.from_numpy(s['frames']).to(dev), torch.from_numpy(s['poses']).to(dev)
     boxes, counts, poses_h = torch.from_numpy(boxes).to(dev), torch.from_numpy(counts).to(dev), torch.from_numpy(s['poses']).to(dev)
     models = synthetic.refine_models(a.seed, mode=a.mode, device=dev)
+    gt = ground_truth_from_infos(synthetic.synthetic_ground_truth(s, a.seed), ['seq'], device=dev) if a.assign else None
 
     def chain(timings=None):
-        ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
         ev[0].record()
         res = track_sequences(boxes, counts, poses_h, max_entries=1 << 20)
         ev[1].record()
-        out = offboard.refine_sequence(frames, s['frame_offsets'], poses, res, models, chunk=a.chunk, seed=a.seed, timings=timings)
+        assign = assign_track_target(res, gt) if a.assign else None                 # not timed: it is not part of the chain
         ev[2].record()
+        out = offboard.refine_sequence(frames, s['frame_offsets'], poses, res, models, chunk=a.chunk, seed=a.seed, timings=timings,
+                                       assign=assign)
+        ev[3].record()
         torch.cuda.synchronize()
-        return res, out, ev[0].elapsed_time(ev[1]), ev[1].elapsed_time(ev[2])
+        return res, out, ev[0].elapsed_time(ev[1]), ev[2].elapsed_time(ev[3])
 
     with torch.no_grad():
         chain()                                                                  # warm-up
@@ -86,6 +94,10 @@ def main():
                       'stage_share': {k: round(v / total, 4) for k, v in stages.items()},
                       'chain_ms': round(best, 2), 'sequences_per_s': round(1e3 / best, 3), 'tracks_per_s': round(n_tracks * 1e3 / best, 1),
                       'generate_s': round(gen_s, 1)}), flush=True)
+    if a.assign:
+        print(json.dumps({'scoring_share_of_chain': {k: round(stages[k] / total, 4) for k in ('targets', 'score')},
+                          'recall': {c: {k: {n: v for n, v in r.items() if not isinstance(v, list)} for k, r in out.recall[c].items()}
+                                     for c in out.recall}}), flush=True)
 
     t = out.tables
     drop = (res.boxes[0], res.counts[0], res.kept[0])
