@@ -15,18 +15,30 @@
 //
 // Kernel structure (one CTA per SM, persistent over the tile list; roles by warp):
 //   warps 0-7      two consumer warpgroups (64 rows each): wgmma bf16 (M64 x Cout x K16) into register accumulators; after the
-//                  tile's last block the accumulators pass through a shared-memory staging tile 32 columns at a time and
-//                  warps 0-3 run the epilogue: scale/shift (+residual) -> ReLU -> plane split -> stores
+//                  tile's last block every consumer thread runs the epilogue of its own fragment (two rows, two adjacent
+//                  columns per 8): scale/shift (+residual) -> ReLU -> plane split -> 32-bit stores, with no staging tile and no
+//                  barrier between the warpgroups
 //   warps 8-15     producers (all of them fill one pipeline stage at a time): cp.async zero-fill gather of the neighbour rows of a 64-element block of
-//                  the (offset, channel) reduction dimension into K-major SW128 smem; one lane TMA-loads the weight tile
+//                  the (offset, channel) reduction dimension into K-major SW128 smem.  A lane's arrival on the stage barrier is
+//                  asynchronous (cp.async.mbarrier.arrive.noinc), so it moves on to the next free stage at once: the gathers of
+//                  every free stage of the ring are in flight together, and their number grows with the stage count
 //   fence warp     one thread turns "the cp.async data of stage s has landed" (async mbarrier arrival of the producers) into "stage s
 //                  is visible to the tensor core": fence.proxy.async, then arrives on the barrier the consumers wait on, so
 //                  neither the producers nor the consumers wait for the landing latency themselves
 //   tile warp      walks the CTA's tiles (heaviest-first tile order of the rulebook schedule, serpentine over the CTAs), loads
 //                  the 128 x 27 neighbour rows of tile t+1/t+2 into the double-buffered table while tile t is computed
+//   weight warp    one thread TMA-loads the weight slice ([w0 ; w1] rows x 64 reduction elements) of each live block into the
+//                  weight ring, in the consumers' block order
 // so a tile's prologue (table load) hides under the neighbouring tile's main loop and the producers run ahead into the next
 // tile while the consumers run the epilogue.  No atomics: deterministic; a row's accumulation order over
 // the reduction blocks never depends on the schedule, so results are bit-identical with or without it.
+//
+// Shared memory (SbCfg, <= 227 KB): [A ring: STAGES x PLANES x 16 KB][weight ring: WSTAGES x PLANES x COUT x 128 B]
+// [table 2 x 14 KB][block lists, scale/shift, barriers].  The gathered A block and its weight slice have separate rings: the
+// weight slice only has to cover the MMA look-ahead (one block in flight, one being issued, one loading), so the rest of
+// shared memory goes to A stages, i.e. to gathers in flight, and what is left after them to weight slots.  bf16x2: 5 A
+// stages at Cout = 16 and 32, 4 at Cout = 64, 3 at Cout = 128; bf16: 8 at every Cout.  The weight warp keeps the
+// tile's block list in registers, so it releases the table buffer as soon as it has read it, like the other roles.
 #include <cuda_bf16.h>
 #include "common.cuh"
 #include "tc.cuh"
@@ -42,14 +54,17 @@ template <int COUT, int PLANES>
 struct SbCfg {
     static constexpr int WROWS = PLANES * COUT;                     // rows of the weight tile: [w0 ; w1]
     static constexpr int W_BYTES = WROWS * 128;
-    static constexpr int STAGE_BYTES = PLANES * SB_A_BYTES + W_BYTES;
+    static constexpr int STAGE_BYTES = PLANES * SB_A_BYTES;         // one gathered A block
     static constexpr int NBR_BYTES = 2 * SB_NPLANES * SB_ROWS * 4;   // double-buffered tile block: K neighbour planes + the row plane
     static constexpr int MISC_BYTES = 2 * 64 * 4 + 2 * COUT * 4 + 512;                     // block lists | scale,shift | barriers
-    static constexpr int CW = COUT < 32 ? COUT : 32;                                         // accumulator columns per epilogue pass
-    static constexpr int STG_LD = CW + 4;
-    static constexpr int STG_BYTES = SB_ROWS * STG_LD * 4;                                   // epilogue staging tile
-    static constexpr int STAGES_FIT = (232448 - NBR_BYTES - MISC_BYTES - STG_BYTES - 1024) / STAGE_BYTES;
-    static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;   // as deep as shared memory allows: 2 (bf16x2, Cout = 128) .. 8
+    static constexpr int RING_BYTES = 232448 - NBR_BYTES - MISC_BYTES - 1024;               // A ring + weight ring
+    // weight ring: at least one slot under the MMA still in flight, one for the MMA being issued and one loading; the A ring
+    // takes as many stages as fit beside that (up to 8), and what is left deepens the weight ring (up to 8 slots)
+    static constexpr int STAGES_FIT = (RING_BYTES - 3 * W_BYTES) / STAGE_BYTES;
+    static constexpr int STAGES = STAGES_FIT > 8 ? 8 : STAGES_FIT;   // 3 (bf16x2, Cout = 128) .. 8
+    static constexpr int WSTAGES_FIT = (RING_BYTES - STAGES * STAGE_BYTES) / W_BYTES;
+    static constexpr int WSTAGES = WSTAGES_FIT > 8 ? 8 : WSTAGES_FIT;
+    static_assert((3 * STAGES + 2 * WSTAGES + 4) * 8 <= 512, "barriers");
     // ALL producer warps fill ONE stage at a time (16 rows each): a stage is complete after 1/NPROD of the LSU time a
     // warp-per-stage split needs, so the oldest stage lands early and the ring covers the MMA -> commit -> refill latency
     // with the two consumer warpgroups holding Cout/2 accumulator registers each, 8 producer warps leave too few registers for
@@ -58,8 +73,9 @@ struct SbCfg {
     static constexpr int CONSUMERS = 8;
     static constexpr int WARP_TILE = CONSUMERS + NPROD;
     static constexpr int WARP_FENCE = WARP_TILE + 1;
-    static constexpr int THREADS = 32 * (WARP_FENCE + 1);
-    static constexpr int SMEM = STAGES * STAGE_BYTES + NBR_BYTES + MISC_BYTES + STG_BYTES + 1024;
+    static constexpr int WARP_W = WARP_FENCE + 1;
+    static constexpr int THREADS = 32 * (WARP_W + 1);
+    static constexpr int SMEM = STAGES * STAGE_BYTES + WSTAGES * W_BYTES + NBR_BYTES + MISC_BYTES + 1024;
 };
 
 // bounded wait: a protocol bug turns into a trap (CUDA error) instead of a hung GPU
@@ -97,16 +113,19 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
 
     extern __shared__ unsigned char smem_raw[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    int* s_nbr = reinterpret_cast<int*>(smem + S * Cfg::STAGE_BYTES);            // [2][28][128]: planes k < K neighbour rows, plane K = output rows (-1: none)
+    constexpr int WS = Cfg::WSTAGES;
+    unsigned char* s_w = smem + S * Cfg::STAGE_BYTES;                              // [WS] weight slices of the live blocks
+    int* s_nbr = reinterpret_cast<int*>(s_w + WS * Cfg::W_BYTES);                 // [2][28][128]: planes k < K neighbour rows, plane K = output rows (-1: none)
     int* s_blk = s_nbr + 2 * SB_NPLANES * SB_ROWS;                                // [2][64]  live reduction blocks; [63] = count, [62] = tile (-1: end)
     float* s_scale = reinterpret_cast<float*>(s_blk + 2 * 64);
     float* s_shift = s_scale + COUT;
-    float* s_stg = s_shift + COUT;                                                 // [128][STG_LD] epilogue staging
-    uint64_t* full = reinterpret_cast<uint64_t*>(s_stg + SB_ROWS * Cfg::STG_LD);
+    uint64_t* full = reinterpret_cast<uint64_t*>(s_shift + COUT);
     uint64_t* empty = full + S;
-    uint64_t* landed = empty + S;                  // producers' cp.async data + weight TMA of a stage have landed (generic proxy)
+    uint64_t* landed = empty + S;                  // producers' cp.async data of a stage have landed (generic proxy)
     uint64_t* nbr_full = landed + S;
     uint64_t* nbr_empty = nbr_full + 2;
+    uint64_t* wfull = nbr_empty + 2;               // weight slot loaded (TMA bytes)
+    uint64_t* wempty = wfull + WS;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int ktot = K * CIN_PAD;
@@ -114,10 +133,11 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
 
     if (threadIdx.x == 0) {
         tc::prefetch_tmap(&tmW);
-        for (int s = 0; s < S; ++s) { tc::mbar_init(landed + s, 32 * Cfg::NPROD + 1); tc::mbar_init(full + s, 1); tc::mbar_init(empty + s, Cfg::CONSUMERS); }
+        for (int s = 0; s < S; ++s) { tc::mbar_init(landed + s, 32 * Cfg::NPROD); tc::mbar_init(full + s, 1); tc::mbar_init(empty + s, Cfg::CONSUMERS); }
+        for (int s = 0; s < WS; ++s) { tc::mbar_init(wfull + s, 1); tc::mbar_init(wempty + s, Cfg::CONSUMERS); }
         for (int b = 0; b < 2; ++b) {
             tc::mbar_init(nbr_full + b, 1);
-            tc::mbar_init(nbr_empty + b, Cfg::NPROD + 1 + Cfg::CONSUMERS);
+            tc::mbar_init(nbr_empty + b, Cfg::NPROD + 1 + Cfg::CONSUMERS + 1);    // producers, fence warp, consumers, weight warp
         }
         tc::fence_barrier_init();
     }
@@ -221,10 +241,6 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
                 const int kb = s_blk[b * 64 + i];
                 mbar_wait_bounded(empty + my_s, ((gi / S) & 1) ^ 1);
                 const uint32_t sa_u = smem_u + (uint32_t)(my_s * Cfg::STAGE_BYTES);
-                if (pw == 0 && lane == 0) {
-                    tc::mbar_arrive_expect_tx(landed + my_s, Cfg::W_BYTES);
-                    tc::tma_load_2d(smem + my_s * Cfg::STAGE_BYTES + PLANES * SB_A_BYTES, &tmW, landed + my_s, kb * 64, 0);
-                }
                 const int e = kb * 64 + j * 8;                       // position of this lane's chunk in the (offset, channel) dimension
                 const int k = e / CIN_PAD, c = e % CIN_PAD;
                 const bool k_ok = k < K;
@@ -271,29 +287,55 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
                 }
             }
         }
-    } else {
-        // ================= consumers: warpgroup cg accumulates rows [64cg, 64cg+64) of each tile; warps 0-3 run the epilogue ======
-        const int cg = warp >> 2;
-        const uint32_t smem_u = tc::smem_u32(smem);
-        constexpr int CW = Cfg::CW;
+    } else if (warp == Cfg::WARP_W) {
+        // ================= weight warp: TMA of each live block's weight slice into the weight ring ===============================
         int g = 0;
         for (int t = 0;; ++t) {
             const int b = t & 1;
             mbar_wait_bounded(nbr_full + b, (t >> 1) & 1);
             if (s_blk[b * 64 + 62] < 0) break;
             const int nb = s_blk[b * 64 + 63];
-            const int r = warp < 4 ? s_nbr[b * SB_NPLANES * SB_ROWS + K * SB_ROWS + threadIdx.x] : -1;
+            // the block list (<= 54 entries) in registers, so the table buffer is released before the weight loads wait on the ring
+            const int kb_lo = s_blk[b * 64 + lane], kb_hi = s_blk[b * 64 + 32 + (lane < 30 ? lane : 0)];
+            __syncwarp();
+            if (lane == 0) tc::mbar_arrive(nbr_empty + b);
+            for (int i = 0; i < nb; ++i, ++g) {
+                const int kb = __shfl_sync(0xffffffffu, i < 32 ? kb_lo : kb_hi, i & 31);
+                if (lane == 0) {
+                    const int ws = g % WS;
+                    mbar_wait_bounded(wempty + ws, ((g / WS) & 1) ^ 1);
+                    tc::mbar_arrive_expect_tx(wfull + ws, Cfg::W_BYTES);
+                    tc::tma_load_2d(s_w + ws * Cfg::W_BYTES, &tmW, wfull + ws, kb * 64, 0);
+                }
+                __syncwarp();
+            }
+        }
+    } else {
+        // ================= consumers: warpgroup cg accumulates rows [64cg, 64cg+64) of each tile and runs their epilogue ========
+        const int cg = warp >> 2;
+        const uint32_t smem_u = tc::smem_u32(smem);
+        const int frow = cg * 64 + 16 * (warp & 3) + (lane >> 2);     // tile rows frow, frow + 8 of this thread's fragment
+        const int fcol = 2 * (lane & 3);                               // its columns 8j + fcol, 8j + fcol + 1
+        int g = 0;
+        for (int t = 0;; ++t) {
+            const int b = t & 1;
+            mbar_wait_bounded(nbr_full + b, (t >> 1) & 1);
+            if (s_blk[b * 64 + 62] < 0) break;
+            const int nb = s_blk[b * 64 + 63];
+            const int* rows_b = s_nbr + b * SB_NPLANES * SB_ROWS + K * SB_ROWS;
+            const int orow[2] = {rows_b[frow], rows_b[frow + 8]};
             __syncwarp();
             if (lane == 0) tc::mbar_arrive(nbr_empty + b);
             float acc[COUT / 2];
 #pragma unroll
             for (int i = 0; i < COUT / 2; ++i) acc[i] = 0.f;
             for (int i = 0; i < nb; ++i, ++g) {
-                const int s = g % S;
+                const int s = g % S, ws = g % WS;
+                mbar_wait_bounded(wfull + ws, (g / WS) & 1);
                 mbar_wait_bounded(full + s, (g / S) & 1);
                 // (the generic->async proxy fence is executed by the fence warp before it arrives)
                 const uint32_t sa = smem_u + (uint32_t)(s * Cfg::STAGE_BYTES) + cg * 64 * 128;
-                const uint32_t sw = smem_u + (uint32_t)(s * Cfg::STAGE_BYTES + PLANES * SB_A_BYTES);
+                const uint32_t sw = tc::smem_u32(s_w + ws * Cfg::W_BYTES);
                 const uint64_t a0 = tc::smem_desc_sw128(sa), w0 = tc::smem_desc_sw128(sw);
                 tc::wgmma_fence();
 #pragma unroll
@@ -309,54 +351,34 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
                 tc::wgmma_commit();
                 tc::wgmma_wait_one();                   // this step's MMAs stay in flight; the previous step's stage is free
                 __syncwarp();
-                if (lane == 0 && i > 0) tc::mbar_arrive(empty + (g - 1) % S);
+                if (lane == 0 && i > 0) { tc::mbar_arrive(empty + (g - 1) % S); tc::mbar_arrive(wempty + (g - 1) % WS); }
             }
             tc::wgmma_wait_all();
             __syncwarp();
-            if (lane == 0 && nb > 0) tc::mbar_arrive(empty + (g - 1) % S);
+            if (lane == 0 && nb > 0) { tc::mbar_arrive(empty + (g - 1) % S); tc::mbar_arrive(wempty + (g - 1) % WS); }
+            // epilogue straight from the accumulator fragment (tc.cuh: d[4j + 2r + c] = D[frow + 8r][8j + fcol + c]): scale/shift
+            // (+ residual plane 0, then plane 1) -> ReLU -> plane split, two adjacent columns (one 32-bit word per plane) at a time
 #pragma unroll
-            for (int c0 = 0; c0 < COUT; c0 += CW) {
-                tc::named_sync(1, 32 * Cfg::CONSUMERS);             // the previous pass has read the staging tile
-                tc::acc_cols_to_smem<COUT>(acc, s_stg, Cfg::STG_LD, cg * 64, c0, CW);
-                tc::named_sync(1, 32 * Cfg::CONSUMERS);
-                if (warp < 4 && r >= 0) {
-                    float o[CW];
+            for (int r = 0; r < 2; ++r) {
+                if (orow[r] < 0) continue;
+                const uint32_t* rp = residual ? reinterpret_cast<const uint32_t*>(residual + (size_t)orow[r] * (PLANES * COUT) + fcol) : nullptr;
+                uint32_t* op = reinterpret_cast<uint32_t*>(out + (size_t)orow[r] * (PLANES * COUT) + fcol);
 #pragma unroll
-                    for (int jj = 0; jj < CW; ++jj) {
-                        const float a = nb == 0 ? 0.f : s_stg[threadIdx.x * Cfg::STG_LD + jj];
-                        o[jj] = fmaf(a, s_scale[c0 + jj], s_shift[c0 + jj]);
-                    }
-                    if (residual) {
-                        const uint4* rp = reinterpret_cast<const uint4*>(residual + (size_t)r * (PLANES * COUT) + c0);
+                for (int j = 0; j < COUT / 8; ++j) {
+                    const int c = 8 * j + fcol;
+                    float o0 = fmaf(acc[4 * j + 2 * r], s_scale[c], s_shift[c]);
+                    float o1 = fmaf(acc[4 * j + 2 * r + 1], s_scale[c + 1], s_shift[c + 1]);
+                    if (rp) {
 #pragma unroll
-                        for (int p = 0; p < PLANES; ++p)
-#pragma unroll
-                            for (int v = 0; v < CW / 8; ++v) {
-                                const uint4 u = __ldg(rp + p * (COUT / 8) + v);
-                                o[8 * v + 0] += bf16_lo(u.x); o[8 * v + 1] += bf16_hi(u.x); o[8 * v + 2] += bf16_lo(u.y); o[8 * v + 3] += bf16_hi(u.y);
-                                o[8 * v + 4] += bf16_lo(u.z); o[8 * v + 5] += bf16_hi(u.z); o[8 * v + 6] += bf16_lo(u.w); o[8 * v + 7] += bf16_hi(u.w);
-                            }
-                    }
-                    if (relu) {
-#pragma unroll
-                        for (int jj = 0; jj < CW; ++jj) o[jj] = fmaxf(o[jj], 0.f);
-                    }
-                    uint4* op = reinterpret_cast<uint4*>(out + (size_t)r * (PLANES * COUT) + c0);
-#pragma unroll
-                    for (int v = 0; v < CW / 8; ++v) {
-                        uint4 h;
-                        h.x = pack_bf16(o[8 * v + 0], o[8 * v + 1]); h.y = pack_bf16(o[8 * v + 2], o[8 * v + 3]);
-                        h.z = pack_bf16(o[8 * v + 4], o[8 * v + 5]); h.w = pack_bf16(o[8 * v + 6], o[8 * v + 7]);
-                        op[v] = h;
-                        if (PLANES == 2) {
-                            uint4 l;
-                            l.x = pack_bf16(o[8 * v + 0] - bf16_lo(h.x), o[8 * v + 1] - bf16_hi(h.x));
-                            l.y = pack_bf16(o[8 * v + 2] - bf16_lo(h.y), o[8 * v + 3] - bf16_hi(h.y));
-                            l.z = pack_bf16(o[8 * v + 4] - bf16_lo(h.z), o[8 * v + 5] - bf16_hi(h.z));
-                            l.w = pack_bf16(o[8 * v + 6] - bf16_lo(h.w), o[8 * v + 7] - bf16_hi(h.w));
-                            op[COUT / 8 + v] = l;
+                        for (int p = 0; p < PLANES; ++p) {
+                            const uint32_t u = __ldg(rp + (p * COUT + 8 * j) / 2);
+                            o0 += bf16_lo(u); o1 += bf16_hi(u);
                         }
                     }
+                    if (relu) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); }
+                    const uint32_t h = pack_bf16(o0, o1);
+                    op[4 * j] = h;
+                    if (PLANES == 2) op[(COUT + 8 * j) / 2] = pack_bf16(o0 - bf16_lo(h), o1 - bf16_hi(h));
                 }
             }
         }
