@@ -372,6 +372,23 @@ int dz_refine_score(const double* in_boxes, const double* out_boxes, const float
 int dz_confidence_score(const float* conf_score, const float* pred_score, const float* iou, const int32_t* box_num, int B, int L,
                         int32_t* rec, dz_stream_t stream);
 
+/* ---- detection AP / APH records (csrc/det_eval.cu) --------------------------------------------------------------------------- */
+/* The per-cutoff counts behind Waymo AP and APH as DetZero's evaluator reports them (evaluator/detzero_eval.py ->
+ * WaymoDetectionMetricsEstimator), restated without the Waymo metric library (the definition is in csrc/det_eval.cu).
+ * pred (NF, R, 9) f32 [x, y, z, dx, dy, dz, heading, score, Waymo type] with pred_cnt (NF) rows per frame; gt_box (NF, G, 7) f32,
+ * gt_type (NF, G) Waymo type, gt_level (NF, G) 1 or 2, gt_cnt (NF).  Waymo types are 1 vehicle, 2 pedestrian, 3 sign, 4 cyclist;
+ * a row of any other type is ignored.  box_type 0: 3-D IoU (boxes_iou3d_gpu), 1: BEV IoU.  breakdown_mask bit 0: OBJECT_TYPE
+ * (records shards 0..3, type - 1), bit 1: RANGE (shards 4..15, 4 + 3 (type - 1) + range, range [0, 30) / [30, 50) / [50, +inf)).
+ * records (16, 2, 101, 4) int64 [shard][LEVEL_1, LEVEL_2][cutoff k: score >= float32(k * 0.01), the last 1.0][TP, FP, FN, TPH
+ * (2^-32 units)] are ADDED to (the caller zeroes them once; records of disjoint frame sets add up); shards outside the mask are not
+ * written.  *overflow (zeroed by the caller) gets bit 1 when a frame has more than max_pairs valid pairs, bit 2 when an assignment
+ * component exceeds the scratch; the records are then invalid.  Persistent blocks, integer atomics (the records are identical run to
+ * run), no host synchronisation. */
+size_t dz_det_eval_ws_bytes(int NF, int R, int G, int max_pairs);
+int dz_det_eval(const float* pred, const int* pred_cnt, const float* gt_box, const int* gt_type, const int* gt_level, const int* gt_cnt,
+                int NF, int R, int G, int box_type, int breakdown_mask, int max_pairs, long long* records, int* overflow, void* ws,
+                size_t ws_bytes, dz_stream_t stream);
+
 /* ---- test-time augmentation (CenterPoint TTA) ------------------------------------------------------------- */
 /* A view is 4 host floats [op, p1, p2, p3]: DZ_TTA_ORIGINAL; DZ_TTA_FLIP_X (y = -y); DZ_TTA_FLIP_Y (x = -x); DZ_TTA_FLIP_XY;
  * DZ_TTA_ROT with p1, p2 = cos, sin of the float32 angle (float32 torch on the CPU, as the reference computes them) and, for
