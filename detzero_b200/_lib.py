@@ -83,6 +83,9 @@ _SIGS = {
     'dz_confidence_score': (ci, [vp, vp, vp, vp, ci, ci, vp, vp]),
     'dz_det_eval_ws_bytes': (sz, [ci, ci, ci, ci]),
     'dz_det_eval': (ci, [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, vp, vp, vp, sz, vp]),
+    'dz_track_eval_ws_bytes': (sz, [ci, ci, ci, ci, ci]),
+    'dz_track_eval': (ci, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, vp, vp, vp, sz, vp]),
+    'dz_track_entry_lidar': (ci, [vp, vp, vp, vp, ci, ci, ci, vp, vp]),
     'dz_tta_expand':(ci, [vp, ci, vp, ci, vp, ci, vp, vp]),
     'dz_tta_unaugment': (ci, [vp, vp, ci, ci, vp, ci, vp, vp]),
     'dz_wbf_3d_ws_bytes': (sz, [ci, ci, ci, ci]),

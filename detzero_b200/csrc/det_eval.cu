@@ -29,6 +29,7 @@
 #include "common.cuh"
 #include "boxgeom.cuh"
 #include "assign.cuh"
+#include "eval_common.cuh"
 
 namespace {
 
@@ -93,11 +94,6 @@ __device__ Ws carve(char* p, int R, int G, int P) {
     w.gbits = (unsigned*)take((size_t)G * WORDS * 4); w.pbits = (unsigned*)take((size_t)R * WORDS * 4);
     w.scr = (double*)take((size_t)SCR_CAP * 8);
     return w;
-}
-
-__device__ __forceinline__ int range_bin(float x, float y) {
-    const float r = __fsqrt_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)));
-    return r < 30.f ? 0 : (r < 50.f ? 1 : 2);
 }
 
 __device__ __forceinline__ int valid_type(int t) { return t >= 1 && t <= 4; }
@@ -225,7 +221,7 @@ k_det_eval(EvIn in, long long* records, int* overflow, char* ws_base, size_t blo
     const int R = in.R, G = in.G, P = in.P;
     Ws w = carve(ws_base + (size_t)blockIdx.x * block_bytes, R, G, P);
     for (int i = threadIdx.x; i < NSHARD * 2 * 4 * NKD; i += NT) w.diff[i] = 0ull;
-    for (int k = threadIdx.x; k < NK; k += NT) sh.cut[k] = k < 100 ? __double2float_rn(__dmul_rn((double)k, 0.01)) : 1.f;
+    for (int k = threadIdx.x; k < NK; k += NT) sh.cut[k] = score_cutoff(k);
     if (threadIdx.x == 0) sh.overflow = 0;
     __syncthreads();
     for (int f = blockIdx.x; f < in.NF; f += gridDim.x) {

@@ -4,8 +4,7 @@
 //
 // One persistent block per sequence:
 //   entries     every track entry's world box goes back to the lidar frame as tracklets_to_frames / transform_boxes3d(inverse=True)
-//               do it: the box cast to float32, the inverse pose rounded to float32 (get_inverse_transform_mat), the centre
-//               product in float64 rounded to float32, the heading through the float32 yaw_filter.  Entries are grouped by frame.
+//               do it (entry_to_lidar of eval_common.cuh).  Entries are grouped by frame.
 //   objects     per object (a per-sequence index of the rows whose class is scored): trajectory length, first / last row, whether
 //               a box is L2 (difficulty 2, or 0 with num_points_in_gt <= 5), and its row in every frame.
 //   frames      in ascending order, every (ground-truth row, track entry) pair of the frame of the same class that is not a far
@@ -29,6 +28,7 @@
 #include "common.cuh"
 #include "boxgeom.cuh"
 #include "assign.cuh"
+#include "eval_common.cuh"
 
 namespace {
 
@@ -54,14 +54,6 @@ struct Ws {
     int *olen, *ofirst, *olast, *oany2, *orow, *mr, *mc;
     double* scr;
 };
-
-__device__ __forceinline__ float yawf(float y) {                      // transform_utils.yaw_filter, ndarray branch, float32
-    const float pi2 = 6.283185307179586f, pi = 3.141592653589793f;
-    if (fabsf(y) >= pi2) y = y - floorf(y / pi2) * pi2;
-    if (y > pi) y -= pi2;
-    if (y <= -pi) y += pi2;
-    return y;
-}
 
 __device__ __forceinline__ unsigned pair_hash(int o, int k) { return (unsigned)o * 0x9E3779B1u ^ (unsigned)k * 0x85EBCA77u; }
 
@@ -198,24 +190,7 @@ k_track_gt(GtIn gt, TkIn tk, GtPar pr, GtOut out, char* ws_base, size_t seq_byte
         const double* b = ebox + (size_t)e * 9;
         float* l = w.elid + (size_t)e * 7;
         if (f < 0 || f >= Fs) continue;
-        const double* Pm = poses + (size_t)f * 16;
-        float inv[12];
-        for (int r = 0; r < 3; ++r) {
-            for (int c = 0; c < 3; ++c) inv[r * 4 + c] = (float)Pm[c * 4 + r];
-            double t = __dmul_rn(Pm[r], Pm[3]);
-            t = __dadd_rn(t, __dmul_rn(Pm[4 + r], Pm[7]));
-            t = __dadd_rn(t, __dmul_rn(Pm[8 + r], Pm[11]));
-            inv[r * 4 + 3] = (float)(-t);
-        }
-        const float x = (float)b[0], y = (float)b[1], z = (float)b[2];
-        for (int r = 0; r < 3; ++r) {
-            double c = __dmul_rn((double)x, (double)inv[r * 4]);
-            c = __dadd_rn(c, __dmul_rn((double)y, (double)inv[r * 4 + 1]));
-            c = __dadd_rn(c, __dmul_rn((double)z, (double)inv[r * 4 + 2]));
-            l[r] = (float)__dadd_rn(c, (double)inv[r * 4 + 3]);
-        }
-        l[3] = (float)b[3]; l[4] = (float)b[4]; l[5] = (float)b[5];
-        l[6] = yawf(__fadd_rn((float)b[6], (float)atan2((double)inv[4], (double)inv[0])));
+        entry_to_lidar(b, poses + (size_t)f * 16, l);
         atomicAdd(&w.fcnt[f], 1);
     }
     __syncthreads();

@@ -16,7 +16,16 @@ Compatibility with the official Waymo metric is not verified.  Points where the 
 by the reference: a RANGE shard matches its ground truth against predictions of every range and counts an FP in the prediction's
 own range only when it is matched in none of the type's range matchings; IoU is DetZero's boxes_iou3d_gpu (3d) or its rotated BEV
 IoU (bev), not Waymo's; ties in the matching follow the first minimum of the Hungarian's column scan; no interpolation between
-distant recall points."""
+distant recall points.
+
+Tracking mode (evaluator/detzero_eval.py --tracking -> WaymoTrackingMetricsEstimator, evaluator/waymo_eval_tracking.py): MOTA, MOTP,
+MISS, MISMATCH and FP per object type, level and range on the device (csrc/track_eval.cu, which states the CLEAR-MOT definition in
+full): ``tracking_metrics`` on padded per-sequence device tables, ``mot_dict`` on the host, ``WaymoTrackingMetricsEstimator`` on
+the reference's frame dicts, ``evaluate_tracks`` on track.track_sequences results and ``evaluate_offboard_tracking`` on
+offboard.refine_sequence results.  Per (sequence, type, cutoff) a chain keeps last frame's still-valid pairs, matches the rest by
+the maximum IoU sum, and counts a mismatch when an object's last matched id changes; RANGE splits the counts of that one chain by
+the ground-truth box's range (the prediction's for an FP), unlike the detection RANGE above.  Compatibility with the official Waymo
+tracking metric is not verified."""
 import numpy as np
 import torch
 
@@ -270,3 +279,329 @@ def evaluate_offboard(results, gt, class_name=CLASS_NAMES, config_type=('object'
     rec, ap = detection_metrics(pred.reshape(S * F, R, 9), pred_cnt.reshape(-1), gbox.reshape(S * F, G, 7), gtype.reshape(S * F, G),
                                 level.reshape(S * F, G), gt.counts.reshape(-1), box_type, breakdowns, max_pairs, frame_chunk)
     return (ap, rec) if return_records else ap
+
+
+# ------------------------------------------------------------------------------------------------------------------- tracking
+#: WAYMO_CLASSES of the reference's tracking evaluator (waymo_eval_tracking.py): type 3 is 'Sign'
+TRACKING_WAYMO_CLASSES = ['unknown', 'Vehicle', 'Pedestrian', 'Sign', 'Cyclist']
+MOT_KEYS = ('MOTA', 'MOTP', 'MISS', 'MISMATCH', 'FP')
+
+
+def _breakdowns(config_type):
+    for c in config_type:
+        if c not in ('object', 'range'):
+            raise ValueError('unknown config type %r (supported: object, range)' % (c,))
+    return tuple(b for b in ('object', 'range') if b in config_type)
+
+
+def mot_dict(records, breakdowns=('object',)):
+    """{'OBJECT_TYPE_TYPE_VEHICLE_LEVEL_1/MOTA': [v], ... /MOTP, /MISS, /MISMATCH, /FP, 'RANGE_TYPE_CYCLIST_[50, +inf)_LEVEL_2/FP':
+    [v], ...} from the tracking records (16, 2, 101, 5), per shard and level at the cutoff with the largest MOTA (the lowest cutoff
+    on a tie): MOTA = 1 - (misses + mismatches + FP) / num_gt, MOTP = cost / matches (0 without matches), MISS, MISMATCH, FP = each
+    count / num_gt, num_gt = matches + misses; a shard with num_gt = 0 gets 0 everywhere.  SIGN keys are always present."""
+    rec = np.asarray(records)
+    shards = []
+    if 'object' in breakdowns:
+        shards += [(t, 'OBJECT_TYPE_TYPE_%s' % TYPE_NAMES[t]) for t in range(4)]
+    if 'range' in breakdowns:
+        shards += [(4 + 3 * t + r, 'RANGE_TYPE_%s_%s' % (TYPE_NAMES[t], RANGE_NAMES[r])) for t in range(4) for r in range(3)]
+    out = {}
+    for s, name in shards:
+        for lvl in (0, 1):
+            m, miss, fp, mm, cost = (rec[s, lvl, :, i].astype(np.float64) for i in range(5))
+            n = m + miss
+            if n[0] == 0:
+                vals = [0.0] * 5
+            else:
+                mota = 1.0 - (miss + mm + fp) / n
+                k = int(np.argmax(mota))
+                vals = [float(mota[k]), float(cost[k] / _FIXED / m[k]) if m[k] else 0.0, float(miss[k] / n[k]), float(mm[k] / n[k]),
+                        float(fp[k] / n[k])]
+            for key, v in zip(MOT_KEYS, vals):
+                out['%s_LEVEL_%d/%s' % (name, lvl + 1, key)] = [v]
+    return out
+
+
+def tracking_metrics(pred, pred_id, pred_cnt, gt_box, gt_obj, gt_type, gt_level, gt_cnt, num_frames=None, n_obj=None,
+                     breakdowns=('object',), max_pairs=1 << 14):
+    """Tracking records and MOTA / MOTP dict of S sequences on the device (csrc/track_eval.cu).  pred (S, F, R, 9) f32 CUDA [x, y, z,
+    dx, dy, dz, heading, score, Waymo type], pred_id (S, F, R) int32 identity per sequence, pred_cnt (S, F) rows per frame; gt_box
+    (S, F, G, 7) f32, gt_obj (S, F, G) per-sequence object index, gt_type (S, F, G) Waymo type, gt_level (S, F, G) 1 or 2, gt_cnt
+    (S, F); num_frames (S) frames per sequence (default F), n_obj (S) objects per sequence (default 1 + the largest index).  Rows of a
+    type outside 1..4 are ignored.  breakdowns from 'object', 'range'.  max_pairs: capacity of valid pairs of one type per frame.
+    Raises ValueError when two rows of a frame share an id or an object index is out of range, RuntimeError past a capacity.
+    Returns (records (16, 2, 101, 5) int64 numpy [shard][level][cutoff][matches, misses, FP, mismatches, cost in 2^-32 units],
+    mot_dict); one device-to-host copy."""
+    for b in breakdowns:
+        if b not in ('object', 'range'):
+            raise ValueError('unknown breakdown %r' % (b,))
+    assert pred.is_cuda and pred.dtype == torch.float32 and pred.dim() == 4 and pred.shape[3] == 9, (pred.shape, pred.dtype)
+    assert gt_box.is_cuda and gt_box.dtype == torch.float32 and gt_box.dim() == 4 and gt_box.shape[3] == 7, (gt_box.shape, gt_box.dtype)
+    S, F, dev = pred.shape[0], pred.shape[1], pred.device
+    if tuple(gt_box.shape[:2]) != (S, F):
+        raise ValueError('predictions of %d sequences x %d frames against ground truth of %d x %d' % (S, F, *gt_box.shape[:2]))
+    i32 = lambda t: torch.as_tensor(t).to(device=dev, dtype=torch.int32).contiguous()
+    pred_id, pred_cnt, gt_obj, gt_type, gt_level, gt_cnt = (i32(t) for t in (pred_id, pred_cnt, gt_obj, gt_type, gt_level, gt_cnt))
+    pred_cnt, gt_cnt = pred_cnt.reshape(S, F), gt_cnt.reshape(S, F)
+    nf = torch.full((S,), F, dtype=torch.int32, device=dev) if num_frames is None else i32(num_frames).reshape(S)
+    if n_obj is None:
+        n_obj = (gt_obj.reshape(S, -1).amax(1) + 1).clamp(min=0) if gt_obj.numel() else torch.zeros(S, dtype=torch.int32, device=dev)
+    n_obj = i32(n_obj).reshape(S)
+    if pred.shape[2] == 0:
+        pred, pred_id, pred_cnt = (torch.zeros((S, F, 1, 9), dtype=torch.float32, device=dev), torch.zeros((S, F, 1), **_I32(dev)),
+                                   torch.zeros_like(pred_cnt))
+    if gt_box.shape[2] == 0:
+        gt_box, gt_cnt = torch.zeros((S, F, 1, 7), dtype=torch.float32, device=dev), torch.zeros_like(gt_cnt)
+        gt_obj = gt_type = gt_level = torch.zeros((S, F, 1), **_I32(dev))
+    pred, gt_box = pred.contiguous(), gt_box.contiguous()
+    R, G = pred.shape[2], gt_box.shape[2]
+    for name, t in (('pred_id', pred_id), ('gt_obj', gt_obj), ('gt_type', gt_type), ('gt_level', gt_level)):
+        if tuple(t.shape) != (S, F, R if name == 'pred_id' else G):
+            raise ValueError('%s must be (S, F, %s)' % (name, 'R' if name == 'pred_id' else 'G'))
+    O = max(int(n_obj.max()) if S else 0, 1)
+    records = torch.zeros((16, 2, NUM_CUTOFFS, 5), dtype=torch.int64, device=dev)
+    flags = torch.zeros((1,), dtype=torch.int32, device=dev)
+    mask = sum(1 << i for i, b in enumerate(('object', 'range')) if b in breakdowns)
+    if S and mask:
+        ws = ops.workspace(lib().dz_track_eval_ws_bytes(S, R, G, O, int(max_pairs)), dev, 'track_eval')
+        check(lib().dz_track_eval(ops._p(pred), ops._p(pred_id), ops._p(pred_cnt), ops._p(gt_box), ops._p(gt_obj), ops._p(gt_type),
+                                  ops._p(gt_level), ops._p(gt_cnt), ops._p(nf), ops._p(n_obj), S, F, R, G, O, mask, int(max_pairs),
+                                  ops._p(records), ops._p(flags), ops._p(ws), ws.numel(), ops._stream()), 'track_eval')
+        ops._count(1)
+    out = torch.cat([records.reshape(-1), flags.long()]).cpu().numpy()
+    rec, fl = out[:-1].reshape(16, 2, NUM_CUTOFFS, 5), int(out[-1])
+    if fl & 12:
+        what = [n for b, n in ((4, 'two rows of one frame share an id'), (8, 'a ground-truth object index is outside [0, n_obj)'))
+                if fl & b]
+        raise ValueError('track_eval: %s' % '; '.join(what))
+    if fl & 3:
+        what = [n for b, n in ((1, 'valid pairs per frame (max_pairs=%d)' % max_pairs), (2, 'the assignment scratch')) if fl & b]
+        raise RuntimeError('track_eval: a frame exceeded the capacity of %s' % ', '.join(what))
+    return rec, mot_dict(rec, breakdowns)
+
+
+def _I32(dev):
+    return dict(dtype=torch.int32, device=dev)
+
+
+def tracking_tables(prediction_infos, gt_infos, class_name, fake_gt_infos=True):
+    """The padded host tables of tracking_metrics from the reference's frame dicts, by generate_waymo_type_results:
+    prediction_infos per frame {'sequence_name', 'obj_ids', 'boxes_lidar', 'score', 'name'}, gt_infos per frame {'sequence_name',
+    'annos': {'name', 'obj_ids', 'difficulty', 'num_points_in_gt', 'gt_boxes_lidar'}}, frame i of both lists the same frame.
+    Ground-truth rows kept when their name is in class_name and num_points_in_gt > 0, difficulty 0 -> 1 (more than 5 points) or 2,
+    the fake-lidar conversion with fake_gt_infos, headings through limit_period(h, 0.5, 2 pi) on the concatenation of every frame's
+    rows, scores through a sigmoid when their maximum exceeds 1.  Names map through TRACKING_WAYMO_CLASSES (an unknown name raises
+    ValueError, as list.index does).  Prediction ids are sequence_name + '-' + str(obj_id), numbered per sequence (of the ground
+    truth's sequence_name) in order of first appearance, as are ground-truth obj_ids.  A sequence's frames keep their list order,
+    also when sequences interleave.  A prediction frame whose obj_ids and boxes_lidar differ in length raises ValueError (frames
+    with dropped detections, which have no identity).  The inputs are not modified.  Returns a dict of numpy arrays pred, pred_id,
+    pred_cnt, gt_box, gt_obj, gt_type, gt_level, gt_cnt, num_frames, n_obj, and 'sequences' (names in order of first frame)."""
+    if len(prediction_infos) != len(gt_infos):
+        raise ValueError('%d prediction frames vs %d ground-truth frames' % (len(prediction_infos), len(gt_infos)))
+    NF = len(gt_infos)
+    seq_names = list(dict.fromkeys(info['sequence_name'] for info in gt_infos))
+    sidx = {n: i for i, n in enumerate(seq_names)}
+    S = len(seq_names)
+    fseq = np.array([sidx[info['sequence_name']] for info in gt_infos], np.int64)
+    nfr = np.bincount(fseq, minlength=S).astype(np.int32)
+    fpos = np.zeros(NF, np.int64)
+    for s in range(S):
+        fpos[fseq == s] = np.arange(nfr[s])
+    pf, pb, ps, pt, pk, gf, gb, gt, gd, gk = [], [], [], [], [], [], [], [], [], []
+    for i, (pinfo, info) in enumerate(zip(prediction_infos, gt_infos)):
+        n = len(pinfo['boxes_lidar'])
+        ids = pinfo['obj_ids'] if n or 'obj_ids' in pinfo else []
+        if len(ids) != n:
+            raise ValueError('prediction frame %d has %d obj_ids for %d boxes_lidar (dropped detections have no identity)'
+                             % (i, len(ids), n))
+        pb.append(np.asarray(pinfo['boxes_lidar'])[:, :7].reshape(-1, 7))
+        ps.append(np.asarray(pinfo['score']).reshape(-1))
+        pt += [TRACKING_WAYMO_CLASSES.index(x) for x in pinfo['name']]
+        pk += [(fseq[i], pinfo['sequence_name'] + '-' + str(x)) for x in ids]
+        pf.append(np.full(n, i))
+        a = info['annos']
+        names, npts = np.asarray(a['name']), np.asarray(a['num_points_in_gt'])
+        diff = np.array(a['difficulty'], copy=True)
+        zero = diff == 0
+        diff[(npts > 5) & zero] = 1
+        diff[(npts <= 5) & zero] = 2
+        keep = np.array([x in class_name for x in names], dtype=np.bool_) & (npts > 0)
+        boxes = _fakelidar_to_lidar(a['gt_boxes_lidar']) if fake_gt_infos else np.asarray(a['gt_boxes_lidar'])
+        gb.append(boxes[keep][:, :7])
+        gt += [TRACKING_WAYMO_CLASSES.index(x) for x in names[keep]]
+        gd.append(diff[keep])
+        gk += [(fseq[i], x) for x in np.asarray(a['obj_ids'])[keep]]
+        gf.append(np.full(int(keep.sum()), i))
+    cat = lambda a, shape: np.concatenate(a, 0) if a else np.zeros(shape)
+    pf, pb, ps, pt = cat(pf, (0,)).astype(np.int64), cat(pb, (0, 7)), cat(ps, (0,)).reshape(-1), np.array(pt, np.int64)
+    gf, gb, gt, gd = cat(gf, (0,)).astype(np.int64), cat(gb, (0, 7)), np.array(gt, np.int64), cat(gd, (0,))
+    pb[:, -1] = _limit_period(pb[:, -1], offset=0.5, period=np.pi * 2)
+    gb[:, -1] = _limit_period(gb[:, -1], offset=0.5, period=np.pi * 2)
+    if ps.size and ps.max() > 1:
+        ps = 1 / (1 + np.exp(-ps))
+    pidx, gidx = [{} for _ in range(S)], [{} for _ in range(S)]
+    pid = np.array([pidx[s].setdefault(k, len(pidx[s])) for s, k in pk], np.int64)
+    gobj = np.array([gidx[s].setdefault(k, len(gidx[s])) for s, k in gk], np.int64)
+    F = max(int(nfr.max()) if S else 0, 1)
+
+    def pad(frame, cols):
+        cnt = np.bincount(frame, minlength=NF).astype(np.int32)
+        slot = np.arange(len(frame)) - (np.cumsum(cnt) - cnt)[frame]
+        out = np.zeros((S, F, max(int(cnt.max()) if NF else 0, 1), cols.shape[1]), np.float64)
+        out[fseq[frame], fpos[frame], slot] = cols
+        c = np.zeros((S, F), np.int32)
+        c[fseq, fpos] = cnt
+        return out, c
+    p, pred_cnt = pad(pf, np.concatenate([pb.astype(np.float32).astype(np.float64), ps.astype(np.float32)[:, None], pt[:, None],
+                                          pid[:, None]], 1))
+    g, gt_cnt = pad(gf, np.concatenate([gb.astype(np.float32).astype(np.float64), gt[:, None], gd[:, None], gobj[:, None]], 1))
+    return {'pred': np.ascontiguousarray(p[..., :9].astype(np.float32)), 'pred_id': p[..., 9].astype(np.int32), 'pred_cnt': pred_cnt,
+            'gt_box': np.ascontiguousarray(g[..., :7].astype(np.float32)), 'gt_type': g[..., 7].astype(np.int32),
+            'gt_level': g[..., 8].astype(np.int32), 'gt_obj': g[..., 9].astype(np.int32), 'gt_cnt': gt_cnt, 'num_frames': nfr,
+            'n_obj': np.array([len(d) for d in gidx], np.int32), 'sequences': seq_names}
+
+
+class WaymoTrackingMetricsEstimator:
+    """WaymoTrackingMetricsEstimator of waymo_eval_tracking.py with the metric on the device (csrc/track_eval.cu).  After a call,
+    ``records`` holds the records (16, 2, 101, 5) it was computed from."""
+    WAYMO_CLASSES = TRACKING_WAYMO_CLASSES
+
+    def __init__(self, device='cuda', max_pairs=1 << 14):
+        self.device, self.max_pairs = device, max_pairs
+        self.records = None
+
+    def waymo_evaluation(self, prediction_infos, gt_infos, class_name, config_type=['object'], distance_thresh=100,
+                         fake_gt_infos=True):
+        """prediction_infos / gt_infos as tracking_tables takes them (detzero_eval.py --tracking passes the full ground-truth infos);
+        config_type from 'object', 'range'.  distance_thresh is accepted and ignored, as the reference's mask_by_distance keeps every
+        box.  Returns the metric dict {key: [value]}, keys as the reference's (MOTA, MOTP, MISS, MISMATCH, FP)."""
+        breakdowns = _breakdowns(config_type)
+        t = tracking_tables(prediction_infos, gt_infos, class_name, fake_gt_infos)
+        d = {k: torch.from_numpy(np.ascontiguousarray(v)).to(self.device) for k, v in t.items() if k != 'sequences'}
+        self.records, out = tracking_metrics(d['pred'], d['pred_id'], d['pred_cnt'], d['gt_box'], d['gt_obj'], d['gt_type'],
+                                             d['gt_level'], d['gt_cnt'], d['num_frames'], d['n_obj'], breakdowns, self.max_pairs)
+        return out
+
+
+def _gt_tracking_tables(gt, class_name):
+    """ground-truth tables of tracking_metrics from a track.GroundTruth: rows of the classes in class_name with num_points > 0 (others
+    get type 0), difficulty 0 remapped by num_points, headings wrapped; boxes as they are (no fake-lidar conversion)"""
+    for c in class_name:
+        if c not in CLASS_NAMES:
+            raise ValueError('class %r is not one of %r' % (c, CLASS_NAMES))
+    dev = gt.box.device
+    G = gt.box.shape[2]
+    cls_type = torch.tensor([0, 1, 2, 4], dtype=torch.int32, device=dev)
+    sel = torch.zeros(4, dtype=torch.bool, device=dev)
+    sel[[CLASS_NAMES.index(c) + 1 for c in class_name]] = True
+    gvalid = torch.arange(G, device=dev)[None, None, :] < gt.counts[..., None].long()
+    gkeep = gvalid & sel[gt.cls.long()] & (gt.num_points > 0)
+    gtype = torch.where(gkeep, cls_type[gt.cls.long()], torch.zeros_like(gt.cls))
+    level = torch.where(gt.difficulty == 0, torch.where(gt.num_points > 5, 1, 2), gt.difficulty).to(torch.int32)
+    gbox = torch.cat([gt.box[..., :6], _wrap_heading(gt.box[..., 6:7])], -1)
+    return gbox, gt.obj, gtype, level
+
+
+def _pred_finish(pred, pred_cnt, label_type):
+    """scores through a sigmoid when the maximum over the rows exceeds 1 (selected on the device), headings wrapped, the label
+    column replaced by its Waymo type"""
+    R = pred.shape[2]
+    valid = torch.arange(R, device=pred.device)[None, None, :] < pred_cnt[..., None].long()
+    score = pred[..., 7]
+    top = torch.where(valid, score, torch.full_like(score, -np.inf)).max() if pred.numel() else score.new_tensor(0.)
+    score = torch.where(top > 1, 1 / (1 + torch.exp(-score)), score)
+    ptype = torch.where(valid, label_type, torch.zeros_like(score))
+    return torch.cat([pred[..., :6], _wrap_heading(pred[..., 6:7]), score[..., None], ptype[..., None]], -1)
+
+
+def track_tables(track_result, gt, class_name=CLASS_NAMES):
+    """The device tables of tracking_metrics (a dict of its argument names) for a track.TrackResult against a track.GroundTruth of
+    the same sequences and frames.  Every entry of every track is a prediction at its frame, as daemon/combine_output.py
+    convert_frame_format places it: its world box back in the frame's lidar frame (the conversion of csrc/track_gt.cu), the entry's
+    score, the track's class (Waymo types 1, 2, 4) and the track id as its identity.  Ground-truth rows of the classes in class_name
+    with num_points > 0, difficulty 0 remapped by num_points, boxes as they are (no fake-lidar conversion); headings wrapped and
+    scores through a sigmoid when their maximum exceeds 1, as tracking_tables does.  Built with torch ops on the device, no host loop
+    over entries."""
+    gbox, gobj, gtype, level = _gt_tracking_tables(gt, class_name)
+    S, F = gt.box.shape[:2]
+    trk = track_result.trk
+    if trk.shape[0] != S or track_result.poses.shape[1] != F:
+        raise ValueError('tracks of %d sequences / %d frames against ground truth of %d / %d' % (trk.shape[0],
+                                                                                              track_result.poses.shape[1], S, F))
+    dev = gt.box.device
+    E = track_result.ent_box.shape[1]
+    ent_frame = track_result.ent_frame.to(torch.int32).contiguous()
+    nf = track_result.num_frames.to(device=dev, dtype=torch.int32).contiguous()
+    lidar = torch.empty((S, E, 7), dtype=torch.float32, device=dev)
+    check(lib().dz_track_entry_lidar(ops._p(track_result.ent_box.contiguous()), ops._p(ent_frame),
+                                     ops._p(track_result.poses.to(torch.float64).contiguous()), ops._p(nf), S, E, F, ops._p(lidar),
+                                     ops._stream()), 'track_entry_lidar')
+    ops._count(1)
+    nt = torch.as_tensor(np.asarray(track_result.n_tracks, np.int64), device=dev)
+    T = trk.shape[1]
+    tvalid = torch.arange(T, device=dev)[None, :] < nt[:, None]
+    off = torch.where(tvalid, trk[..., 5].long(), torch.full_like(trk[..., 5].long(), 1 << 40))
+    n_ent = torch.where(tvalid, trk[..., 5].long() + trk[..., 3].long(), torch.zeros_like(off)).amax(1) if T else nt
+    e = torch.arange(E, device=dev)
+    k = (torch.searchsorted(off.contiguous(), e[None, :].expand(S, E).contiguous(), right=True) - 1).clamp(0, max(T - 1, 0))
+    ef = ent_frame.long()
+    valid = (e[None, :] < n_ent[:, None]) & (ef >= 0) & (ef < nf.long()[:, None])
+    cell = (torch.arange(S, device=dev)[:, None] * F + ef)[valid]
+    order = torch.sort(cell, stable=True).indices
+    cell = cell[order]
+    cnt = torch.bincount(cell, minlength=S * F)
+    R = max(int(cnt.max()) if cell.numel() else 0, 1)
+    slot = torch.arange(cell.numel(), device=dev) - (torch.cumsum(cnt, 0) - cnt)[cell]
+    label_type = torch.tensor([0, 1, 2, 4], dtype=torch.float32, device=dev)
+    cls = torch.gather(trk[..., 1].long(), 1, k)[valid][order]
+    rows = torch.cat([lidar[valid][order], track_result.ent_score[valid][order].float()[:, None], cls.float()[:, None]], 1)
+    pred = torch.zeros((S * F, R, 9), dtype=torch.float32, device=dev)
+    pred[cell, slot] = rows
+    pred_id = torch.zeros((S * F, R), dtype=torch.int32, device=dev)
+    pred_id[cell, slot] = torch.gather(trk[..., 0], 1, k)[valid][order]
+    pred_cnt = cnt.reshape(S, F).to(torch.int32)
+    pred = pred.reshape(S, F, R, 9)
+    pred = _pred_finish(pred, pred_cnt, label_type[pred[..., 8].long().clamp(0, 3)])
+    return {'pred': pred, 'pred_id': pred_id.reshape(S, F, R), 'pred_cnt': pred_cnt, 'gt_box': gbox, 'gt_obj': gobj, 'gt_type': gtype,
+            'gt_level': level, 'gt_cnt': gt.counts, 'num_frames': gt.num_frames, 'n_obj': gt.n_obj}
+
+
+def evaluate_tracks(track_result, gt, class_name=CLASS_NAMES, config_type=('object',), max_pairs=1 << 14, return_records=False):
+    """MOTA / MOTP of the raw tracker output (track.track_sequences) against ground truth, on the device: track_result a
+    track.TrackResult and gt a track.GroundTruth of the same sequences and frames, tables by track_tables.  Returns the metric dict
+    (and the records with return_records)."""
+    breakdowns = _breakdowns(config_type)
+    rec, out = tracking_metrics(**track_tables(track_result, gt, class_name), breakdowns=breakdowns, max_pairs=max_pairs)
+    return (out, rec) if return_records else out
+
+
+def evaluate_offboard_tracking(results, gt, class_name=CLASS_NAMES, config_type=('object',), max_pairs=1 << 14, return_records=False):
+    """MOTA / MOTP of offboard.refine_sequence's final boxes against ground truth, on the device: results a list of OffboardResult
+    (one per sequence of ``gt``, a track.GroundTruth of the same frames, in order).  The track rows (obj_id >= 0) are the
+    predictions, with the track id as their identity; dropped detections (obj_id -1) have no identity and are left out.
+    Labels 1..3 map to Waymo types 1, 2, 4; ground truth as evaluate_tracks takes it.  Returns the metric dict (and the records
+    with return_records)."""
+    breakdowns = _breakdowns(config_type)
+    gbox, gobj, gtype, level = _gt_tracking_tables(gt, class_name)
+    S, F = gt.box.shape[:2]
+    if len(results) != S:
+        raise ValueError('%d results for %d ground-truth sequences' % (len(results), S))
+    dev = gt.box.device
+    R = max([r.rows.shape[1] for r in results] + [1])
+    pred = torch.zeros((S, F, R, 9), dtype=torch.float32, device=dev)
+    pred_id = torch.zeros((S, F, R), dtype=torch.int32, device=dev)
+    pred_cnt = torch.zeros((S, F), dtype=torch.int32, device=dev)
+    for s, r in enumerate(results):
+        n = r.rows.shape[0]
+        if n != len(gt.frame_ids[s]):
+            raise ValueError('sequence %d: %d result frames against %d ground-truth frames' % (s, n, len(gt.frame_ids[s])))
+        w = r.rows.shape[1]
+        live = torch.arange(w, device=dev)[None, :] < r.count.to(dev).long()[:, None]
+        pred[s, :n, :w] = r.rows
+        pred_id[s, :n, :w] = r.obj_id.to(torch.int32)
+        pred_cnt[s, :n] = ((r.obj_id >= 0) & live).sum(1).to(torch.int32)     # the track rows come first
+    label_type = torch.tensor([0, 1, 2, 4], dtype=torch.float32, device=dev)
+    pred = _pred_finish(pred, pred_cnt, label_type[pred[..., 8].long().clamp(0, 3)])
+    rec, out = tracking_metrics(pred, pred_id, pred_cnt, gbox, gobj, gtype, level, gt.counts, gt.num_frames, gt.n_obj, breakdowns,
+                                max_pairs)
+    return (out, rec) if return_records else out

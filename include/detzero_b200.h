@@ -389,6 +389,29 @@ int dz_det_eval(const float* pred, const int* pred_cnt, const float* gt_box, con
                 int NF, int R, int G, int box_type, int breakdown_mask, int max_pairs, long long* records, int* overflow, void* ws,
                 size_t ws_bytes, dz_stream_t stream);
 
+/* ---- tracking MOTA / MOTP records (csrc/track_eval.cu) ---------------------------------------------------------------------- */
+/* The per-cutoff counts behind Waymo MOTA, MOTP, MISS, MISMATCH and FP as DetZero's evaluator reports them in tracking mode
+ * (evaluator/detzero_eval.py --tracking -> WaymoTrackingMetricsEstimator), restated as CLEAR-MOT without the Waymo metric library
+ * (the definition is in csrc/track_eval.cu).  Per-sequence padded tables: pred (S, F, R, 9) f32 [x, y, z, dx, dy, dz, heading,
+ * score, Waymo type], pred_id (S, F, R) int32 identity per sequence, pred_cnt (S, F); gt_box (S, F, G, 7) f32, gt_obj (S, F, G)
+ * object index in [0, n_obj[s]), gt_type (S, F, G) Waymo type (any other type: the row is ignored), gt_level 1 or 2, gt_cnt (S, F);
+ * num_frames (S) frames per sequence, in order; max_objects >= every n_obj.  breakdown_mask bit 0 OBJECT_TYPE, bit 1 RANGE (shards
+ * as dz_det_eval).  records (16, 2, 101, 5) int64 [shard][LEVEL_1, LEVEL_2][cutoff][matches, misses, FP, mismatches, cost (2^-32
+ * units)] are ADDED to (records of disjoint sequence sets add up).  *flags (zeroed by the caller): bit 1 a frame has more than
+ * max_pairs valid pairs of one type, bit 2 an assignment component exceeds the scratch (the records are then invalid), bit 4 two
+ * rows of a frame share an id, bit 8 an object index is out of range.  One block per (type, sequence), integer atomics (identical
+ * run to run), no host synchronisation. */
+size_t dz_track_eval_ws_bytes(int S, int R, int G, int max_objects, int max_pairs);
+int dz_track_eval(const float* pred, const int* pred_id, const int* pred_cnt, const float* gt_box, const int* gt_obj, const int* gt_type,
+                  const int* gt_level, const int* gt_cnt, const int* num_frames, const int* n_obj, int S, int F, int R, int G,
+                  int max_objects, int breakdown_mask, int max_pairs, long long* records, int* flags, void* ws, size_t ws_bytes,
+                  dz_stream_t stream);
+/* Track entries back to the lidar frame as dz_track_gt does (transform_boxes3d(inverse=True) of convert_frame_format): ent_box
+ * (S, E, 9) f64 world boxes, ent_frame (S, E), poses (S, F, 4, 4) lidar -> world, num_frames (S) -> out (S, E, 7) f32 (zeros for an
+ * entry whose frame is not in [0, num_frames[s])). */
+int dz_track_entry_lidar(const double* ent_box, const int* ent_frame, const double* poses, const int* num_frames, int S, int E, int F,
+                         float* out, dz_stream_t stream);
+
 /* ---- test-time augmentation (CenterPoint TTA) ------------------------------------------------------------- */
 /* A view is 4 host floats [op, p1, p2, p3]: DZ_TTA_ORIGINAL; DZ_TTA_FLIP_X (y = -y); DZ_TTA_FLIP_Y (x = -x); DZ_TTA_FLIP_XY;
  * DZ_TTA_ROT with p1, p2 = cos, sin of the float32 angle (float32 torch on the CPU, as the reference computes them) and, for
