@@ -1,7 +1,14 @@
-// assign.cuh -- the exact rectangular assignment shared by the tracker's association (tracker.cu) and the ground-truth trajectory
-// assignment (track_gt.cu): union-find labels of the valid-edge graph, the Hungarian method with potentials on one thread, and the
-// same method with every column loop spread over the block.  Both solvers use the same arithmetic and take the first minimum of an
-// ascending column scan, so a component gives the same assignment whichever of them solves it.
+// assign.cuh -- the exact assignment by connected components of a valid-edge graph, shared by the tracker's association
+// (tracker.cu), the ground-truth trajectory assignment (track_gt.cu) and the Waymo scorings (det_eval.cu, track_eval.cu):
+//
+//   uf_label / group_edges   min-hooking union-find labels of the edge graph, then the edges grouped by component root
+//   sort_edges               a small component's edges in (row, column) order on one thread
+//   solve_dense(_block)      one component as a dense cost matrix (rows the smaller side) solved by the Hungarian method with
+//                            potentials, on one thread (hungarian) or with every column loop spread over the block (hungarian_block)
+//
+// Both solvers use the same arithmetic and take the first minimum of an ascending column scan, so a cost matrix gives the same
+// assignment whichever of them solves it; the order of the local rows and columns is the caller's and decides exact ties.  Each
+// caller keeps its edge list, its component loops and its cost convention.
 #pragma once
 #include <float.h>
 #include <limits.h>
@@ -13,6 +20,55 @@ __device__ __forceinline__ int uf_find(volatile int* lab, int x) {
     int p = lab[x];
     while (p != x) { x = p; p = lab[x]; }
     return x;
+}
+
+// min-hooking union-find over the edges e < ne joining node row(e) to node col(e): lab (lab[v] = v, preset by the caller) ends
+// with every node's component rooted at its smallest node.  changed: a shared flag of the block.
+template <int NT, class Row, class Col>
+__device__ void uf_label(int* lab, int ne, Row row, Col col, int& changed) {
+    volatile int* vl = lab;
+    while (ne) {
+        if (threadIdx.x == 0) changed = 0;
+        __syncthreads();
+        for (int e = threadIdx.x; e < ne; e += NT) {
+            const int a = uf_find(vl, row(e)), b = uf_find(vl, col(e));
+            if (a != b) { atomicMin(&lab[max(a, b)], min(a, b)); changed = 1; }
+        }
+        __syncthreads();
+        const int ch = changed;
+        __syncthreads();
+        if (!ch) break;
+    }
+}
+
+// the edges (er, ec, ew)[e < ne] grouped by component into (sr, sc, sw), where every root is a row node r < nrows: rcnt (zeroed
+// for the rows by the caller) ends as each root's end offset, so a component is [rcnt[root - 1], rcnt[root]) (from 0 for row 0)
+template <int NT>
+__device__ void group_edges(int* lab, int ne, int nrows, int* rcnt, const int* er, const int* ec, const float* ew, int* sr, int* sc,
+                            float* sw) {
+    for (int e = threadIdx.x; e < ne; e += NT) atomicAdd(&rcnt[uf_find(lab, er[e])], 1);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int run = 0;
+        for (int r = 0; r < nrows; ++r) { const int c = rcnt[r]; rcnt[r] = run; run += c; }
+    }
+    __syncthreads();
+    for (int e = threadIdx.x; e < ne; e += NT) {
+        const int pos = atomicAdd(&rcnt[uf_find(lab, er[e])], 1);
+        sr[pos] = er[e]; sc[pos] = ec[e]; sw[pos] = ew[e];
+    }
+    __syncthreads();
+}
+
+// a small component's m edges sorted by (row, column) on one thread: a deterministic component whatever the grouping order
+__device__ void sort_edges(int* er, int* ec, float* ew, int m) {
+    for (int i = 1; i < m; ++i) {
+        const int r = er[i], c = ec[i];
+        const float a = ew[i];
+        int j = i - 1;
+        while (j >= 0 && (er[j] > r || (er[j] == r && ec[j] > c))) { er[j + 1] = er[j]; ec[j + 1] = ec[j]; ew[j + 1] = ew[j]; --j; }
+        er[j + 1] = r; ec[j + 1] = c; ew[j + 1] = a;
+    }
 }
 
 // exact rectangular assignment (Hungarian with potentials, rows <= cols), a row-major n x m; p[j] = row (1-based) of column j
@@ -110,6 +166,80 @@ __device__ void hungarian_block(const double* a, int n, int m, double* u, double
         if (threadIdx.x == 0)
             do { const int j1 = way[j0]; p[j0] = p[j1]; j0 = j1; } while (j0);
         __syncthreads();
+    }
+}
+
+// doubles of scratch a component of nr rows and nc columns takes: the (smaller side) x (larger side) cost matrix, then the
+// Hungarian's u, v, minv, p, way and used (hungarian_carve)
+__host__ __device__ constexpr size_t hungarian_scratch(int nr, int nc) {
+    const size_t hn = nr < nc ? nr : nc, hm = nr < nc ? nc : nr;
+    return hn * hm + (hn + 1) + 2 * (hm + 1) + (hm + 1) + (hm + 1) / 8 + 2;
+}
+
+struct HungArrays {
+    double *u, *v, *minv;
+    int *p, *way;
+    unsigned char* used;
+};
+
+// the Hungarian's arrays after an hn x hm cost matrix A
+__device__ __forceinline__ HungArrays hungarian_carve(double* A, int hn, int hm) {
+    HungArrays h;
+    h.u = A + (size_t)hn * hm;
+    h.v = h.u + hn + 1;
+    h.minv = h.v + hm + 1;
+    h.p = (int*)(h.minv + hm + 1);
+    h.way = h.p + hm + 1;
+    h.used = (unsigned char*)(h.way + hm + 1);
+    return h;
+}
+
+// one component of nr local rows and nc local columns on one thread.  edge(i, r, c, cost) gives the i-th of m edges as (local row,
+// local column, cost), or false to leave it out; every other entry of the matrix is pad.  The rows of the matrix are the smaller
+// side (the transpose when nr > nc).  match(r, c) gets every assigned (local row, local column) whose cost is below bound.  scr:
+// hungarian_scratch(nr, nc) doubles.
+template <class Edge, class Match>
+__device__ void solve_dense(int nr, int nc, int m, Edge edge, double pad, double bound, double* scr, Match match) {
+    const bool tr = nr > nc;
+    const int hn = tr ? nc : nr, hm = tr ? nr : nc;
+    for (int k = 0; k < hn * hm; ++k) scr[k] = pad;
+    for (int i = 0; i < m; ++i) {
+        int r, c;
+        double cost;
+        if (edge(i, r, c, cost)) scr[tr ? (size_t)c * hm + r : (size_t)r * hm + c] = cost;
+    }
+    const HungArrays h = hungarian_carve(scr, hn, hm);
+    hungarian(scr, hn, hm, h.u, h.v, h.minv, h.p, h.way, h.used);
+    for (int j = 1; j <= hm; ++j) {
+        if (!h.p[j]) continue;
+        const int hi = h.p[j] - 1, hj = j - 1;
+        if (!(scr[(size_t)hi * hm + hj] < bound)) continue;
+        if (tr) match(hj, hi); else match(hi, hj);
+    }
+}
+
+// solve_dense with the whole block of NT threads: edge is called for i < m spread over the block, and match for the assigned pairs
+// spread over the block; the caller synchronises before it reads what match wrote
+template <int NT, class Edge, class Match>
+__device__ void solve_dense_block(int nr, int nc, int m, Edge edge, double pad, double bound, double* scr, HungShared<NT>& sh,
+                                  Match match) {
+    const bool tr = nr > nc;
+    const int hn = tr ? nc : nr, hm = tr ? nr : nc;
+    for (size_t k = threadIdx.x; k < (size_t)hn * hm; k += NT) scr[k] = pad;
+    __syncthreads();
+    for (int i = threadIdx.x; i < m; i += NT) {
+        int r, c;
+        double cost;
+        if (edge(i, r, c, cost)) scr[tr ? (size_t)c * hm + r : (size_t)r * hm + c] = cost;
+    }
+    __syncthreads();
+    const HungArrays h = hungarian_carve(scr, hn, hm);
+    hungarian_block<NT>(scr, hn, hm, h.u, h.v, h.minv, h.p, h.way, h.used, sh);
+    for (int j = 1 + threadIdx.x; j <= hm; j += NT) {
+        if (!h.p[j]) continue;
+        const int hi = h.p[j] - 1, hj = j - 1;
+        if (!(scr[(size_t)hi * hm + hj] < bound)) continue;
+        if (tr) match(hj, hi); else match(hi, hj);
     }
 }
 

@@ -93,3 +93,33 @@ __device__ __forceinline__ int block_exclusive_scan(int v, int* total) {
     __syncthreads();
     return r;
 }
+
+// ordered block-wide compaction: emit(i, pos) for the items i < n with pred(i) true, pos counting them in index order; returns
+// the count.  Every emit is visible to the whole block on return.
+template <class Pred, class Emit>
+__device__ int block_compact(int n, Pred pred, Emit emit) {
+    int total = 0;
+    for (int base = 0; base < n; base += blockDim.x) {
+        const int i = base + threadIdx.x;
+        const int q = i < n && pred(i);
+        int sum;
+        const int pos = block_exclusive_scan(q, &sum);
+        if (q) emit(i, total + pos);
+        total += sum;
+    }
+    __syncthreads();
+    return total;
+}
+
+// a workspace carved in 256-byte aligned pieces, the same list on the host and the device: from a null base it only adds up the
+// bytes, which is how the *_ws_bytes entry points size it
+struct DzCarve {
+    char* base;
+    size_t bytes = 0;
+    __host__ __device__ explicit DzCarve(char* b) : base(b) {}
+    template <typename T> __host__ __device__ T* take(size_t n) {
+        T* r = (T*)(base + bytes);
+        bytes += (n * sizeof(T) + 255) / 256 * 256;
+        return r;
+    }
+};

@@ -41,6 +41,8 @@ constexpr int NSHARD = 16;
 constexpr int WORDS = 4;                    // cutoff bitmask words per node
 constexpr int SMALL_EDGES = 16;             // components with more edges are solved by the whole block
 constexpr int SMALL_CAP = SMALL_EDGES + 2;
+// solve_small's scratch: a component has at most SMALL_EDGES + 1 nodes, and no split of them into rows and columns takes more
+constexpr int SMALL_SCR = hungarian_scratch(SMALL_CAP / 2, SMALL_CAP / 2 + 1);
 constexpr int SCR_CAP = 1 << 16;            // float64 assignment scratch per block
 constexpr double TWO_PI = 6.283185307179586;
 constexpr double PI = 3.141592653589793;
@@ -69,31 +71,25 @@ struct EvIn {
     int NF, R, G, bev, mask, P;
 };
 
-size_t block_ws_bytes(int R, int G, int P) {
-    size_t b = 0;
-    auto add = [&](size_t n) { b += dz_align_up(n, 256); };
-    add((size_t)NSHARD * 2 * 4 * NKD * 8);
-    add((size_t)P * 4 * 6);
-    add((size_t)(G + 3 * R) * 4);
-    add((size_t)G * 4 * 4); add((size_t)R * 4 * 6);
-    add((size_t)G * WORDS * 4); add((size_t)R * WORDS * 4);
-    add((size_t)SCR_CAP * 8);
-    return dz_align_up(b, 256);
+// one block's workspace; carved from a null base it only sizes it (block_ws_bytes)
+__host__ __device__ Ws carve(DzCarve& c, int R, int G, int P) {
+    Ws w;
+    w.diff = c.take<unsigned long long>((size_t)NSHARD * 2 * 4 * NKD);
+    w.eg = c.take<int>((size_t)P * 6); w.ep = w.eg + P; w.sg = w.ep + P; w.sp = w.sg + P;
+    w.eiou = (float*)(w.sp + P); w.siou = w.eiou + P;
+    w.lab = c.take<int>((size_t)G + 3 * R);
+    w.rcnt = c.take<int>((size_t)G * 4); w.rlist = w.rcnt + G; w.rmap = w.rlist + G; w.gbin = w.rmap + G;
+    w.clist = c.take<int>((size_t)R * 6); w.cmap = w.clist + R; w.alist = w.cmap + R; w.amap = w.alist + R; w.pkc = w.amap + R;
+    w.pbin = w.pkc + R;
+    w.gbits = c.take<unsigned>((size_t)G * WORDS); w.pbits = c.take<unsigned>((size_t)R * WORDS);
+    w.scr = c.take<double>(SCR_CAP);
+    return w;
 }
 
-__device__ Ws carve(char* p, int R, int G, int P) {
-    auto take = [&](size_t n) { char* r = p; p += (n + 255) / 256 * 256; return r; };
-    Ws w;
-    w.diff = (unsigned long long*)take((size_t)NSHARD * 2 * 4 * NKD * 8);
-    w.eg = (int*)take((size_t)P * 4 * 6); w.ep = w.eg + P; w.sg = w.ep + P; w.sp = w.sg + P;
-    w.eiou = (float*)(w.sp + P); w.siou = w.eiou + P;
-    w.lab = (int*)take((size_t)(G + 3 * R) * 4);
-    w.rcnt = (int*)take((size_t)G * 4 * 4); w.rlist = w.rcnt + G; w.rmap = w.rlist + G; w.gbin = w.rmap + G;
-    w.clist = (int*)take((size_t)R * 4 * 6); w.cmap = w.clist + R; w.alist = w.cmap + R; w.amap = w.alist + R; w.pkc = w.amap + R;
-    w.pbin = w.pkc + R;
-    w.gbits = (unsigned*)take((size_t)G * WORDS * 4); w.pbits = (unsigned*)take((size_t)R * WORDS * 4);
-    w.scr = (double*)take((size_t)SCR_CAP * 8);
-    return w;
+size_t block_ws_bytes(int R, int G, int P) {
+    DzCarve c(nullptr);
+    carve(c, R, G, P);
+    return c.bytes;
 }
 
 __device__ __forceinline__ int valid_type(int t) { return t >= 1 && t <= 4; }
@@ -152,21 +148,6 @@ __device__ void record_match(const EvIn& in, const Ws& w, int f, int bd, int g, 
     set_bits(w.pbits + (size_t)p * WORDS, lo, hi);
 }
 
-// ordered block-wide compaction of the items i < n with pred(i) true; returns the count
-template <class Pred, class Emit>
-__device__ int ordered_compact(int n, Pred pred, Emit emit) {
-    int total = 0;
-    for (int base = 0; base < n; base += NT) {
-        const int i = base + threadIdx.x;
-        const int q = i < n && pred(i);
-        int sum;
-        const int pos = block_exclusive_scan(q, &sum);
-        if (q) emit(i, total + pos);
-        total += sum;
-    }
-    return total;
-}
-
 // one component of m <= SMALL_EDGES edges (sorted by ground truth, then prediction) on one thread
 __device__ void solve_small(const EvIn& in, const Ws& w, int f, int bd, const int* er, const int* ec, const float* ea, int m) {
     int rows[SMALL_CAP], cols[SMALL_CAP], ckc[SMALL_CAP], eri[SMALL_EDGES], eci[SMALL_EDGES], th[SMALL_CAP], amap[SMALL_CAP];
@@ -187,31 +168,19 @@ __device__ void solve_small(const EvIn& in, const Ws& w, int f, int bd, const in
         for (int q = nth; q > j; --q) th[q] = th[q - 1];
         th[j] = v; ++nth;
     }
-    double A[(SMALL_CAP / 2) * (SMALL_CAP / 2 + 1)], u[SMALL_CAP], v[SMALL_CAP], minv[SMALL_CAP];
-    int p[SMALL_CAP], way[SMALL_CAP];
-    unsigned char used[SMALL_CAP];
+    double scr[SMALL_SCR];
     for (int j = 0; j < nth && th[j] > 0; ++j) {
         const int hi = th[j], lo = j + 1 < nth ? th[j + 1] : 0;
         int na = 0;
         for (int c = 0; c < nc; ++c) amap[c] = ckc[c] >= hi ? na++ : -1;
-        const bool tr = nr > na;
-        const int hn = tr ? na : nr, hm = tr ? nr : na;
-        for (int k = 0; k < hn * hm; ++k) A[k] = 0.;
-        for (int i = 0; i < m; ++i) {
-            const int a = amap[eci[i]];
-            if (a < 0) continue;
-            if (tr) A[a * hm + eri[i]] = -(double)ea[i]; else A[eri[i] * hm + a] = -(double)ea[i];
-        }
-        hungarian(A, hn, hm, u, v, minv, p, way, used);
-        for (int q = 1; q <= hm; ++q) {
-            if (!p[q]) continue;
-            const int hr = p[q] - 1, hc = q - 1;
-            if (!(A[hr * hm + hc] < 0.)) continue;
-            const int ri = tr ? hc : hr, ai = tr ? hr : hc;
+        solve_dense(nr, na, m, [&](int i, int& r, int& a, double& cost) {
+            r = eri[i]; a = amap[eci[i]]; cost = -(double)ea[i];
+            return a >= 0;
+        }, 0., 0., scr, [&](int ri, int ai) {
             int c = 0;
             while (amap[c] != ai) ++c;
             record_match(in, w, f, bd, rows[ri], cols[c], lo, hi);
-        }
+        });
     }
 }
 
@@ -219,7 +188,8 @@ __global__ void __launch_bounds__(NT)
 k_det_eval(EvIn in, long long* records, int* overflow, char* ws_base, size_t block_bytes) {
     __shared__ Shared sh;
     const int R = in.R, G = in.G, P = in.P;
-    Ws w = carve(ws_base + (size_t)blockIdx.x * block_bytes, R, G, P);
+    DzCarve wc(ws_base + (size_t)blockIdx.x * block_bytes);
+    Ws w = carve(wc, R, G, P);
     for (int i = threadIdx.x; i < NSHARD * 2 * 4 * NKD; i += NT) w.diff[i] = 0ull;
     for (int k = threadIdx.x; k < NK; k += NT) sh.cut[k] = score_cutoff(k);
     if (threadIdx.x == 0) sh.overflow = 0;
@@ -266,31 +236,9 @@ k_det_eval(EvIn in, long long* records, int* overflow, char* ws_base, size_t blo
             }
             for (int q = threadIdx.x; q < np * WORDS; q += NT) w.pbits[q] = 0u;
             __syncthreads();
+            uf_label<NT>(w.lab, ne, [&](int e) { return w.eg[e]; }, [&](int e) { return pnode(w.gbin[w.eg[e]], w.ep[e]); }, sh.changed);
+            group_edges<NT>(w.lab, ne, ng, w.rcnt, w.eg, w.ep, w.eiou, w.sg, w.sp, w.siou);
             volatile int* lab = w.lab;
-            while (ne) {                                                  // min-hooking: a component's root is its smallest node
-                if (threadIdx.x == 0) sh.changed = 0;
-                __syncthreads();
-                for (int e = threadIdx.x; e < ne; e += NT) {
-                    const int a = uf_find(lab, w.eg[e]), b = uf_find(lab, pnode(w.gbin[w.eg[e]], w.ep[e]));
-                    if (a != b) { atomicMin(&w.lab[max(a, b)], min(a, b)); sh.changed = 1; }
-                }
-                __syncthreads();
-                const int ch = sh.changed;
-                __syncthreads();
-                if (!ch) break;
-            }
-            for (int e = threadIdx.x; e < ne; e += NT) atomicAdd(&w.rcnt[uf_find(lab, w.eg[e])], 1);
-            __syncthreads();
-            if (threadIdx.x == 0) {
-                int run = 0;
-                for (int g = 0; g < ng; ++g) { const int c = w.rcnt[g]; w.rcnt[g] = run; run += c; }
-            }
-            __syncthreads();
-            for (int e = threadIdx.x; e < ne; e += NT) {
-                const int pos = atomicAdd(&w.rcnt[uf_find(lab, w.eg[e])], 1);   // rcnt becomes the end offset of the component
-                w.sg[pos] = w.eg[e]; w.sp[pos] = w.ep[e]; w.siou[pos] = w.eiou[e];
-            }
-            __syncthreads();
             // small components: one thread each
             for (int root = threadIdx.x; root < ng; root += NT) {
                 const int end = w.rcnt[root], beg = root ? w.rcnt[root - 1] : 0, m = end - beg;
@@ -302,13 +250,7 @@ k_det_eval(EvIn in, long long* records, int* overflow, char* ws_base, size_t blo
                     if (w.pkc[ec[0]] > 0) record_match(in, w, f, bd, er[0], ec[0], 0, w.pkc[ec[0]]);
                     continue;
                 }
-                for (int i = 1; i < m; ++i) {
-                    const int r = er[i], c = ec[i];
-                    const float a = ea[i];
-                    int j = i - 1;
-                    while (j >= 0 && (er[j] > r || (er[j] == r && ec[j] > c))) { er[j + 1] = er[j]; ec[j + 1] = ec[j]; ea[j + 1] = ea[j]; --j; }
-                    er[j + 1] = r; ec[j + 1] = c; ea[j + 1] = a;
-                }
+                sort_edges(er, ec, ea, m);
                 solve_small(in, w, f, bd, er, ec, ea, m);
             }
             __syncthreads();
@@ -317,10 +259,10 @@ k_det_eval(EvIn in, long long* records, int* overflow, char* ws_base, size_t blo
                 const int end = w.rcnt[root], beg = root ? w.rcnt[root - 1] : 0;
                 if (end - beg <= SMALL_EDGES || uf_find(lab, root) != root) continue;
                 const int gb = w.gbin[root];
-                const int nr = ordered_compact(ng, [&](int g) { return uf_find(lab, g) == root; },
-                                               [&](int g, int pos) { w.rmap[g] = pos; w.rlist[pos] = g; });
-                const int nc = ordered_compact(np, [&](int p) { return uf_find(lab, pnode(gb, p)) == root; },
-                                               [&](int p, int pos) { w.cmap[p] = pos; w.clist[pos] = p; });
+                const int nr = block_compact(ng, [&](int g) { return uf_find(lab, g) == root; },
+                                             [&](int g, int pos) { w.rmap[g] = pos; w.rlist[pos] = g; });
+                const int nc = block_compact(np, [&](int p) { return uf_find(lab, pnode(gb, p)) == root; },
+                                             [&](int p, int pos) { w.cmap[p] = pos; w.clist[pos] = p; });
                 for (int k = threadIdx.x; k < NKD; k += NT) sh.present[k] = 0;
                 __syncthreads();
                 for (int c = threadIdx.x; c < nc; c += NT) sh.present[w.pkc[w.clist[c]]] = 1;
@@ -329,40 +271,21 @@ k_det_eval(EvIn in, long long* records, int* overflow, char* ws_base, size_t blo
                     if (!sh.present[hi]) continue;
                     int lo = hi - 1;
                     while (lo > 0 && !sh.present[lo]) --lo;
-                    const int na = ordered_compact(nc, [&](int c) { return w.pkc[w.clist[c]] >= hi; },
-                                                   [&](int c, int pos) { w.amap[c] = pos; w.alist[pos] = c; });
-                    const bool tr = nr > na;
-                    const int hn = tr ? na : nr, hm = tr ? nr : na;
-                    const size_t need = (size_t)hn * hm + (hn + 1) + 2 * (hm + 1) + (hm + 1) + (hm + 1) / 8 + 2;
-                    if (need > (size_t)SCR_CAP) {
+                    const int na = block_compact(nc, [&](int c) { return w.pkc[w.clist[c]] >= hi; },
+                                                 [&](int c, int pos) { w.amap[c] = pos; w.alist[pos] = c; });
+                    if (hungarian_scratch(nr, na) > (size_t)SCR_CAP) {
                         if (threadIdx.x == 0) sh.overflow |= 2;
                         __syncthreads();
                         continue;
                     }
-                    double* A = w.scr;
-                    for (size_t k = threadIdx.x; k < (size_t)hn * hm; k += NT) A[k] = 0.;
-                    __syncthreads();
-                    for (int e = beg + threadIdx.x; e < end; e += NT) {
-                        const int p = w.sp[e];
-                        if (w.pkc[p] < hi) continue;
-                        const int ri = w.rmap[w.sg[e]], ai = w.amap[w.cmap[p]];
-                        if (tr) A[(size_t)ai * hm + ri] = -(double)w.siou[e]; else A[(size_t)ri * hm + ai] = -(double)w.siou[e];
-                    }
-                    __syncthreads();
-                    double* u = A + (size_t)hn * hm;
-                    double* v = u + hn + 1;
-                    double* minv = v + hm + 1;
-                    int* pp = (int*)(minv + hm + 1);
-                    int* way = pp + hm + 1;
-                    unsigned char* used = (unsigned char*)(way + hm + 1);
-                    hungarian_block<NT>(A, hn, hm, u, v, minv, pp, way, used, sh.hs);
-                    for (int q = 1 + threadIdx.x; q <= hm; q += NT) {
-                        if (!pp[q]) continue;
-                        const int hr = pp[q] - 1, hc = q - 1;
-                        if (!(A[(size_t)hr * hm + hc] < 0.)) continue;
-                        const int ri = tr ? hc : hr, ai = tr ? hr : hc;
+                    solve_dense_block<NT>(nr, na, end - beg, [&](int i, int& ri, int& ai, double& cost) {
+                        const int p = w.sp[beg + i];
+                        if (w.pkc[p] < hi) return false;
+                        ri = w.rmap[w.sg[beg + i]]; ai = w.amap[w.cmap[p]]; cost = -(double)w.siou[beg + i];
+                        return true;
+                    }, 0., 0., w.scr, sh.hs, [&](int ri, int ai) {
                         record_match(in, w, f, bd, w.rlist[ri], w.clist[w.alist[ai]], lo, hi);
-                    }
+                    });
                     __syncthreads();
                 }
             }

@@ -1,5 +1,5 @@
 // eval_common.cuh -- device pieces shared by the scorings against ground truth: det_eval.cu (Waymo AP / APH), track_gt.cu (tracks
-// against ground truth) and track_eval.cu (Waymo MOTA / MOTP).
+// against ground truth) and track_eval.cu (Waymo MOTA / MOTP); yawf also by the tracker (tracker.cu).
 #pragma once
 #include <cuda_runtime.h>
 

@@ -30,12 +30,12 @@
 // component of at most SMALL_EDGES edges (sorted by ground truth, then prediction, so the result does not depend on the edge order)
 // is run by every chain thread on its own: a single edge in closed form, otherwise retention by a scan of the edges for each row's
 // previous id and the Hungarian of assign.cuh on the rest.  A larger component is run by the whole block, one cutoff at a time,
-// with hungarian_block (rows and columns compacted in index order).  The chain state, each object's last matched id and frame per
+// with solve_dense_block of assign.cuh (rows and columns compacted in index order).  The chain state, each object's last matched id and frame per
 // cutoff, is in the workspace.  Misses and FP are not tracked per row: the block counts the counting ground truth per (range, level)
 // and the active predictions per (range, cutoff), and the records take the matched ones off.  Counts go to shared-memory
 // accumulators and then to the int64 records by integer atomics, so the records are identical run to run and whatever the grouping
-// of sequences into calls.  A chain thread's one-thread Hungarian keeps its arrays on the stack; ptxas reports 52 bytes of spill
-// stores around it (det_eval.cu's k_det_eval, built the same way, reports 88), off the per-frame edge and IoU passes.
+// of sequences into calls.  A chain thread's one-thread solve keeps its scratch on the stack (SMALL_SCR doubles); ptxas reports 72
+// bytes of spill stores around it for sm_90a, off the per-frame edge and IoU passes.
 //
 // Flags (*overflow): bit 1 a frame has more than max_pairs valid edges of one type, bit 2 a component exceeds the assignment
 // scratch (the records are then invalid); bit 4 two rows of one frame share a prediction id or a ground-truth object, bit 8 a
@@ -52,11 +52,13 @@ constexpr int NK = 101;                     // score cutoffs = chains per (seque
 constexpr int NKD = NK + 1;
 constexpr int SMALL_EDGES = 16;             // components with more edges are run by the whole block
 constexpr int SMALL_CAP = SMALL_EDGES + 2;
+// chain_small's scratch: a component has at most SMALL_EDGES + 1 nodes, and no split of them into rows and columns takes more
+constexpr int SMALL_SCR = hungarian_scratch(SMALL_CAP / 2, SMALL_CAP / 2 + 1);
 constexpr int SCR_CAP = 1 << 15;            // float64 assignment scratch per block
 constexpr double FIXED = 4294967296.;
 
 struct Shared {
-    int overflow, n_edges, changed, n_comp, kmax;
+    int overflow, n_edges, changed, kmax;
     unsigned long long mt[NK][3][2], mm[NK][3][2], cost[NK][3][2];   // matches, mismatches, cost per (cutoff, gt range, level)
     unsigned long long pm[NK][3];                                    // matched predictions per (cutoff, prediction range)
     unsigned long long act[3][NKD];                                  // predictions per (range, number of active cutoffs)
@@ -83,46 +85,25 @@ struct TeIn {
     int S, F, R, G, O, P, mask;
 };
 
-size_t block_ws_bytes(int R, int G, int O, int P) {
-    size_t b = 0;
-    auto add = [&](size_t n) { b += dz_align_up(n, 256); };
-    add((size_t)P * 4 * 6);
-    add((size_t)(G + R) * 4);
-    add((size_t)G * 4 * 9);
-    add((size_t)R * 4 * 6);
-    add((size_t)O * NK * 4 * 2);
-    add((size_t)SCR_CAP * 8);
-    return dz_align_up(b, 256);
-}
-
-__device__ Ws carve(char* p, int R, int G, int O, int P) {
-    auto take = [&](size_t n) { char* r = p; p += (n + 255) / 256 * 256; return r; };
+// one block's workspace; carved from a null base it only sizes it (block_ws_bytes)
+__host__ __device__ Ws carve(DzCarve& c, int R, int G, int O, int P) {
     Ws w;
-    w.eg = (int*)take((size_t)P * 4 * 6); w.ep = w.eg + P; w.sg = w.ep + P; w.sp = w.sg + P;
+    w.eg = c.take<int>((size_t)P * 6); w.ep = w.eg + P; w.sg = w.ep + P; w.sp = w.sg + P;
     w.eiou = (float*)(w.sp + P); w.siou = w.eiou + P;
-    w.lab = (int*)take((size_t)(G + R) * 4);
-    w.rcnt = (int*)take((size_t)G * 4 * 9); w.comp = w.rcnt + G; w.gobj = w.comp + G; w.gbin = w.gobj + G; w.glv = w.gbin + G;
+    w.lab = c.take<int>((size_t)G + R);
+    w.rcnt = c.take<int>((size_t)G * 9); w.comp = w.rcnt + G; w.gobj = w.comp + G; w.gbin = w.gobj + G; w.glv = w.gbin + G;
     w.rret = w.glv + G; w.rmatch = w.rret + G; w.rmap = w.rmatch + G; w.rlist = w.rmap + G;
-    w.pkc = (int*)take((size_t)R * 4 * 6); w.pbin = w.pkc + R; w.pid = w.pbin + R; w.cret = w.pid + R; w.cmap = w.cret + R;
+    w.pkc = c.take<int>((size_t)R * 6); w.pbin = w.pkc + R; w.pid = w.pbin + R; w.cret = w.pid + R; w.cmap = w.cret + R;
     w.clist = w.cmap + R;
-    w.lid = (int*)take((size_t)O * NK * 4 * 2); w.lf = w.lid + (size_t)O * NK;
-    w.scr = (double*)take((size_t)SCR_CAP * 8);
+    w.lid = c.take<int>((size_t)O * NK * 2); w.lf = w.lid + (size_t)O * NK;
+    w.scr = c.take<double>(SCR_CAP);
     return w;
 }
 
-// ordered block-wide compaction of the items i < n with pred(i) true; returns the count
-template <class Pred, class Emit>
-__device__ int ordered_compact(int n, Pred pred, Emit emit) {
-    int total = 0;
-    for (int base = 0; base < n; base += NT) {
-        const int i = base + threadIdx.x;
-        const int q = i < n && pred(i);
-        int sum;
-        const int pos = block_exclusive_scan(q, &sum);
-        if (q) emit(i, total + pos);
-        total += sum;
-    }
-    return total;
+size_t block_ws_bytes(int R, int G, int O, int P) {
+    DzCarve c(nullptr);
+    carve(c, R, G, O, P);
+    return c.bytes;
 }
 
 // ground-truth row g matched to prediction row p in frame f by the chain of cutoff k: counts, then the chain state of g's object
@@ -175,29 +156,19 @@ __device__ void chain_small(Shared& sh, const Ws& w, int f, int k, const int* er
     for (int r = 0; r < nr; ++r) rmap[r] = rr[r] ? -1 : hr++;
     for (int c = 0; c < nc; ++c) amap[c] = (!rc[c] && w.pkc[cols[c]] > k) ? na++ : -1;
     if (hr && na) {                                                       // fresh matching of the rest
-        double A[(SMALL_CAP / 2) * (SMALL_CAP / 2 + 1)], u[SMALL_CAP], v[SMALL_CAP], minv[SMALL_CAP];
-        int pp[SMALL_CAP], way[SMALL_CAP], rl[SMALL_CAP], al[SMALL_CAP];
-        unsigned char used[SMALL_CAP];
+        double scr[SMALL_SCR];
+        int rl[SMALL_CAP], al[SMALL_CAP];
         for (int r = 0; r < nr; ++r) if (rmap[r] >= 0) rl[rmap[r]] = r;
         for (int c = 0; c < nc; ++c) if (amap[c] >= 0) al[amap[c]] = c;
-        const bool tr = hr > na;
-        const int hn = tr ? na : hr, hm = tr ? hr : na;
-        for (int q = 0; q < hn * hm; ++q) A[q] = 0.;
-        for (int i = 0; i < m; ++i) {
-            const int a = rmap[eri[i]], b = amap[eci[i]];
-            if (a < 0 || b < 0) continue;
-            if (tr) A[b * hm + a] = -(double)ea[i]; else A[a * hm + b] = -(double)ea[i];
-        }
-        hungarian(A, hn, hm, u, v, minv, pp, way, used);
-        for (int q = 1; q <= hm; ++q) {
-            if (!pp[q]) continue;
-            const int h0 = pp[q] - 1, h1 = q - 1;
-            if (!(A[h0 * hm + h1] < 0.)) continue;
-            const int r = rl[tr ? h1 : h0], c = al[tr ? h0 : h1];
+        solve_dense(hr, na, m, [&](int i, int& a, int& b, double& cost) {
+            a = rmap[eri[i]]; b = amap[eci[i]]; cost = -(double)ea[i];
+            return a >= 0 && b >= 0;
+        }, 0., 0., scr, [&](int a, int b) {
+            const int r = rl[a], c = al[b];
             int i = 0;
             while (eri[i] != r || eci[i] != c) ++i;
             mg[nm] = er[i]; mp[nm] = ec[i]; mi[nm] = ea[i]; ++nm;
-        }
+        });
     }
     for (int q = 0; q < nm; ++q) record_match(sh, w, f, k, mg[q], mp[q], mi[q]);
 }
@@ -207,7 +178,8 @@ k_track_eval(TeIn in, long long* records, int* flags, char* ws_base, size_t bloc
     __shared__ Shared sh;
     const int t = blockIdx.x + 1, s = blockIdx.y;
     const int R = in.R, G = in.G, P = in.P;
-    Ws w = carve(ws_base + ((size_t)s * 4 + blockIdx.x) * block_bytes, R, G, in.O, P);
+    DzCarve wc(ws_base + ((size_t)s * 4 + blockIdx.x) * block_bytes);
+    Ws w = carve(wc, R, G, in.O, P);
     const int Fs = min(max(in.num_frames[s], 0), in.F), no = min(max(in.n_obj[s], 0), in.O);
     for (size_t i = threadIdx.x; i < (size_t)no * NK; i += NT) { w.lid[i] = -1; w.lf[i] = -2; }
     for (int i = threadIdx.x; i < NK * 6; i += NT) {
@@ -284,50 +256,14 @@ k_track_eval(TeIn in, long long* records, int* flags, char* ws_base, size_t bloc
         const int ne = min(sh.n_edges, P);
         __syncthreads();
         if (ne == 0) continue;
+        uf_label<NT>(w.lab, ne, [&](int e) { return w.eg[e]; }, [&](int e) { return G + w.ep[e]; }, sh.changed);
+        group_edges<NT>(w.lab, ne, ng, w.rcnt, w.eg, w.ep, w.eiou, w.sg, w.sp, w.siou);
         volatile int* lab = w.lab;
-        while (true) {                                                    // min-hooking: a component's root is its smallest row
-            if (threadIdx.x == 0) sh.changed = 0;
-            __syncthreads();
-            for (int e = threadIdx.x; e < ne; e += NT) {
-                const int a = uf_find(lab, w.eg[e]), b = uf_find(lab, G + w.ep[e]);
-                if (a != b) { atomicMin(&w.lab[max(a, b)], min(a, b)); sh.changed = 1; }
-            }
-            __syncthreads();
-            const int ch = sh.changed;
-            __syncthreads();
-            if (!ch) break;
-        }
-        for (int e = threadIdx.x; e < ne; e += NT) atomicAdd(&w.rcnt[uf_find(lab, w.eg[e])], 1);
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            int run = 0, nc = 0;
-            for (int g = 0; g < ng; ++g) {
-                const int c = w.rcnt[g];
-                if (c) w.comp[nc++] = g;
-                w.rcnt[g] = run; run += c;
-            }
-            sh.n_comp = nc;
-        }
-        __syncthreads();
-        for (int e = threadIdx.x; e < ne; e += NT) {
-            const int pos = atomicAdd(&w.rcnt[uf_find(lab, w.eg[e])], 1);   // rcnt becomes the end offset of the component
-            w.sg[pos] = w.eg[e]; w.sp[pos] = w.ep[e]; w.siou[pos] = w.eiou[e];
-        }
-        __syncthreads();
-        const int ncomp = sh.n_comp;
+        const int ncomp = block_compact(ng, [&](int g) { return w.rcnt[g] != (g ? w.rcnt[g - 1] : 0); },
+                                        [&](int g, int pos) { w.comp[pos] = g; });
         for (int c = threadIdx.x; c < ncomp; c += NT) {                   // sort the small components by (row, prediction)
             const int root = w.comp[c], end = w.rcnt[root], beg = root ? w.rcnt[root - 1] : 0, m = end - beg;
-            if (m > SMALL_EDGES) continue;
-            int* er = w.sg + beg;
-            int* ec = w.sp + beg;
-            float* ea = w.siou + beg;
-            for (int i = 1; i < m; ++i) {
-                const int r = er[i], cc = ec[i];
-                const float a = ea[i];
-                int j = i - 1;
-                while (j >= 0 && (er[j] > r || (er[j] == r && ec[j] > cc))) { er[j + 1] = er[j]; ec[j + 1] = ec[j]; ea[j + 1] = ea[j]; --j; }
-                er[j + 1] = r; ec[j + 1] = cc; ea[j + 1] = a;
-            }
+            if (m <= SMALL_EDGES) sort_edges(w.sg + beg, w.sp + beg, w.siou + beg, m);
         }
         __syncthreads();
         // ------------------------------------------------------------ small components: every chain on its own thread
@@ -355,40 +291,20 @@ k_track_eval(TeIn in, long long* records, int* flags, char* ws_base, size_t bloc
                     if (w.pkc[p] > k && retained(w, f, k, g, p)) { w.rret[g] = 1; w.cret[p] = 1; w.rmatch[g] = e; }
                 }
                 __syncthreads();
-                const int nr = ordered_compact(ng, [&](int g) { return !w.rret[g] && uf_find(lab, g) == root; },
-                                               [&](int g, int pos) { w.rmap[g] = pos; w.rlist[pos] = g; });
-                const int na = ordered_compact(np, [&](int p) { return w.pkc[p] > k && !w.cret[p] && uf_find(lab, G + p) == root; },
-                                               [&](int p, int pos) { w.cmap[p] = pos; w.clist[pos] = p; });
+                const int nr = block_compact(ng, [&](int g) { return !w.rret[g] && uf_find(lab, g) == root; },
+                                             [&](int g, int pos) { w.rmap[g] = pos; w.rlist[pos] = g; });
+                const int na = block_compact(np, [&](int p) { return w.pkc[p] > k && !w.cret[p] && uf_find(lab, G + p) == root; },
+                                             [&](int p, int pos) { w.cmap[p] = pos; w.clist[pos] = p; });
                 if (nr && na) {
-                    const bool tr = nr > na;
-                    const int hn = tr ? na : nr, hm = tr ? nr : na;
-                    const size_t need = (size_t)hn * hm + (hn + 1) + 2 * (hm + 1) + (hm + 1) + (hm + 1) / 8 + 2;
-                    if (need > (size_t)SCR_CAP) {
+                    if (hungarian_scratch(nr, na) > (size_t)SCR_CAP) {
                         if (threadIdx.x == 0) sh.overflow |= 2;
                     } else {
-                        double* A = w.scr;
-                        for (size_t q = threadIdx.x; q < (size_t)hn * hm; q += NT) A[q] = 0.;
-                        __syncthreads();
-                        for (int e = beg + threadIdx.x; e < end; e += NT) {
-                            const int g = w.sg[e], p = w.sp[e];
-                            if (w.pkc[p] <= k || w.rret[g] || w.cret[p]) continue;
-                            const int ri = w.rmap[g], ai = w.cmap[p];
-                            if (tr) A[(size_t)ai * hm + ri] = -(double)w.siou[e]; else A[(size_t)ri * hm + ai] = -(double)w.siou[e];
-                        }
-                        __syncthreads();
-                        double* u = A + (size_t)hn * hm;
-                        double* v = u + hn + 1;
-                        double* minv = v + hm + 1;
-                        int* pp = (int*)(minv + hm + 1);
-                        int* way = pp + hm + 1;
-                        unsigned char* used = (unsigned char*)(way + hm + 1);
-                        hungarian_block<NT>(A, hn, hm, u, v, minv, pp, way, used, sh.hs);
-                        for (int q = 1 + threadIdx.x; q <= hm; q += NT) {
-                            if (!pp[q]) continue;
-                            const int h0 = pp[q] - 1, h1 = q - 1;
-                            if (!(A[(size_t)h0 * hm + h1] < 0.)) continue;
-                            w.rmatch[w.rlist[tr ? h1 : h0]] = -2 - w.clist[tr ? h0 : h1];
-                        }
+                        solve_dense_block<NT>(nr, na, end - beg, [&](int i, int& ri, int& ai, double& cost) {
+                            const int g = w.sg[beg + i], p = w.sp[beg + i];
+                            if (w.pkc[p] <= k || w.rret[g] || w.cret[p]) return false;
+                            ri = w.rmap[g]; ai = w.cmap[p]; cost = -(double)w.siou[beg + i];
+                            return true;
+                        }, 0., 0., w.scr, sh.hs, [&](int ri, int ai) { w.rmatch[w.rlist[ri]] = -2 - w.clist[ai]; });
                     }
                 }
                 __syncthreads();

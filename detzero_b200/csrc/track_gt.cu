@@ -15,8 +15,8 @@
 //               order and the results are bit-identical run to run and whatever the batch.
 //   assignment  similarity = sum / trajectory length (float32) for the pairs with a positive count, cost (double)(1.f - sim);
 //               GNN_assignment of the reference (scipy linear_sum_assignment, 5000 where the cost is >= 1) is solved as in
-//               tracker.cu: union-find components of the valid edges, the exact Hungarian of assign.cuh per component, on one thread
-//               for a small component and on the whole block for a large one.
+//               tracker.cu: union-find components of the valid edges and the exact Hungarian per component (assign.cuh), on one
+//               thread for a small component and on the whole block for a large one.
 //   outputs     per object [matched track, match count, trajectory length, L1/L2 bucket, class of the first row]; per track
 //               [matched object, class, entry count, dynamic]; per entry the BEV IoU with the matched object in that frame (0
 //               where the object is absent or of another class).  An object's bucket is 2 if it is matched and any of its boxes is
@@ -78,21 +78,6 @@ __device__ int pair_slot(unsigned long long* keys, int H, int o, int k, bool ins
     return -1;
 }
 
-// ordered block-wide compaction of the items i < n with pred(i) true (block_exclusive_scan per NT items); returns the count
-template <class Pred, class Emit>
-__device__ int ordered_compact(int n, Pred pred, Emit emit) {
-    int total = 0;
-    for (int base = 0; base < n; base += NT) {
-        const int i = base + threadIdx.x;
-        const int p = i < n && pred(i);
-        int sum;
-        const int pos = block_exclusive_scan(p, &sum);
-        if (p) emit(i, total + pos);
-        total += sum;
-    }
-    return total;
-}
-
 struct GtIn {
     const float* box;     // (S, F, G, 7) lidar
     const double* world;  // (S, F, G, 9)
@@ -127,35 +112,26 @@ struct GtPar {
 
 }  // namespace
 
-static size_t gt_seq_ws_bytes(int F, int O, int T, int E, int P, int H) {
-    size_t b = 0;
-    auto add = [&](size_t n) { b += dz_align_up(n, 256); };
-    add((size_t)E * 7 * 4); add((size_t)E * 4); add((size_t)(F + 1) * 4); add((size_t)(F + 1) * 4); add((size_t)E * 4);
-    add((size_t)H * 8); add((size_t)H * 4); add((size_t)H * 4);
-    add((size_t)P * 4 * 6);
-    add((size_t)(O + T) * 4); add((size_t)O * 4); add((size_t)O * 4); add((size_t)T * 4); add((size_t)O * 4); add((size_t)T * 4);
-    add((size_t)O * 4 * 4); add((size_t)O * F * 4); add((size_t)O * 4); add((size_t)T * 4);
-    add((size_t)SCR_CAP * 8);
-    return b + 256;
+// one sequence's workspace; carved from a null base it only sizes it (gt_seq_ws_bytes)
+static __host__ __device__ Ws carve_gt(DzCarve& c, int F, int O, int T, int E, int P, int H) {
+    Ws w;
+    w.elid = c.take<float>((size_t)E * 7); w.ent_trk = c.take<int>(E);
+    w.fcnt = c.take<int>((size_t)F + 1); w.foff = c.take<int>((size_t)F + 1); w.flist = c.take<int>(E);
+    w.keys = c.take<unsigned long long>(H); w.psum = c.take<float>(H); w.pcnt = c.take<int>(H);
+    w.er = c.take<int>((size_t)P * 6); w.ec = w.er + P; w.es_r = w.ec + P; w.es_c = w.es_r + P;
+    w.esim = (float*)(w.es_c + P); w.es_sim = w.esim + P;
+    w.lab = c.take<int>((size_t)O + T); w.rcnt = c.take<int>(O);
+    w.rmap = c.take<int>(O); w.cmap = c.take<int>(T); w.rlist = c.take<int>(O); w.clist = c.take<int>(T);
+    w.olen = c.take<int>((size_t)O * 4); w.ofirst = w.olen + O; w.olast = w.ofirst + O; w.oany2 = w.olast + O;
+    w.orow = c.take<int>((size_t)O * F); w.mr = c.take<int>(O); w.mc = c.take<int>(T);
+    w.scr = c.take<double>(SCR_CAP);
+    return w;
 }
 
-static __device__ Ws carve_gt(char* p, int F, int O, int T, int E, int P, int H) {
-    Ws w;
-#define take(n) take_gt(p, (n))
-    auto take_gt = [](char*& q, size_t n) { char* r = q; q += (n + 255) / 256 * 256; return r; };
-    w.elid = (float*)take((size_t)E * 7 * 4); w.ent_trk = (int*)take((size_t)E * 4);
-    w.fcnt = (int*)take((size_t)(F + 1) * 4); w.foff = (int*)take((size_t)(F + 1) * 4); w.flist = (int*)take((size_t)E * 4);
-    w.keys = (unsigned long long*)take((size_t)H * 8); w.psum = (float*)take((size_t)H * 4); w.pcnt = (int*)take((size_t)H * 4);
-    w.er = (int*)take((size_t)P * 4 * 6); w.ec = w.er + P; w.es_r = w.ec + P; w.es_c = w.es_r + P;
-    w.esim = (float*)(w.es_c + P); w.es_sim = w.esim + P;
-    w.lab = (int*)take((size_t)(O + T) * 4); w.rcnt = (int*)take((size_t)O * 4);
-    w.rmap = (int*)take((size_t)O * 4); w.cmap = (int*)take((size_t)T * 4); w.rlist = (int*)take((size_t)O * 4);
-    w.clist = (int*)take((size_t)T * 4);
-    w.olen = (int*)take((size_t)O * 4 * 4); w.ofirst = w.olen + O; w.olast = w.ofirst + O; w.oany2 = w.olast + O;
-    w.orow = (int*)take((size_t)O * F * 4); w.mr = (int*)take((size_t)O * 4); w.mc = (int*)take((size_t)T * 4);
-    w.scr = (double*)take((size_t)SCR_CAP * 8);
-#undef take
-    return w;
+static size_t gt_seq_ws_bytes(int F, int O, int T, int E, int P, int H) {
+    DzCarve c(nullptr);
+    carve_gt(c, F, O, T, E, P, H);
+    return c.bytes + 256;
 }
 
 __global__ void __launch_bounds__(NT, 1)
@@ -164,7 +140,8 @@ k_track_gt(GtIn gt, TkIn tk, GtPar pr, GtOut out, char* ws_base, size_t seq_byte
     const int F = gt.F, G = gt.G, T = tk.T, E = tk.E, P = pr.P, H = pr.H;
     const int O = gt.O;
     __shared__ Shared sh;
-    Ws w = carve_gt(ws_base + (size_t)s * seq_bytes, F, O, T, E, P, H);
+    DzCarve wc(ws_base + (size_t)s * seq_bytes);
+    Ws w = carve_gt(wc, F, O, T, E, P, H);
     const int nt = min(max(tk.n_tracks[s], 0), T);
     const int no = min(max(gt.n_obj[s], 0), O);
     const int Fs = min(max(gt.nf[s], 0), F);
@@ -174,7 +151,7 @@ k_track_gt(GtIn gt, TkIn tk, GtPar pr, GtOut out, char* ws_base, size_t seq_byte
     const double* poses = tk.poses + (size_t)s * F * 16;
     const size_t gbase = (size_t)s * F * G;
     const int n_ent = nt ? min(trk[(size_t)(nt - 1) * 6 + 5] + trk[(size_t)(nt - 1) * 6 + 3], E) : 0;
-    if (threadIdx.x == 0) { sh.overflow = 0; sh.n_pairs = 0; sh.n_edges = 0; }
+    if (threadIdx.x == 0) { sh.overflow = 0; sh.n_pairs = 0; sh.n_edges = 0; sh.scr_used = 0; }
     for (int i = threadIdx.x; i < H; i += NT) { w.keys[i] = EMPTY; w.psum[i] = 0.f; w.pcnt[i] = 0; }
     for (int o = threadIdx.x; o < no; o += NT) { w.olen[o] = 0; w.ofirst[o] = INT_MAX; w.olast[o] = -1; w.oany2[o] = 0; w.mr[o] = -1; }
     for (size_t i = threadIdx.x; i < (size_t)no * F; i += NT) w.orow[i] = -1;
@@ -256,32 +233,10 @@ k_track_gt(GtIn gt, TkIn tk, GtPar pr, GtOut out, char* ws_base, size_t seq_byte
     for (int o = threadIdx.x; o < no; o += NT) w.rcnt[o] = 0;
     __syncthreads();
     const int ne = min(sh.n_edges, P);
+    uf_label<NT>(w.lab, ne, [&](int e) { return w.er[e]; }, [&](int e) { return no + w.ec[e]; }, sh.changed);
+    group_edges<NT>(w.lab, ne, no, w.rcnt, w.er, w.ec, w.esim, w.es_r, w.es_c, w.es_sim);
     volatile int* lab = w.lab;
-    while (ne) {                                                         // min-hooking: a component's root is its smallest object
-        if (threadIdx.x == 0) sh.changed = 0;
-        __syncthreads();
-        for (int e = threadIdx.x; e < ne; e += NT) {
-            const int a = uf_find(lab, w.er[e]), b = uf_find(lab, no + w.ec[e]);
-            if (a != b) { atomicMin(&w.lab[max(a, b)], min(a, b)); sh.changed = 1; }
-        }
-        __syncthreads();
-        const int ch = sh.changed;
-        __syncthreads();
-        if (!ch) break;
-    }
-    for (int e = threadIdx.x; e < ne; e += NT) atomicAdd(&w.rcnt[uf_find(lab, w.er[e])], 1);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        int run = 0;
-        for (int o = 0; o < no; ++o) { const int c = w.rcnt[o]; w.rcnt[o] = run; run += c; }
-        sh.scr_used = 0;
-    }
-    __syncthreads();
-    for (int e = threadIdx.x; e < ne; e += NT) {
-        const int pos = atomicAdd(&w.rcnt[uf_find(lab, w.er[e])], 1);      // rcnt becomes the end offset of the component
-        w.es_r[pos] = w.er[e]; w.es_c[pos] = w.ec[e]; w.es_sim[pos] = w.esim[e];
-    }
-    __syncthreads();
+    // cost (double)(1.f - sim), 5000 off the valid edges; a chosen pair is a match when its cost is below 1
     // small components: one thread each, edges sorted by (object, track)
     for (int root = threadIdx.x; root < no; root += NT) {
         const int end = w.rcnt[root], beg = root ? w.rcnt[root - 1] : 0;
@@ -292,17 +247,11 @@ k_track_gt(GtIn gt, TkIn tk, GtPar pr, GtOut out, char* ws_base, size_t seq_byte
         const int m = end - beg;
         if (m == 1) { w.mr[er[0]] = ec[0]; continue; }
         if (m > SMALL_EDGES) continue;
-        for (int i = 1; i < m; ++i) {
-            const int r = er[i], c = ec[i];
-            const float a = ea[i];
-            int j = i - 1;
-            while (j >= 0 && (er[j] > r || (er[j] == r && ec[j] > c))) { er[j + 1] = er[j]; ec[j + 1] = ec[j]; ea[j + 1] = ea[j]; --j; }
-            er[j + 1] = r; ec[j + 1] = c; ea[j + 1] = a;
-        }
+        sort_edges(er, ec, ea, m);
         const int need = 3 * m + 8;
         const int base = atomicAdd(&sh.scr_used, need);
         if (base + need > SCR_CAP) { atomicOr(&sh.overflow, 2); continue; }
-        int* cols = (int*)(w.scr + base);
+        int* cols = (int*)(w.scr + base);                                // distinct tracks, ascending
         int nc = 0;
         for (int i = 0; i < m; ++i) {
             const int c = ec[i];
@@ -315,74 +264,37 @@ k_track_gt(GtIn gt, TkIn tk, GtPar pr, GtOut out, char* ws_base, size_t seq_byte
         int* rows = cols + nc;
         int nr = 0;
         for (int i = 0; i < m; ++i) if (i == 0 || er[i] != er[i - 1]) rows[nr++] = er[i];
-        const bool tr = nr > nc;                                         // Hungarian rows = the smaller side
-        const int hn = tr ? nc : nr, hm = tr ? nr : nc;
-        const int need2 = hn * hm + 3 * (hm + 1) + (hn + 1) + 3 * (hm + 1) / 2 + 8;
+        const int need2 = (int)hungarian_scratch(nr, nc);
         const int base2 = atomicAdd(&sh.scr_used, need2);
         if (base2 + need2 > SCR_CAP) { atomicOr(&sh.overflow, 2); continue; }
-        double* A = w.scr + base2;
-        for (int k = 0; k < hn * hm; ++k) A[k] = 5000.;
-        for (int i = 0; i < m; ++i) {
-            int ri = 0, ci = 0;
+        solve_dense(nr, nc, m, [&](int i, int& ri, int& ci, double& cost) {
+            ri = 0; ci = 0;
             while (rows[ri] != er[i]) ++ri;
             while (cols[ci] != ec[i]) ++ci;
-            const double cost = (double)(1.f - ea[i]);
-            if (tr) A[(size_t)ci * hm + ri] = cost; else A[(size_t)ri * hm + ci] = cost;
-        }
-        double* u = A + hn * hm;
-        double* v = u + hn + 1;
-        double* minv = v + hm + 1;
-        int* p = (int*)(minv + hm + 1);
-        int* way = p + hm + 1;
-        unsigned char* used = (unsigned char*)(way + hm + 1);
-        hungarian(A, hn, hm, u, v, minv, p, way, used);
-        for (int j = 1; j <= hm; ++j) {
-            if (!p[j]) continue;
-            const int hi = p[j] - 1, hj = j - 1;
-            if (!(A[(size_t)hi * hm + hj] < 1.)) continue;
-            w.mr[tr ? rows[hj] : rows[hi]] = tr ? cols[hi] : cols[hj];
-        }
+            cost = (double)(1.f - ea[i]);
+            return true;
+        }, 5000., 1., w.scr + base2, [&](int ri, int ci) { w.mr[rows[ri]] = cols[ci]; });
     }
     __syncthreads();
     // large components: one at a time, the whole block on each
     for (int root = 0; root < no; ++root) {
         const int end = w.rcnt[root], beg = root ? w.rcnt[root - 1] : 0;
         if (end - beg <= SMALL_EDGES || uf_find(lab, root) != root) continue;
-        const int nr = ordered_compact(no, [&](int r) { return uf_find(lab, r) == root; },
-                                       [&](int r, int pos) { w.rmap[r] = pos; w.rlist[pos] = r; });
-        const int nc = ordered_compact(nt, [&](int c) { return uf_find(lab, no + c) == root; },
-                                       [&](int c, int pos) { w.cmap[c] = pos; w.clist[pos] = c; });
-        const bool tr = nr > nc;
-        const int hn = tr ? nc : nr, hm = tr ? nr : nc;
+        const int nr = block_compact(no, [&](int r) { return uf_find(lab, r) == root; },
+                                     [&](int r, int pos) { w.rmap[r] = pos; w.rlist[pos] = r; });
+        const int nc = block_compact(nt, [&](int c) { return uf_find(lab, no + c) == root; },
+                                     [&](int c, int pos) { w.cmap[c] = pos; w.clist[pos] = c; });
         const size_t a0 = (size_t)sh.scr_used;                           // the small components' scratch stays untouched
-        const size_t need = (size_t)hn * hm + (hn + 1) + 2 * (hm + 1) + (hm + 1) + (hm + 1) / 8 + 2;
-        if (a0 + need > (size_t)SCR_CAP) {
+        if (a0 + hungarian_scratch(nr, nc) > (size_t)SCR_CAP) {
             if (threadIdx.x == 0) atomicOr(&sh.overflow, 2);
             __syncthreads();
             continue;
         }
-        double* A = w.scr + a0;
-        for (size_t k = threadIdx.x; k < (size_t)hn * hm; k += NT) A[k] = 5000.;
-        __syncthreads();
-        for (int e = beg + threadIdx.x; e < end; e += NT) {
-            const int ri = w.rmap[w.es_r[e]], ci = w.cmap[w.es_c[e]];
-            const double cost = (double)(1.f - w.es_sim[e]);
-            if (tr) A[(size_t)ci * hm + ri] = cost; else A[(size_t)ri * hm + ci] = cost;
-        }
-        __syncthreads();
-        double* u = A + (size_t)hn * hm;
-        double* v = u + hn + 1;
-        double* minv = v + hm + 1;
-        int* p = (int*)(minv + hm + 1);
-        int* way = p + hm + 1;
-        unsigned char* used = (unsigned char*)(way + hm + 1);
-        hungarian_block<NT>(A, hn, hm, u, v, minv, p, way, used, sh.hs);
-        for (int j = 1 + threadIdx.x; j <= hm; j += NT) {
-            if (!p[j]) continue;
-            const int hi = p[j] - 1, hj = j - 1;
-            if (!(A[(size_t)hi * hm + hj] < 1.)) continue;
-            w.mr[tr ? w.rlist[hj] : w.rlist[hi]] = tr ? w.clist[hi] : w.clist[hj];
-        }
+        solve_dense_block<NT>(nr, nc, end - beg, [&](int i, int& ri, int& ci, double& cost) {
+            ri = w.rmap[w.es_r[beg + i]]; ci = w.cmap[w.es_c[beg + i]];
+            cost = (double)(1.f - w.es_sim[beg + i]);
+            return true;
+        }, 5000., 1., w.scr + a0, sh.hs, [&](int ri, int ci) { w.mr[w.rlist[ri]] = w.clist[ci]; });
         __syncthreads();
     }
     __syncthreads();

@@ -15,11 +15,12 @@
 // a pair beyond that has BEV IoU exactly 0 (no corner lies within the 1e-2 in-box margin, no edges cross), so only near pairs go
 // through bev_iou of boxgeom.cuh.  The reference's cost (1 - affinity, 5000 where cost >= 1, scipy linear_sum_assignment) makes
 // the optimum a maximum-cardinality matching of the valid edges with the least total cost; that objective separates over the
-// connected components of the valid-edge graph.  The components are labelled by min-hooking union-find; each one is solved
-// exactly (Hungarian with potentials of assign.cuh, float64 costs (double)(1.f - iou)).  A component of at most SMALL_EDGES edges (nearly all:
-// one detection and its track) is solved by one thread on its edges sorted by (row, column); a larger one (a chain of pedestrians,
-// a crowd) by the whole block, one component at a time, with the same arithmetic and tie rule.  The dense cost matrix of a
-// component lives in the per-sequence assignment scratch (SCR_CAP doubles, e.g. a 700 x 700 component).
+// connected components of the valid-edge graph.  The components are labelled by min-hooking union-find and their edges grouped
+// by root (uf_label, group_edges of assign.cuh); each one is solved exactly as a dense float64 cost matrix (double)(1.f - iou)
+// by the Hungarian method with potentials (solve_dense, solve_dense_block of assign.cuh).  A component of at most SMALL_EDGES
+// edges (nearly all: one detection and its track) is solved by one thread on its edges sorted by (row, column); a larger one (a
+// chain of pedestrians, a crowd) by the whole block, one component at a time, with the same arithmetic and tie rule.  The dense
+// cost matrix of a component lives in the per-sequence assignment scratch (SCR_CAP doubles, e.g. a 700 x 700 component).
 //
 // The ordered scans (the overlap filter, both merges, births) run on one thread over lists computed in parallel.
 //
@@ -39,10 +40,11 @@
 #include "common.cuh"
 #include "boxgeom.cuh"
 #include "assign.cuh"
+#include "eval_common.cuh"
 
 namespace {
 
-constexpr int NT = 512, NW = NT / 32;
+constexpr int NT = 512;
 constexpr int EDGE_CAP = 32768;            // association edges per call
 constexpr int MEDGE_CAP = 32768;           // merge edges per call
 constexpr int SCR_CAP = 1 << 19;           // float64 assignment scratch per sequence
@@ -71,18 +73,9 @@ struct Seq {
 
 struct Shared {
     int n_live, n_rlive, next_id, n_edges, n_medges, changed, overflow, f_used, r_used, scr_used, n_rows, n_cols, n_tmp, n_births;
-    int warp[NW + 1];
     int n_big;
     HungShared<NT> hs;                      // block-wide Hungarian
 };
-
-__device__ __forceinline__ float yawf(float y) {                      // transform_utils.yaw_filter, ndarray branch, float32
-    const float pi2 = 6.283185307179586f, pi = 3.141592653589793f;
-    if (fabsf(y) >= pi2) y = y - floorf(y / pi2) * pi2;
-    if (y > pi) y -= pi2;
-    if (y <= -pi) y += pi2;
-    return y;
-}
 
 __device__ __forceinline__ double yawd(double y) {
     const double pi2 = 6.283185307179586, pi = 3.141592653589793;
@@ -90,27 +83,6 @@ __device__ __forceinline__ double yawd(double y) {
     if (y > pi) y -= pi2;
     if (y <= -pi) y += pi2;
     return y;
-}
-
-// ordered block-wide compaction: out positions of the items i < n with pred(i) true, in index order; returns the count
-template <class Pred, class Emit>
-__device__ int block_compact(int n, Pred pred, Emit emit, Shared& sh) {
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    int total = 0;
-    for (int base = 0; base < n; base += NT) {
-        const int i = base + threadIdx.x;
-        const bool p = i < n && pred(i);
-        const unsigned b = __ballot_sync(0xffffffffu, p);
-        if (lane == 0) sh.warp[w] = __popc(b);
-        __syncthreads();
-        int before = 0, sum = 0;
-#pragma unroll
-        for (int k = 0; k < NW; ++k) { const int c = sh.warp[k]; before += k < w ? c : 0; sum += c; }
-        if (p) emit(i, total + before + __popc(b & ((1u << lane) - 1u)));
-        total += sum;
-        __syncthreads();
-    }
-    return total;
 }
 
 struct Frame {                      // one frame's detections in shared memory
@@ -183,7 +155,7 @@ __device__ void set_overflow(Shared& sh, int bit) { atomicOr(&sh.overflow, bit);
 __device__ void associate(Frame& fr, Seq& sq, Shared& sh, int n_rows, int n_cols, const double* thr) {
     for (int r = threadIdx.x; r < max(n_rows, fr.n); r += NT) { fr.match[r] = -1; fr.rcnt[r] = 0; }
     for (int v = threadIdx.x; v < n_rows + n_cols; v += NT) sq.lab[v] = v;
-    if (threadIdx.x == 0) { sh.n_edges = 0; }
+    if (threadIdx.x == 0) { sh.n_edges = 0; sh.scr_used = 0; }
     __syncthreads();
     if (n_rows == 0 || n_cols == 0) return;
     const long long pairs = (long long)n_rows * n_cols;
@@ -202,33 +174,10 @@ __device__ void associate(Frame& fr, Seq& sq, Shared& sh, int n_rows, int n_cols
     __syncthreads();
     const int ne = min(sh.n_edges, EDGE_CAP);
     if (ne == 0) return;
+    uf_label<NT>(sq.lab, ne, [&](int e) { return sq.e_r[e]; }, [&](int e) { return n_rows + sq.e_c[e]; }, sh.changed);
+    group_edges<NT>(sq.lab, ne, n_rows, fr.rcnt, sq.e_r, sq.e_c, sq.e_a, sq.es_r, sq.es_c, sq.es_a);
     volatile int* lab = sq.lab;
-    while (true) {                                   // min-hooking: the root of a component is its smallest row
-        if (threadIdx.x == 0) sh.changed = 0;
-        __syncthreads();
-        for (int e = threadIdx.x; e < ne; e += NT) {
-            const int a = uf_find(lab, sq.e_r[e]), b = uf_find(lab, n_rows + sq.e_c[e]);
-            if (a != b) { atomicMin(&sq.lab[max(a, b)], min(a, b)); sh.changed = 1; }
-        }
-        __syncthreads();
-        const int ch = sh.changed;
-        __syncthreads();
-        if (!ch) break;
-    }
-    for (int e = threadIdx.x; e < ne; e += NT) atomicAdd(&fr.rcnt[uf_find(lab, sq.e_r[e])], 1);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        int run = 0;
-        for (int r = 0; r < n_rows; ++r) { const int c = fr.rcnt[r]; fr.rcnt[r] = run; run += c; }
-        sh.scr_used = 0;
-    }
-    __syncthreads();
-    for (int e = threadIdx.x; e < ne; e += NT) {
-        const int root = uf_find(lab, sq.e_r[e]);
-        const int pos = atomicAdd(&fr.rcnt[root], 1);               // rcnt becomes the end offset of the component
-        sq.es_r[pos] = sq.e_r[e]; sq.es_c[pos] = sq.e_c[e]; sq.es_a[pos] = sq.e_a[e];
-    }
-    __syncthreads();
+    // cost (double)(1.f - iou), 5000 off the valid edges; a chosen pair is a match when its cost is below 1
     for (int root = threadIdx.x; root < n_rows; root += NT) {
         const int end = fr.rcnt[root], beg = root ? fr.rcnt[root - 1] : 0;
         if (end == beg || uf_find(lab, root) != root) continue;
@@ -238,20 +187,11 @@ __device__ void associate(Frame& fr, Seq& sq, Shared& sh, int n_rows, int n_cols
         const int m = end - beg;
         if (m == 1) { fr.match[er[0]] = ec[0]; continue; }
         if (m > SMALL_EDGES) continue;                              // solved block-wide below
-        for (int i = 1; i < m; ++i) {                               // sort by (row, column): a deterministic component
-            const int r = er[i], c = ec[i];
-            const float a = ea[i];
-            int j = i - 1;
-            while (j >= 0 && (er[j] > r || (er[j] == r && ec[j] > c))) { er[j + 1] = er[j]; ec[j + 1] = ec[j]; ea[j + 1] = ea[j]; --j; }
-            er[j + 1] = r; ec[j + 1] = c; ea[j + 1] = a;
-        }
-        // distinct rows (sorted already) and columns
-        int nr = 0;
-        for (int i = 0; i < m; ++i) nr += (i == 0 || er[i] != er[i - 1]);
-        const int need = 3 * m + 8;                                 // columns list, in doubles (ints fit)
+        sort_edges(er, ec, ea, m);
+        const int need = 3 * m + 8;                                 // rows and columns lists, in doubles (ints fit)
         const int base = atomicAdd(&sh.scr_used, need);
         if (base + need > SCR_CAP) { set_overflow(sh, 8); continue; }
-        int* cols = (int*)(sq.scr + base);
+        int* cols = (int*)(sq.scr + base);                          // distinct columns, ascending
         int nc = 0;
         for (int i = 0; i < m; ++i) {
             const int c = ec[i];
@@ -261,43 +201,25 @@ __device__ void associate(Frame& fr, Seq& sq, Shared& sh, int n_rows, int n_cols
             for (int k = nc; k > j + 1; --k) cols[k] = cols[k - 1];
             cols[j + 1] = c; ++nc;
         }
-        int* rows = cols + nc;
-        nr = 0;
+        int* rows = cols + nc;                                      // distinct rows (sorted already)
+        int nr = 0;
         for (int i = 0; i < m; ++i) if (i == 0 || er[i] != er[i - 1]) rows[nr++] = er[i];
-        const bool tr = nr > nc;                                    // Hungarian rows = the smaller side
-        const int hn = tr ? nc : nr, hm = tr ? nr : nc;
-        const int need2 = hn * hm + 3 * (hm + 1) + (hn + 1) + 3 * (hm + 1) / 2 + 8;
+        const int need2 = (int)hungarian_scratch(nr, nc);
         const int base2 = atomicAdd(&sh.scr_used, need2);
         if (base2 + need2 > SCR_CAP) { set_overflow(sh, 8); continue; }
-        double* A = sq.scr + base2;
-        for (int k = 0; k < hn * hm; ++k) A[k] = 5000.;
-        for (int i = 0; i < m; ++i) {
-            int ri = 0, ci = 0;
+        solve_dense(nr, nc, m, [&](int i, int& ri, int& ci, double& cost) {
+            ri = 0; ci = 0;
             while (rows[ri] != er[i]) ++ri;
             while (cols[ci] != ec[i]) ++ci;
-            const double cost = (double)(1.f - ea[i]);
-            if (tr) A[(size_t)ci * hm + ri] = cost; else A[(size_t)ri * hm + ci] = cost;
-        }
-        double* u = A + hn * hm;
-        double* v = u + hn + 1;
-        double* minv = v + hm + 1;
-        int* p = (int*)(minv + hm + 1);
-        int* way = p + hm + 1;
-        unsigned char* used = (unsigned char*)(way + hm + 1);
-        hungarian(A, hn, hm, u, v, minv, p, way, used);
-        for (int j = 1; j <= hm; ++j) {
-            if (!p[j]) continue;
-            const int hi = p[j] - 1, hj = j - 1;
-            if (!(A[(size_t)hi * hm + hj] < 1.)) continue;
-            const int r = tr ? rows[hj] : rows[hi], c = tr ? cols[hi] : cols[hj];
-            fr.match[r] = c;
-        }
+            cost = (double)(1.f - ea[i]);
+            return true;
+        }, 5000., 1., sq.scr + base2, [&](int ri, int ci) { fr.match[rows[ri]] = cols[ci]; });
     }
     __syncthreads();
     // large components (a chain of pedestrians, a crowd): one at a time, the whole block on each
     const int nbig = block_compact(n_rows, [&](int r) {
         const int m = fr.rcnt[r] - (r ? fr.rcnt[r - 1] : 0);
-        return m > SMALL_EDGES && uf_find(lab, r) == r; }, [&](int r, int pos) { fr.big[pos] = r; }, sh);
+        return m > SMALL_EDGES && uf_find(lab, r) == r; }, [&](int r, int pos) { fr.big[pos] = r; });
     for (int b = 0; b < nbig; ++b) {
         const int root = fr.big[b], end = fr.rcnt[root], beg = root ? fr.rcnt[root - 1] : 0;
         const int base = sh.scr_used;                               // the small components' scratch stays untouched
@@ -306,41 +228,20 @@ __device__ void associate(Frame& fr, Seq& sq, Shared& sh, int n_rows, int n_cols
         int* rlist = cmap + n_cols;
         int* clist = rlist + n_rows;
         const int nr = block_compact(n_rows, [&](int r) { return uf_find(lab, r) == root; },
-                                     [&](int r, int pos) { rmap[r] = pos; rlist[pos] = r; }, sh);
+                                     [&](int r, int pos) { rmap[r] = pos; rlist[pos] = r; });
         const int nc = block_compact(n_cols, [&](int c) { return uf_find(lab, n_rows + c) == root; },
-                                     [&](int c, int pos) { cmap[c] = pos; clist[pos] = c; }, sh);
-        const bool tr = nr > nc;
-        const int hn = tr ? nc : nr, hm = tr ? nr : nc;
+                                     [&](int c, int pos) { cmap[c] = pos; clist[pos] = c; });
         const size_t a0 = base + (size_t)(2 * n_rows + 2 * n_cols + 1) / 2 + 1;
-        const size_t need = (size_t)hn * hm + (hn + 1) + 2 * (hm + 1) + (hm + 1) + (hm + 1) / 8 + 2;
-        if (a0 + need > (size_t)SCR_CAP) {
+        if (a0 + hungarian_scratch(nr, nc) > (size_t)SCR_CAP) {
             if (threadIdx.x == 0) set_overflow(sh, 8);
             __syncthreads();
             continue;
         }
-        double* A = sq.scr + a0;
-        for (size_t k = threadIdx.x; k < (size_t)hn * hm; k += NT) A[k] = 5000.;
-        __syncthreads();
-        for (int e = beg + threadIdx.x; e < end; e += NT) {
-            const int ri = rmap[sq.es_r[e]], ci = cmap[sq.es_c[e]];
-            const double cost = (double)(1.f - sq.es_a[e]);
-            if (tr) A[(size_t)ci * hm + ri] = cost; else A[(size_t)ri * hm + ci] = cost;
-        }
-        __syncthreads();
-        double* u = A + (size_t)hn * hm;
-        double* v = u + hn + 1;
-        double* minv = v + hm + 1;
-        int* p = (int*)(minv + hm + 1);
-        int* way = p + hm + 1;
-        unsigned char* used = (unsigned char*)(way + hm + 1);
-        hungarian_block<NT>(A, hn, hm, u, v, minv, p, way, used, sh.hs);
-        for (int j = 1 + threadIdx.x; j <= hm; j += NT) {
-            if (!p[j]) continue;
-            const int hi = p[j] - 1, hj = j - 1;
-            if (!(A[(size_t)hi * hm + hj] < 1.)) continue;
-            const int r = tr ? rlist[hj] : rlist[hi], c = tr ? clist[hi] : clist[hj];
-            fr.match[r] = c;
-        }
+        solve_dense_block<NT>(nr, nc, end - beg, [&](int i, int& ri, int& ci, double& cost) {
+            ri = rmap[sq.es_r[beg + i]]; ci = cmap[sq.es_c[beg + i]];
+            cost = (double)(1.f - sq.es_a[beg + i]);
+            return true;
+        }, 5000., 1., sq.scr + a0, sh.hs, [&](int ri, int ci) { fr.match[rlist[ri]] = clist[ci]; });
         __syncthreads();
     }
 }
@@ -490,51 +391,39 @@ struct DzTrackOut {
     int* overflow;            // (S)
 };
 
-static size_t seq_ws_bytes(int F, int K, int T, int E) {
-    size_t b = 0;
-    auto add = [&](size_t n) { b += dz_align_up(n, 256); };
-    add((size_t)T * (5 + 3 + 1 + 9 + 7) * 8); add((size_t)T * (25 + 2 + 2) * 4); add((size_t)T * 4 * 4);
-    add((size_t)T * 4 * 3);
-    add((size_t)2 * T * 7 * 4); add((size_t)2 * T * 4 * 2); add((size_t)(K + 2 * T) * 4); add(4);
-    add((size_t)EDGE_CAP * 4 * 6);
-    add((size_t)MEDGE_CAP * 4 * 3); add((size_t)2 * T * 4 * 2); add((size_t)2 * T * 2);
-    add((size_t)SCR_CAP * 8);
-    add((size_t)E * (4 + 4 + 4 + 72)); add((size_t)(F + 1) * 4); add((size_t)E * 12); add((size_t)(F + 1) * 4);
-    add((size_t)T * 16);
-    return b + 256;
-}
-
-__host__ __device__ inline char* take_bytes(char*& p, size_t n) { char* r = p; p += (n + 255) / 256 * 256; return r; }
-
-__device__ Seq carve(char* base, int F, int K, int T, int E) {
+// one sequence's workspace; carved from a null base it only sizes it (seq_ws_bytes)
+__host__ __device__ Seq carve(DzCarve& c, int F, int K, int T, int E) {
     Seq s;
-    char* p = base;
-#define take(n) take_bytes(p, (n))
-    s.x = (double*)take((size_t)T * (5 + 3 + 1 + 9 + 7) * 8);
+    s.x = c.take<double>((size_t)T * (5 + 3 + 1 + 9 + 7));
     s.size = s.x + (size_t)T * 5; s.head = s.size + (size_t)T * 3; s.box = s.head + T; s.birth = s.box + (size_t)T * 9;
-    s.P = (float*)take((size_t)T * (25 + 2 + 2) * 4);
+    s.P = c.take<float>((size_t)T * (25 + 2 + 2));
     s.q = s.P + (size_t)T * 25; s.score = s.q + (size_t)T * 2; s.rscore = s.score + T;
-    s.cls = (int*)take((size_t)T * 4 * 4); s.hit = s.cls + T; s.first = s.hit + T; s.rhit = s.first + T;
-    s.live = (int*)take((size_t)T * 4 * 3); s.live2 = s.live + T; s.rlive = s.live2 + T;
-    s.cbox = (float*)take((size_t)2 * T * 7 * 4);
-    s.ccls = (int*)take((size_t)2 * T * 4 * 2); s.cref = s.ccls + 2 * T;
-    s.lab = (int*)take((size_t)(K + 2 * T) * 4);
-    s.cnt = (int*)take(4);
-    s.e_r = (int*)take((size_t)EDGE_CAP * 4 * 6);
+    s.cls = c.take<int>((size_t)T * 4); s.hit = s.cls + T; s.first = s.hit + T; s.rhit = s.first + T;
+    s.live = c.take<int>((size_t)T * 3); s.live2 = s.live + T; s.rlive = s.live2 + T;
+    s.cbox = c.take<float>((size_t)2 * T * 7);
+    s.ccls = c.take<int>((size_t)2 * T * 2); s.cref = s.ccls + 2 * T;
+    s.lab = c.take<int>((size_t)K + 2 * T);
+    s.cnt = c.take<int>(1);
+    s.e_r = c.take<int>((size_t)EDGE_CAP * 6);
     s.e_c = s.e_r + EDGE_CAP; s.es_r = s.e_c + EDGE_CAP; s.es_c = s.es_r + EDGE_CAP;
     s.e_a = (float*)(s.es_c + EDGE_CAP); s.es_a = s.e_a + EDGE_CAP;
-    s.m_i = (int*)take((size_t)MEDGE_CAP * 4 * 3); s.m_j = s.m_i + MEDGE_CAP; s.madj = s.m_j + MEDGE_CAP;
-    s.mcnt = (int*)take((size_t)2 * T * 4 * 2); s.moff = s.mcnt + 2 * T;
-    s.interesting = (unsigned char*)take((size_t)2 * T * 2); s.dep = s.interesting + 2 * T;
-    s.scr = (double*)take((size_t)SCR_CAP * 8);
-    char* fe = take((size_t)E * (4 + 4 + 4 + 72));
-    s.f_box = (double*)fe; s.f_id = (int*)(s.f_box + (size_t)E * 9); s.f_hit = s.f_id + E; s.f_score = (float*)(s.f_hit + E);
-    s.f_off = (int*)take((size_t)(F + 1) * 4);
-    s.r_id = (int*)take((size_t)E * 12); s.r_hit = s.r_id + E; s.r_score = (float*)(s.r_hit + E);
-    s.r_off = (int*)take((size_t)(F + 1) * 4);
-    s.pcnt = (int*)take((size_t)T * 16); s.plo = s.pcnt + T; s.phi = s.plo + T; s.poff = s.phi + T;
-#undef take
+    s.m_i = c.take<int>((size_t)MEDGE_CAP * 3); s.m_j = s.m_i + MEDGE_CAP; s.madj = s.m_j + MEDGE_CAP;
+    s.mcnt = c.take<int>((size_t)2 * T * 2); s.moff = s.mcnt + 2 * T;
+    s.interesting = c.take<unsigned char>((size_t)2 * T * 2); s.dep = s.interesting + 2 * T;
+    s.scr = c.take<double>(SCR_CAP);
+    s.f_box = (double*)c.take<char>((size_t)E * (4 + 4 + 4 + 72));
+    s.f_id = (int*)(s.f_box + (size_t)E * 9); s.f_hit = s.f_id + E; s.f_score = (float*)(s.f_hit + E);
+    s.f_off = c.take<int>((size_t)F + 1);
+    s.r_id = c.take<int>((size_t)E * 3); s.r_hit = s.r_id + E; s.r_score = (float*)(s.r_hit + E);
+    s.r_off = c.take<int>((size_t)F + 1);
+    s.pcnt = c.take<int>((size_t)T * 4); s.plo = s.pcnt + T; s.phi = s.plo + T; s.poff = s.phi + T;
     return s;
+}
+
+static size_t seq_ws_bytes(int F, int K, int T, int E) {
+    DzCarve c(nullptr);
+    carve(c, F, K, T, E);
+    return c.bytes + 256;
 }
 
 __global__ void __launch_bounds__(NT, 1)
@@ -558,7 +447,8 @@ k_track_sequences(const float* __restrict__ boxes, const int* __restrict__ count
         fr.big = (int*)p; p += (size_t)K * 4;
         fr.kept = p;
     }
-    Seq sq = carve(ws + (size_t)s * seq_bytes, F, K, T, E);
+    DzCarve wc(ws + (size_t)s * seq_bytes);
+    Seq sq = carve(wc, F, K, T, E);
     const int Fs = min(max(num_frames[s], 0), F);
     if (threadIdx.x == 0) {
         sh.n_live = sh.n_rlive = sh.next_id = 0; sh.overflow = 0; sh.f_used = sh.r_used = 0;
@@ -610,7 +500,7 @@ k_track_sequences(const float* __restrict__ boxes, const int* __restrict__ count
         for (int b = threadIdx.x; b < nbk; b += NT) sq.live2[b] = fr.rcnt[b];       // park the birth list
         __syncthreads();
         const int nc2 = block_compact(nl, [&](int k) { return sq.ccls[k] >= 0; },
-                                      [&](int k, int pos) { sq.mcnt[pos] = k; }, sh);
+                                      [&](int k, int pos) { sq.mcnt[pos] = k; });
         // mcnt holds the live positions of the stage-2 columns; copy their boxes into column slots nl..nl+nc2
         for (int k = threadIdx.x; k < nc2; k += NT) {
             const int c = sq.mcnt[k], id = sq.live[c];
@@ -644,7 +534,7 @@ k_track_sequences(const float* __restrict__ boxes, const int* __restrict__ count
         for (int k = threadIdx.x; k < nl2; k += NT) { const int id = sq.live[k]; box_to_col(sq, k, sq.box + (size_t)id * 9, sq.cls[id], id); }
         __syncthreads();
         merge(sq, sh, sq.live, nl2, pr);
-        const int nl3 = block_compact(nl2, [&](int k) { return !sq.dep[k]; }, [&](int k, int pos) { sq.live2[pos] = sq.live[k]; }, sh);
+        const int nl3 = block_compact(nl2, [&](int k) { return !sq.dep[k]; }, [&](int k, int pos) { sq.live2[pos] = sq.live[k]; });
         // emit the forward entries of this frame
         const int base = sh.f_used;
         const int ne = min(nl3, E - base);
@@ -680,7 +570,7 @@ k_track_sequences(const float* __restrict__ boxes, const int* __restrict__ count
                                       [&](int k, int pos) {
                                           const int e = eb + k;
                                           box_to_col(sq, nrv + pos, sq.f_box + (size_t)e * 9, sq.cls[sq.f_id[e]], -1);
-                                      }, sh);
+                                      });
         if (threadIdx.x == 0) {
             int nr = 0;
             for (int i = 0; i < n; ++i) if (fr.kept[i] && !((double)fr.score[i] >= pr.score[fr.cls[i] - 1])) fr.rows[nr++] = i;
@@ -697,7 +587,7 @@ k_track_sequences(const float* __restrict__ boxes, const int* __restrict__ count
         }
         __syncthreads();
         merge(sq, sh, sq.rlive, nrv, pr);
-        const int nrv2 = block_compact(nrv, [&](int k) { return !sq.dep[k]; }, [&](int k, int pos) { sq.live2[pos] = sq.rlive[k]; }, sh);
+        const int nrv2 = block_compact(nrv, [&](int k) { return !sq.dep[k]; }, [&](int k, int pos) { sq.live2[pos] = sq.rlive[k]; });
         const int base = sh.r_used;
         const int ne = min(nrv2, E - base);
         for (int k = threadIdx.x; k < nrv2; k += NT) {
@@ -711,7 +601,7 @@ k_track_sequences(const float* __restrict__ boxes, const int* __restrict__ count
                                       [&](int k, int pos) {
                                           const int e = eb + k, id = sq.f_id[e];
                                           sq.rlive[nrv2 + pos] = id; sq.rscore[id] = sq.f_score[e]; sq.rhit[id] = 1;
-                                      }, sh);
+                                      });
         if (threadIdx.x == 0) {
             if (ne < nrv2) set_overflow(sh, 2);
             sq.r_off[f] = base; sh.r_used = base + ne; sh.n_rlive = nrv2 + nsp;
@@ -736,7 +626,7 @@ k_track_sequences(const float* __restrict__ boxes, const int* __restrict__ count
     __syncthreads();
     // surviving ids in id order; their entry offsets by a running sum (thread 0 handles the scan over the compacted list)
     const int nsurv = block_compact(nid, [&](int id) { return sq.pcnt[id] >= pr.least_age; },
-                                    [&](int id, int pos) { sq.poff[pos] = id; }, sh);
+                                    [&](int id, int pos) { sq.poff[pos] = id; });
     if (threadIdx.x == 0) {
         int run = 0;
         for (int k = 0; k < nsurv; ++k) {
