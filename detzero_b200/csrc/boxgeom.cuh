@@ -8,7 +8,13 @@
 
 struct P2 { float x, y; };
 
-__device__ __forceinline__ float cross_o(P2 a, P2 b, P2 o) { return (a.x - o.x) * (b.y - o.y) - (b.x - o.x) * (a.y - o.y); }
+// Both products are rounded before the difference (no FMA contraction), so cross_o(a, b, o) == -cross_o(b, a, o) exactly.
+// seg_hit relies on it: s1 * s2 > 0 must imply that s1 and s5 = -s2 have opposite signs, which keeps the crossing point between
+// q0 and q1.  With a contracted product the two sides of two collinear edges (abutting boxes, boxes turned by k*pi/2) come out
+// as unrelated rounding noise, and the crossing point can land metres outside both boxes.
+__device__ __forceinline__ float cross_o(P2 a, P2 b, P2 o) {
+    return __fsub_rn(__fmul_rn(a.x - o.x, b.y - o.y), __fmul_rn(b.x - o.x, a.y - o.y));
+}
 
 __device__ __forceinline__ bool seg_hit(P2 p1, P2 p0, P2 q1, P2 q0, P2& out) {
     bool bb = fminf(p0.x, p1.x) <= fmaxf(q0.x, q1.x) && fminf(q0.x, q1.x) <= fmaxf(p0.x, p1.x) &&

@@ -394,15 +394,16 @@ extern "C" int dz_nms_bev(const float* boxes, const float* scores, const int32_t
     cudaStream_t st = (cudaStream_t)stream;
     int col_blocks = (cap + 63) / 64;
     unsigned long long* mask = (unsigned long long*)ws;
-    dim3 grid(col_blocks, dz_cdiv(cap, 8), B);
-    k_nms_mask<<<grid, 256, 0, st>>>(boxes, d_n, cap, thresh, mask);
+    // refuse an unsupported cap before anything is enqueued: a rejected call leaves the workspace and the outputs as they were
     size_t smem = (size_t)cap * col_blocks * 8 + (size_t)cap * 4;
+    if (smem > 200 * 1024) { dz_set_error("dz_nms_bev: cap too large for shared-memory scan"); return DZ_ERR_UNSUPPORTED; }
     static bool configured = false;
     if (!configured) {
         DZ_CUDA(cudaFuncSetAttribute(k_nms_scan, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
         configured = true;
     }
-    if (smem > 200 * 1024) { dz_set_error("dz_nms_bev: cap too large for shared-memory scan"); return DZ_ERR_UNSUPPORTED; }
+    dim3 grid(col_blocks, dz_cdiv(cap, 8), B);
+    k_nms_mask<<<grid, 256, 0, st>>>(boxes, d_n, cap, thresh, mask);
     k_nms_scan<<<B, 256, smem, st>>>(boxes, scores, labels, d_n, cap, mask, post_max, label_offset, out, d_out_n);
     DZ_LAUNCH_CHECK();
     return DZ_OK;

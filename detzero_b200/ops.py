@@ -482,8 +482,9 @@ def boxes_iou_bev(a, b):
     a = a[:, :7].contiguous().float()
     b = b[:, :7].contiguous().float()
     out = torch.empty((a.shape[0], b.shape[0]), dtype=torch.float32, device=a.device)
-    check(lib().dz_boxes_iou_bev(_p(a), a.shape[0], _p(b), b.shape[0], _p(out), _stream()), 'boxes_iou_bev')
-    _count(1)
+    if a.shape[0] and b.shape[0]:                      # an empty tensor has no data pointer
+        check(lib().dz_boxes_iou_bev(_p(a), a.shape[0], _p(b), b.shape[0], _p(out), _stream()), 'boxes_iou_bev')
+        _count(1)
     return out
 
 
