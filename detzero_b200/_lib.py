@@ -97,6 +97,8 @@ _SIGS = {
     'dz_attention_fwd': (ci, [vp, ci, vp, ci, vp, ci, vp, ci, ci, ci, ci, ci, vp, ci, ci, vp]),
     'dz_layernorm_residual': (ci, [vp, vp, vp, vp, cf, ci, ci, vp, vp]),
     'dz_add': (ci, [vp, vp, sz, vp, vp]),
+    'dz_crm_point_ws_bytes': (sz, [ci]),
+    'dz_crm_point_pass': (ci, [ci, ci, vp, ci, ci, ci] + [vp] * 17 + [sz, vp]),
 }
 
 

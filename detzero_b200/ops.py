@@ -611,3 +611,19 @@ def add(a, b):
     check(lib().dz_add(_p(a), _p(b), a.numel(), _p(out), _stream()), 'add')
     _count(1)
     return out
+
+
+def crm_point_pass(pass_, mode, x, P, wf, wb, tab, shift4=None, sel=None, dsel=None, zext=None, iext=None, csum=None, stats=None,
+                   slab=None):
+    """one pass of the train-mode CRM point encoders (see dz_crm_point_pass).  x (crops*P, c0); wf = (w1t, w2t, w3t, w4pt) forward
+    weights transposed, wb = (w2, w3, w4p) as stored, all fp32 contiguous; outputs are caller-allocated"""
+    _need_cuda(x, tab)
+    rows, c0 = x.shape
+    crops = rows // P
+    assert crops * P == rows
+    ws = workspace(lib().dz_crm_point_ws_bytes(crops), x.device, 'crm_point')
+    check(lib().dz_crm_point_pass(int(pass_), int(mode), _p(_f32c(x)), crops, int(P), c0, *[_p(_f32c(w)) for w in wf],
+                                  *[_p(_f32c(w)) for w in wb], _p(_f32c(tab)), _p(shift4), _p(sel), _p(dsel), _p(zext), _p(iext),
+                                  _p(csum), _p(stats), _p(slab), _p(ws), ws.numel(), _stream()), 'crm_point_pass')
+    _count(2 + (slab is not None))
+    return stats

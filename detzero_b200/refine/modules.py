@@ -12,15 +12,17 @@ token-major on libdetzero_b200:
 Layout: activations are (tokens, channels) row-major; the reference's (B,C,P) <-> (P,B,C) permute copies disappear.
 Every 1x1 Conv / Linear (+BatchNorm eval +ReLU) is one fused GEMM launch; attention streams keys with an online
 softmax and never materialises the (B*H, Pq, Pk) score tensor; the query scaling head_dim**-0.5 is folded into the
-in-projection epilogue.  Eval only (training is a next row, SURVEY.md §8f)."""
+in-projection epilogue.  ConfidencePointnet also trains (refine/train.py); the PRM and GRM are eval only."""
 import copy
 import math
 
 import numpy as np
 import torch
 import torch.nn as nn
+import torch.nn.functional as F
 
 from .. import _lib, ops
+from . import train
 from ..spconv.pytorch import fold_bn
 
 
@@ -81,6 +83,17 @@ def _first_group(mods, i=0):
     j = i + (2 if bn is not None else 1)
     relu = j < len(mods) and isinstance(mods[j], nn.ReLU)
     return m, bn, relu, j + (1 if relu else 0)
+
+
+def _train_mlp(seq, x):
+    """train-mode Conv1d(k=1) / BatchNorm1d / ReLU stack on token-major (rows, C) input through torch autograd: F.linear, not cuDNN
+    Conv1d, so that it follows torch.backends.cuda.matmul.allow_tf32 (off by default) rather than cuDNN's TF32 default"""
+    for m in seq:
+        if isinstance(m, nn.Conv1d):
+            x = F.linear(x, m.weight.squeeze(-1), m.bias)
+        else:
+            x = m(x)
+    return x
 
 
 def run_mlp_concat(seq, glob, per, gsize, mode, glob_first=True, pool=None):
@@ -342,7 +355,7 @@ class GeometryHead(_HeadBase):
 
 
 class TargetAssigner:
-    """decode half of target_assign.py (:73-104)"""
+    """decode half of target_assign.py (:73-104) and its confidence-mode encode (:55-70)"""
 
     def __init__(self, anchor_sizes=None, mode='size', **kwargs):
         self.anchor_sizes = anchor_sizes
@@ -350,6 +363,16 @@ class TargetAssigner:
         self.mode = mode
         self.dir_bin_num = 12
         self.anchor_angles = torch.arange(self.dir_bin_num, dtype=torch.float) * (2 * np.pi / self.dir_bin_num) - np.pi
+        self.score_thresh = kwargs.get('score_thresh', [0.25, 0.5])
+
+    def encode_torch(self, data_dict):
+        """confidence mode: iou clamped to [0, 1]; negatives iou < th0, positives iou >= th1, the boxes between masked out.  A padded
+        box (iou = -1) clamps to 0 and so enters the loss as a negative, as in the reference"""
+        if self.mode != 'confidence':
+            raise NotImplementedError('TargetAssigner.encode_torch: only the confidence mode is implemented (CRM training)')
+        iou = torch.clamp(data_dict['iou'], 0, 1).reshape(-1)
+        pos = iou >= self.score_thresh[1]
+        return {'score_gt': pos.to(iou.dtype), 'iou_gt': iou, 'mask': (iou < self.score_thresh[0]) | pos}
 
     def decode_torch(self, preds, data_dict):
         if self.mode == 'geometry':
@@ -487,11 +510,51 @@ class ConfidencePointnet(nn.Module):
         self.regression_mlp = make_fc_layers(model_cfg.REGRESSION_MLP, E * 2, E, True)
         self.heads = nn.ModuleDict({t: make_fc_layers([int(E / 2)], E, 1, False) for t in ('score_reg', 'iou_reg')})
         self.preds_dict = {}
+        self.targets_dict = {}
+        self.score_thresh = model_cfg.get('SCORE_THRESH', [0.25, 0.5])
+        self.loss_weight = [1.0, 1.0]
+        self.target_assigner = TargetAssigner(mode='confidence', score_thresh=self.score_thresh)
 
-    @torch.no_grad()
     def forward(self, data_dict):
         if self.training:
-            raise NotImplementedError('refiner training is a next row (SURVEY.md §8f)')
+            return self.forward_train(data_dict)
+        return self.forward_eval(data_dict)
+
+    def forward_train(self, data_dict):
+        """confidence_pointnet.py:80-108 in training: the point encoders on the device (refine/train.py), the per-box part through
+        autograd on this module's own layers, token-major ((B*L, C) rows: BatchNorm1d takes the same statistics as on (B, C, L))"""
+        if self.mode == _lib.DZ_F32 and torch.backends.cuda.matmul.allow_tf32:
+            raise RuntimeError('ConfidencePointnet with COMPUTE_MODE fp32 trains in fp32, but torch.backends.cuda.matmul.allow_tf32 is '
+                               'set: the per-box layers would run TF32')
+        pts = data_dict['conf_points'].float()
+        B, L, P, C = pts.shape
+        E = self.embed_dims
+        pool = train.point_encoders(self, pts)                                          # (B*L, E)
+        tap = _train_mlp(self.pts_mlp, pool)                                            # pts_mlp[5] == the stack's output
+        gg = tap.view(B, L, E).max(dim=1)[0]
+        out = _train_mlp(self.regression_mlp, torch.cat([gg.unsqueeze(1).expand(B, L, E), tap.view(B, L, E)], dim=2).reshape(B * L, 2 * E))
+        preds = {t: torch.sigmoid(_train_mlp(self.heads[t], out).view(B, L, 1)) for t in ('score_reg', 'iou_reg')}
+        self.preds_dict.update(preds)
+        self.targets_dict.update(self.target_assigner.encode_torch(data_dict))
+        return data_dict
+
+    def get_loss(self, tb_dict=None):
+        """confidence_pointnet.py:115-150: BCE (log clamped at -100) summed over the mask / the mask count, score and iou heads"""
+        tb_dict = {} if tb_dict is None else tb_dict
+        mask = self.targets_dict['mask']
+        n = mask.sum()
+        bin_cls_loss = F.binary_cross_entropy(self.preds_dict['score_reg'].reshape(-1)[mask], self.targets_dict['score_gt'][mask],
+                                              reduction='none').sum() / n
+        iou_loss = F.binary_cross_entropy(self.preds_dict['iou_reg'].reshape(-1)[mask], self.targets_dict['iou_gt'][mask],
+                                          reduction='none').sum() / n
+        w1, w2 = self.loss_weight
+        conf_loss = bin_cls_loss * w1 + iou_loss * w2
+        tb_dict.update({'bin_cls_loss': bin_cls_loss, 'iou_loss': iou_loss})
+        tb_dict['confidence_loss'] = conf_loss
+        return conf_loss, tb_dict
+
+    @torch.no_grad()
+    def forward_eval(self, data_dict):
         pts = data_dict['conf_points'].float()
         B, L, P, C = pts.shape
         mode = self.mode
@@ -514,7 +577,7 @@ refine_modules = {'GeometryTransformer': GeometryTransformer, 'PositionTransform
 
 
 class RefineTemplate(nn.Module):
-    """refine_template.py:18-77 (eval path): builds ``self.reg`` by NAME from the config"""
+    """refine_template.py:18-77: builds ``self.reg`` by NAME from the config"""
 
     def __init__(self, model_cfg, dataset=None):
         super().__init__()
@@ -526,8 +589,21 @@ class RefineTemplate(nn.Module):
             model_cfg=model_cfg.REGRESSION, query_point_dims=model_cfg.get('QUERY_POINT_DIMS', 0),
             memory_point_dims=model_cfg.get('MEMORY_POINT_DIMS', 0)))
 
+    def update_global_step(self):
+        self.global_step += 1
+
+    def get_training_loss(self):
+        """refine_template.py:52-62"""
+        disp_dict = {}
+        loss, tb_dict = self.reg.get_loss({})
+        tb_dict['full_loss'] = loss
+        return loss, tb_dict, disp_dict
+
     def forward(self, data_dict):
         data_dict = self.reg(data_dict)
+        if self.training:
+            loss, tb_dict, disp_dict = self.get_training_loss()
+            return {'loss': loss}, tb_dict, disp_dict
         key = 'pred_score' if 'pred_score' in data_dict else 'batch_box_preds'
         return {('pred_score' if key == 'pred_score' else 'pred_boxes'): data_dict[key]}, {}, {}
 

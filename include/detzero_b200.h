@@ -464,6 +464,23 @@ int dz_group_max(const float* x, int G, int group, int C, float* y, dz_stream_t 
 int dz_attention_fwd(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv,
                      const unsigned char* key_padding_mask, int B, int Pq, int Pk, int H, int dh, float* out,
                      int ldo, int mode, dz_stream_t stream);
+/* ConfidencePointnet point encoders in TRAIN mode, forward and backward, recomputing the point layers tile by tile instead of storing
+ * them (confidence_pointnet.py:80-92 with BatchNorm2d batch statistics, and the autograd backward of those lines).  One pass over the
+ * x (crops*P, c0) point rows, P % 64 == 0, c0 % 8 == 0 and <= 64, layers c0 -> 128 -> 128 -> 256 and [g | y2] 384 -> 256:
+ *   1..4  sums of z_l and z_l^2 of layer l -> stats[0..256), stats[256..512) (float64); 3 and 4 also: zext / iext (2, crops, 256) the
+ *         max / min z over each crop and their lowest row in the crop; 4 also csum (crops, 256), the crop sums of z4
+ *   5     slab (2, 256, 128) = dW4p, dW3 (float64); stats = sum dh2, sum dh2 * xhat2
+ *   6     slab (128, 128) = dW2; stats = sum dh1, sum dh1 * xhat1
+ *   7     slab (128, c0) = dW1
+ * w*t: forward weights transposed (K x N); w2, w3, w4p: as stored (N x K), w4p = the last 128 input columns of pts_encoder_2's weight.
+ * tab (4, 6, 256): per layer and channel [a = gamma*rstd, b = beta - mean*a, mean, rstd, m1 = sum dh / N, m2 = sum dh*xhat / N];
+ * shift4 (crops, 256) = g W4g^T; sel / dsel (2, crops, 256): the pooled row and dL/dh there, layer 3 then layer 4.  Partials are
+ * per CTA and reduced in a fixed order: the same inputs give the same bits.  mode DZ_F32 (fp32 FMA) or DZ_TF32 (TF32 tensor cores). */
+size_t dz_crm_point_ws_bytes(int crops);
+int dz_crm_point_pass(int pass, int mode, const float* x, int crops, int P, int c0, const float* w1t, const float* w2t,
+                      const float* w3t, const float* w4pt, const float* w2, const float* w3, const float* w4p, const float* tab,
+                      const float* shift4, const int* sel, const float* dsel, float* zext, int* iext, double* csum, double* stats,
+                      double* slab, void* ws, size_t ws_bytes, dz_stream_t stream);
 /* y = LayerNorm(x + r) * gamma + beta over the last dim C (decoder.py:73-75,85-90) ; r may be NULL */
 int dz_layernorm_residual(const float* x, const float* r, const float* gamma, const float* beta, float eps,
                           int M, int C, float* y, dz_stream_t stream);
