@@ -636,6 +636,7 @@ class ConfidencePointnet(nn.Module):
         self.score_thresh = model_cfg.get('SCORE_THRESH', [0.25, 0.5])
         self.loss_weight = [1.0, 1.0]
         self.target_assigner = TargetAssigner(mode='confidence', score_thresh=self.score_thresh)
+        self.pooled_rows = {}           # the rows the last training step's max-pools picked: 'enc1', 'enc2' (B*L, 256)
 
     def forward(self, data_dict):
         if self.training:

@@ -25,11 +25,12 @@ def _bn_update(bn, mean, var, n):
 
 
 class CrmPointEncoders(torch.autograd.Function):
-    """x (crops*P, c0) -> (crops, 256).  Arguments after ``bns`` (the four BatchNorm2d modules, whose running statistics the forward
-    updates): per layer the conv weight, BN weight and BN bias."""
+    """x (crops*P, c0) -> (crops, 256).  ``rows`` (a dict) receives the pooled row of each (crop, channel) under 'enc1' and 'enc2'.
+    Arguments after ``bns`` (the four BatchNorm2d modules, whose running statistics the forward updates): per layer the conv weight,
+    BN weight and BN bias."""
 
     @staticmethod
-    def forward(ctx, x, P, mode, bns, w1, g1, b1, w2, g2, b2, w3, g3, b3, w4, g4, b4):
+    def forward(ctx, x, P, mode, rows, bns, w1, g1, b1, w2, g2, b2, w3, g3, b3, w4, g4, b4):
         R, c0 = x.shape
         crops, dev = R // P, x.device
         W1, W2, W3, W4 = (w.detach().reshape(w.shape[0], -1).float() for w in (w1, w2, w3, w4))
@@ -65,6 +66,7 @@ class CrmPointEncoders(torch.autograd.Function):
                 if l == 3:
                     g = pooled
                     shift4 = ops.linear(g, W4g)         # (crops, 256) = g W4g^T, the concatenated half of pts_encoder_2
+        rows['enc1'], rows['enc2'] = sels
         ctx.save_for_backward(x, g, pooled)
         ctx.st = (P, mode, wf, wb, W4g, shift4, tab, per, torch.stack(sels), zsels, csum)
         return pooled
@@ -107,7 +109,7 @@ class CrmPointEncoders(torch.autograd.Function):
         dW1 = slab[:C1 * c0].view(C1, c0)
         f = lambda t: t.float()                                          # noqa: E731
         dW4 = torch.cat([dW4g, dW4p], dim=1)
-        return (None, None, None, None,
+        return (None, None, None, None, None,
                 f(dW1).view(C1, c0, 1, 1), f(dgam1), f(dbet1), f(dW2).view(C2, C1, 1, 1), f(dgam2), f(dbet2),
                 f(dW3).view(C3, C2, 1, 1), f(dgam3), f(dbet3), f(dW4).view(C4, C3 + C2, 1, 1), f(dgam4), f(dbet4))
 
@@ -118,8 +120,11 @@ def point_encoders(module, pts):
     if P % 64 != 0:
         raise ValueError('train-mode ConfidencePointnet needs the points per crop to be a multiple of 64 (a tile never straddles two '
                          'crops); got %d' % P)
+    if C % 8 != 0 or not 8 <= C <= 64:
+        raise ValueError('train-mode ConfidencePointnet needs the point dims to be a multiple of 8 in [8, 64] (the first layer\'s '
+                         'reduction is staged 8 channels at a time, at most 64); got %d' % C)
     e1, e2 = module.pts_encoder_1, module.pts_encoder_2
-    return CrmPointEncoders.apply(pts.reshape(B * L * P, C).contiguous(), P, module.mode, (e1[1], e1[4], e1[7], e2[1]),
+    return CrmPointEncoders.apply(pts.reshape(B * L * P, C).contiguous(), P, module.mode, module.pooled_rows, (e1[1], e1[4], e1[7], e2[1]),
                                   e1[0].weight, e1[1].weight, e1[1].bias, e1[3].weight, e1[4].weight, e1[4].bias,
                                   e1[6].weight, e1[7].weight, e1[7].bias, e2[0].weight, e2[1].weight, e2[1].bias)
 

@@ -2,7 +2,9 @@
 target_assign.py:55-70) on a state dict, with autograd doing the backward -- TEST INFRASTRUCTURE.
 
 Token-major: every 1x1 conv is a matmul on (rows, C), every BatchNorm takes batch statistics over all rows (F.batch_norm, training),
-which is what BatchNorm2d over (B, C, L, P) and BatchNorm1d over (B, C, L) compute."""
+which is what BatchNorm2d over (B, C, L, P) and BatchNorm1d over (B, C, L) compute.  ``pooled_rows`` = {'enc1': (B*L, 256), 'enc2':
+(B*L, 256)} rows within each crop replaces each max over the crop's points by a gather at those rows, so that a test can pool where
+the device did."""
 import numpy as np
 import torch
 import torch.nn.functional as F
@@ -35,14 +37,24 @@ def _layer(x, sd, conv, bn, stats, relu=True):
     return torch.relu(x) if relu else x
 
 
-def crm_train_step(state_dict, conf_points, iou, score_thresh=SCORE_THRESH, device='cpu'):
-    """one training forward + backward in float64.  state_dict: ConfidencePointnet keys (no 'reg.' prefix).  Returns (losses {name:
-    float}, grads {param: tensor}, running stats after the step {buffer: tensor})"""
-    sd = {k: v.to(device, torch.float64).clone().requires_grad_(True) for k, v in state_dict.items()
-          if not k.endswith(('running_mean', 'running_var', 'num_batches_tracked'))}
-    stats = {k: v.to(device).clone().double() if not k.endswith('num_batches_tracked') else v.to(device).clone()
-             for k, v in state_dict.items() if k.endswith(('running_mean', 'running_var', 'num_batches_tracked'))}
-    x = conf_points.to(device, torch.float64)
+def _pool(y, groups, rows):
+    y = y.view(groups, -1, y.shape[-1])
+    if rows is None:
+        return y.max(dim=1)[0]
+    return y.gather(1, rows.long().to(y.device).unsqueeze(1)).squeeze(1)
+
+
+def crm_train_step(state_dict, conf_points, iou, score_thresh=SCORE_THRESH, device='cpu', pooled_rows=None, dtype=torch.float64,
+                   record=None):
+    """one training forward + backward in float64 (or ``dtype``).  state_dict: ConfidencePointnet keys (no 'reg.' prefix).  Returns
+    (losses {name: float}, grads {param: tensor}, running stats after the step {buffer: tensor}).  ``record`` (a dict) receives the
+    inputs of the two max-pools over each crop's points, 'enc1' and 'enc2' (B*L, P, 256), and the second one's output 'pool' (B*L, 256)"""
+    stat_keys = ('running_mean', 'running_var', 'num_batches_tracked')
+    sd = {k: v.to(device, dtype).clone().requires_grad_(True) for k, v in state_dict.items() if not k.endswith(stat_keys)}
+    stats = {k: v.to(device).clone().to(dtype) if not k.endswith('num_batches_tracked') else v.to(device).clone()
+             for k, v in state_dict.items() if k.endswith(stat_keys)}
+    pr = pooled_rows or {}
+    x = conf_points.to(device, dtype)
     B, L, P, C = x.shape
     x = x.reshape(B * L * P, C)
     e = 'pts_encoder_1.'
@@ -50,10 +62,13 @@ def crm_train_step(state_dict, conf_points, iou, score_thresh=SCORE_THRESH, devi
     y2 = _layer(y1, sd, e + '3', e + '4', stats)                     # the hook on pts_encoder_1[5]
     y3 = _layer(y2, sd, e + '6', e + '7', stats)
     E = y3.shape[1]
-    g = y3.view(B * L, P, E).max(dim=1)[0]
+    g = _pool(y3, B * L, pr.get('enc1'))
     x4 = torch.cat([g.unsqueeze(1).expand(B * L, P, E), y2.view(B * L, P, -1)], dim=2).reshape(B * L * P, -1)
     y4 = _layer(x4, sd, 'pts_encoder_2.0', 'pts_encoder_2.1', stats)
-    pool = y4.view(B * L, P, E).max(dim=1)[0]
+    pool = _pool(y4, B * L, pr.get('enc2'))
+    if record is not None:
+        record['enc1'], record['enc2'] = y3.detach().view(B * L, P, E), y4.detach().view(B * L, P, E)
+        record['pool'] = pool.detach()
     h = _layer(pool, sd, 'pts_mlp.0', 'pts_mlp.1', stats)
     tap = _layer(h, sd, 'pts_mlp.3', 'pts_mlp.4', stats)             # the hook on pts_mlp[5]
     gg = tap.view(B, L, E).max(dim=1)[0]
@@ -64,11 +79,11 @@ def crm_train_step(state_dict, conf_points, iou, score_thresh=SCORE_THRESH, devi
     for t in ('score_reg', 'iou_reg'):
         hh = _layer(out, sd, 'heads.%s.0' % t, 'heads.%s.1' % t, stats)
         preds[t] = torch.sigmoid(_layer(hh, sd, 'heads.%s.3' % t, None, stats, relu=False)).reshape(-1)
-    lab = torch.clamp(iou.to(device, torch.float64), 0, 1).reshape(-1)
+    lab = torch.clamp(iou.to(device, dtype), 0, 1).reshape(-1)
     pos = lab >= score_thresh[1]
     mask = (lab < score_thresh[0]) | pos
     n = mask.sum()
-    cls = F.binary_cross_entropy(preds['score_reg'][mask], pos.double()[mask], reduction='none').sum() / n
+    cls = F.binary_cross_entropy(preds['score_reg'][mask], pos.to(dtype)[mask], reduction='none').sum() / n
     iol = F.binary_cross_entropy(preds['iou_reg'][mask], lab[mask], reduction='none').sum() / n
     loss = cls + iol
     loss.backward()

@@ -38,3 +38,29 @@ def test_restatement_matches_reference_golden():
             assert int(v) == int(ref) == 1, k
         else:
             assert torch.allclose(v, ref.double(), rtol=1e-12, atol=1e-14), k
+
+
+def test_pooling_at_the_argmax_rows_is_the_default_path():
+    """pooled_rows at the float64 argmax of each crop and channel reproduces the max-pooled step bit for bit; record holds the
+    inputs of both maxes and the pooled output"""
+    m = ConfidencePointnet(ri.crm_cfg(), 32, 32)
+    sd = weights.load_seeded(m, SEED)
+    pts = ri.crm_inputs(SEED, B=B)['conf_points']
+    iou = crm_train_ref.crm_train_iou(SEED, B, pts.shape[1])
+    rec = {}
+    losses, grads, stats = crm_train_ref.crm_train_step(sd, pts, iou, record=rec)
+    crops, P = B * pts.shape[1], pts.shape[2]
+    assert rec['enc1'].shape == rec['enc2'].shape == (crops, P, 256) and rec['pool'].shape == (crops, 256)
+    assert torch.equal(rec['pool'], rec['enc2'].max(dim=1)[0])
+    rows = {k: rec[k].max(dim=1)[1].int() for k in ('enc1', 'enc2')}
+    l2, g2, s2 = crm_train_ref.crm_train_step(sd, pts, iou, pooled_rows=rows)
+    assert l2 == losses
+    for k in grads:
+        assert torch.equal(g2[k], grads[k]), k
+    for k in stats:
+        assert torch.equal(s2[k], stats[k]), k
+    # float32 autograd of the same forward runs and stays close to float64
+    l32, g32, _ = crm_train_ref.crm_train_step(sd, pts, iou, pooled_rows=rows, dtype=torch.float32)
+    assert all(g.dtype == torch.float32 for g in g32.values())
+    for k, v in losses.items():
+        assert abs(l32[k] - v) <= 1e-4 * abs(v), k
