@@ -16,8 +16,8 @@
 // Kernel structure (one CTA per SM, persistent over the tile list; roles by warp):
 //   warps 0-7      two consumer warpgroups (64 rows each): wgmma bf16 (M64 x Cout x K16) into register accumulators; after the
 //                  tile's last block every consumer thread runs the epilogue of its own fragment (two rows, two adjacent
-//                  columns per 8): scale/shift (+residual) -> ReLU -> plane split -> 32-bit stores, with no staging tile and no
-//                  barrier between the warpgroups
+//                  columns per 8): scale/shift (+residual) -> ReLU -> plane split -> a 4 x 4 word transpose within each quad ->
+//                  16-byte stores (32-bit at Cout = 16), with no staging tile and no barrier between the warpgroups
 //   warps 8-15     producers (all of them fill one pipeline stage at a time): cp.async zero-fill gather of the neighbour rows of a 64-element block of
 //                  the (offset, channel) reduction dimension into K-major SW128 smem.  A lane's arrival on the stage barrier is
 //                  asynchronous (cp.async.mbarrier.arrive.noinc), so it moves on to the next free stage at once: the gathers of
@@ -97,6 +97,8 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
 }
 __device__ __forceinline__ float bf16_lo(uint32_t u) { return __uint_as_float(u << 16); }
 __device__ __forceinline__ float bf16_hi(uint32_t u) { return __uint_as_float(u & 0xffff0000u); }
+// a[i] for a lane-dependent i, by selects (an indexed register array would go to local memory)
+__device__ __forceinline__ uint32_t sel4(const uint32_t (&a)[4], int i) { return i == 0 ? a[0] : i == 1 ? a[1] : i == 2 ? a[2] : a[3]; }
 
 template <int CIN_PAD, int COUT, int PLANES>
 __global__ void __launch_bounds__(SbCfg<COUT, PLANES>::THREADS, 1)
@@ -357,28 +359,54 @@ k_spconv_bf16(const __grid_constant__ CUtensorMap tmW, const uint16_t* __restric
             __syncwarp();
             if (lane == 0 && nb > 0) { tc::mbar_arrive(empty + (g - 1) % S); tc::mbar_arrive(wempty + (g - 1) % WS); }
             // epilogue straight from the accumulator fragment (tc.cuh: d[4j + 2r + c] = D[frow + 8r][8j + fcol + c]): scale/shift
-            // (+ residual plane 0, then plane 1) -> ReLU -> plane split, two adjacent columns (one 32-bit word per plane) at a time
+            // (+ residual plane 0, then plane 1) -> ReLU -> plane split, two adjacent columns (one 32-bit word per plane) per
+            // thread.  With Cout >= 32 the quad (the 4 lanes of a row) then transposes each group of 4 column blocks, so every
+            // lane stores one 16-byte vector (8 columns) per plane instead of four 32-bit words: a quarter of the store
+            // instructions, each writing 64 contiguous bytes per row instead of 16.  Same words, same addresses
+            constexpr int QG = COUT >= 32 ? 4 : 1;                        // column blocks per quad transpose
+            const int q = lane & 3;
 #pragma unroll
             for (int r = 0; r < 2; ++r) {
-                if (orow[r] < 0) continue;
-                const uint32_t* rp = residual ? reinterpret_cast<const uint32_t*>(residual + (size_t)orow[r] * (PLANES * COUT) + fcol) : nullptr;
-                uint32_t* op = reinterpret_cast<uint32_t*>(out + (size_t)orow[r] * (PLANES * COUT) + fcol);
+                const bool live = orow[r] >= 0;                            // uniform over the quad, not the warp: shuffles stay outside
+                const size_t rbase = (size_t)(live ? orow[r] : 0) * (PLANES * COUT);
+                const uint32_t* rp = residual ? reinterpret_cast<const uint32_t*>(residual + rbase + fcol) : nullptr;
 #pragma unroll
-                for (int j = 0; j < COUT / 8; ++j) {
-                    const int c = 8 * j + fcol;
-                    float o0 = fmaf(acc[4 * j + 2 * r], s_scale[c], s_shift[c]);
-                    float o1 = fmaf(acc[4 * j + 2 * r + 1], s_scale[c + 1], s_shift[c + 1]);
-                    if (rp) {
+                for (int j0 = 0; j0 < COUT / 8; j0 += QG) {
+                    uint32_t h[PLANES][QG];
 #pragma unroll
-                        for (int p = 0; p < PLANES; ++p) {
-                            const uint32_t u = __ldg(rp + (p * COUT + 8 * j) / 2);
-                            o0 += bf16_lo(u); o1 += bf16_hi(u);
+                    for (int t = 0; t < QG; ++t) {
+                        const int j = j0 + t, c = 8 * j + fcol;
+                        float o0 = fmaf(acc[4 * j + 2 * r], s_scale[c], s_shift[c]);
+                        float o1 = fmaf(acc[4 * j + 2 * r + 1], s_scale[c + 1], s_shift[c + 1]);
+                        if (rp && live) {
+#pragma unroll
+                            for (int p = 0; p < PLANES; ++p) {
+                                const uint32_t u = __ldg(rp + (p * COUT + 8 * j) / 2);
+                                o0 += bf16_lo(u); o1 += bf16_hi(u);
+                            }
+                        }
+                        if (relu) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); }
+                        h[0][t] = pack_bf16(o0, o1);
+                        if (PLANES == 2) h[1][t] = pack_bf16(o0 - bf16_lo(h[0][t]), o1 - bf16_hi(h[0][t]));
+                    }
+#pragma unroll
+                    for (int p = 0; p < PLANES; ++p) {
+                        uint32_t* op = reinterpret_cast<uint32_t*>(out + rbase + p * COUT);
+                        if constexpr (QG == 1) {
+                            if (live) op[4 * j0 + q] = h[p][0];
+                        } else {
+                        // lane q gathers column block j0 + q: in round t it takes, from lane q ^ t, that lane's word of block q
+                        uint32_t v[4];
+#pragma unroll
+                        for (int t = 0; t < 4; ++t) {
+                            const uint32_t send = sel4(h[p], q ^ t);          // the block the partner lane q ^ t needs from me
+                            v[t] = t ? __shfl_xor_sync(0xffffffffu, send, t) : send;
+                        }
+                        // word s of the vector (columns 2s, 2s+1 of the block) came from lane s, i.e. in round q ^ s
+                        const uint4 w = make_uint4(sel4(v, q), sel4(v, q ^ 1), sel4(v, q ^ 2), sel4(v, q ^ 3));
+                        if (live) *reinterpret_cast<uint4*>(op + 4 * (j0 + q)) = w;
                         }
                     }
-                    if (relu) { o0 = fmaxf(o0, 0.f); o1 = fmaxf(o1, 0.f); }
-                    const uint32_t h = pack_bf16(o0, o1);
-                    op[4 * j] = h;
-                    if (PLANES == 2) op[(COUT + 8 * j) / 2] = pack_bf16(o0 - bf16_lo(h), o1 - bf16_hi(h));
                 }
             }
         }
