@@ -147,13 +147,17 @@ __global__ void __launch_bounds__(NT) k_combine_write(const double* __restrict__
     }
 }
 
-size_t cnt_bytes(int B, int F) { return dz_align_up((size_t)F * B * sizeof(int32_t), 256); }
+struct CombineWs { int32_t *cnt, *rank; };          // cnt (F, B), rank (B, L)
+
+CombineWs carve_combine(DzCarve& cv, int B, int L, int F) {
+    CombineWs w;
+    w.cnt = cv.take<int32_t>((size_t)F * B); w.rank = cv.take<int32_t>((size_t)B * L);
+    return w;
+}
 
 }  // namespace
 
-extern "C" size_t dz_combine_frames_ws_bytes(int B, int L, int F) {
-    return cnt_bytes(B, F) + dz_align_up((size_t)B * L * sizeof(int32_t), 256) + 256;
-}
+extern "C" size_t dz_combine_frames_ws_bytes(int B, int L, int F) { return dz_carve_bytes(carve_combine, B, L, F); }
 
 extern "C" int dz_combine_frames(const double* prm_lidar, const float* grm_pred, const float* score, const int32_t* frame_of_box,
                                  const int32_t* box_num, const int32_t* cls, const int32_t* track_id, int B, int L,
@@ -163,23 +167,19 @@ extern "C" int dz_combine_frames(const double* prm_lidar, const float* grm_pred,
     DZ_CHECK_ARG(B >= 0 && L >= 1 && F >= 1 && R >= 1 && rows && obj_id && count && overflow && ws);
     DZ_CHECK_ARG(B == 0 || (prm_lidar && grm_pred && score && frame_of_box && box_num && cls && track_id));
     DZ_CHECK_ARG(!det || (det_count && kept && K >= 1));
-    if (ws_bytes < dz_combine_frames_ws_bytes(B, L, F)) {
-        dz_set_error("dz_combine_frames: workspace too small");
-        return DZ_ERR_WORKSPACE;
-    }
+    DZ_CHECK_WS(dz_combine_frames_ws_bytes(B, L, F));
     cudaStream_t st = (cudaStream_t)stream;
-    DzWs w(ws, ws_bytes);
-    int32_t* cnt = w.take<int32_t>((size_t)F * B);
-    int32_t* rank = w.take<int32_t>((size_t)B * L);
-    if (B) DZ_CUDA(cudaMemsetAsync(cnt, 0, (size_t)F * B * sizeof(int32_t), st));
+    DzCarve cv((char*)ws);
+    const CombineWs w = carve_combine(cv, B, L, F);
+    if (B) DZ_CUDA(cudaMemsetAsync(w.cnt, 0, (size_t)F * B * sizeof(int32_t), st));
     if (B) {
-        k_combine_count<<<B, NT, 0, st>>>(frame_of_box, box_num, B, L, F, cnt, rank, overflow);
+        k_combine_count<<<B, NT, 0, st>>>(frame_of_box, box_num, B, L, F, w.cnt, w.rank, overflow);
         DZ_LAUNCH_CHECK();
     }
-    k_combine_frame<<<F, NT, 0, st>>>(cnt, B, det, det_count, kept, K, R, rows, obj_id, count, overflow);
+    k_combine_frame<<<F, NT, 0, st>>>(w.cnt, B, det, det_count, kept, K, R, rows, obj_id, count, overflow);
     DZ_LAUNCH_CHECK();
     if (B) {
-        k_combine_write<<<B, NT, 0, st>>>(prm_lidar, grm_pred, score, frame_of_box, box_num, cls, track_id, B, L, F, R, cnt, rank, rows,
+        k_combine_write<<<B, NT, 0, st>>>(prm_lidar, grm_pred, score, frame_of_box, box_num, cls, track_id, B, L, F, R, w.cnt, w.rank, rows,
                                           obj_id);
         DZ_LAUNCH_CHECK();
     }

@@ -13,6 +13,10 @@ void dz_set_error(const char* fmt, ...);
 #define DZ_CHECK_ARG(cond)                                                            \
     do { if (!(cond)) { dz_set_error("%s:%d: bad argument: %s", __FILE__, __LINE__, #cond); return DZ_ERR_ARG; } } while (0)
 
+// a workspace of ws_bytes smaller than `need` (the entry point's *_ws_bytes): fail before anything is enqueued
+#define DZ_CHECK_WS(need)                                                             \
+    do { if (ws_bytes < (need)) { dz_set_error("%s: workspace too small", __func__); return DZ_ERR_WORKSPACE; } } while (0)
+
 #define DZ_CUDA(call)                                                                 \
     do { cudaError_t e__ = (call); if (e__ != cudaSuccess) {                          \
         dz_set_error("%s:%d: %s -> %s", __FILE__, __LINE__, #call, cudaGetErrorString(e__)); return DZ_ERR_CUDA; } } while (0)
@@ -23,17 +27,6 @@ void dz_set_error(const char* fmt, ...);
 
 static inline size_t dz_align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 static inline int dz_cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
-
-// carve a workspace
-struct DzWs {
-    char* p; size_t left;
-    DzWs(void* ws, size_t bytes) : p((char*)ws), left(bytes) {}
-    template <typename T> T* take(size_t n) {
-        size_t b = dz_align_up(n * sizeof(T), 256);
-        if (b > left) return nullptr;
-        T* r = (T*)p; p += b; left -= b; return r;
-    }
-};
 
 // ---- grid index lookup (device) ----------------------------------------------------------------------------
 struct GridIndex {
@@ -111,8 +104,9 @@ __device__ int block_compact(int n, Pred pred, Emit emit) {
     return total;
 }
 
-// a workspace carved in 256-byte aligned pieces, the same list on the host and the device: from a null base it only adds up the
-// bytes, which is how the *_ws_bytes entry points size it
+// a workspace carved in 256-byte aligned pieces.  Each entry point lays its workspace out in one carve function: its *_ws_bytes
+// runs it from a null base, where it only adds up the bytes, and the entry point runs it on the caller's buffer once that size is
+// checked.  Where a kernel carves for itself, the function is __host__ __device__ and the list is the same on both sides.
 struct DzCarve {
     char* base;
     size_t bytes = 0;
@@ -123,3 +117,10 @@ struct DzCarve {
         return r;
     }
 };
+
+// the bytes carve(cv, args...) takes: what a *_ws_bytes entry point returns
+template <class Carve, class... A> static size_t dz_carve_bytes(Carve carve, A... args) {
+    DzCarve cv(nullptr);
+    carve(cv, args...);
+    return cv.bytes;
+}

@@ -86,11 +86,7 @@ __host__ __device__ Ws carve(DzCarve& c, int R, int G, int P) {
     return w;
 }
 
-size_t block_ws_bytes(int R, int G, int P) {
-    DzCarve c(nullptr);
-    carve(c, R, G, P);
-    return c.bytes;
-}
+size_t block_ws_bytes(int R, int G, int P) { return dz_carve_bytes(carve, R, G, P); }
 
 __device__ __forceinline__ int valid_type(int t) { return t >= 1 && t <= 4; }
 
@@ -341,10 +337,7 @@ extern "C" int dz_det_eval(const float* pred, const int* pred_cnt, const float* 
                  G >= 1 && (box_type == 0 || box_type == 1) && breakdown_mask >= 0 && breakdown_mask <= 3 && max_pairs >= 1 &&
                  max_pairs <= (1 << 26) && (long long)G * R < INT_MAX && G + 3LL * R < INT_MAX);
     if (NF == 0 || breakdown_mask == 0) return DZ_OK;
-    if (ws_bytes < dz_det_eval_ws_bytes(NF, R, G, max_pairs)) {
-        dz_set_error("dz_det_eval: workspace too small");
-        return DZ_ERR_WORKSPACE;
-    }
+    DZ_CHECK_WS(dz_det_eval_ws_bytes(NF, R, G, max_pairs));
     EvIn in{pred, pred_cnt, gt_box, gt_type, gt_level, gt_cnt, NF, R, G, box_type, breakdown_mask, max_pairs};
     char* base = (char*)dz_align_up((size_t)ws, 256);
     k_det_eval<<<eval_blocks(NF), NT, 0, (cudaStream_t)stream>>>(in, records, overflow, base, block_ws_bytes(R, G, max_pairs));

@@ -221,10 +221,22 @@ __global__ void __launch_bounds__(HD_THREADS) k_topk_merge_decode(const float* _
     if (threadIdx.x == 0) d_cand_n[b] = written;
 }
 
+// Kp: K rounded up to a power of two, the top-K sort's size
+struct DecodeWs { float* score; unsigned long long *cand_keys, *cand; int *cand_cnt, *overflow, Kp; };
+
+static DecodeWs carve_decode(DzCarve& cv, int B, int H, int W, int num_class, int K) {
+    const size_t BC = (size_t)B * num_class;
+    DecodeWs w;
+    w.Kp = 1;
+    while (w.Kp < K) w.Kp <<= 1;
+    w.score = cv.take<float>(BC * H * W);
+    w.cand_keys = cv.take<unsigned long long>(BC * w.Kp); w.cand = cv.take<unsigned long long>(BC * HD_CAND_CAP);
+    w.cand_cnt = cv.take<int>(BC); w.overflow = cv.take<int>(BC);
+    return w;
+}
+
 extern "C" size_t dz_centerhead_decode_ws_bytes(int B, int H, int W, int num_class, int K) {
-    int Kp = 1; while (Kp < K) Kp <<= 1;
-    return dz_align_up((size_t)B * num_class * H * W * 4, 256) + dz_align_up((size_t)B * num_class * Kp * 8, 256) +
-           dz_align_up((size_t)B * num_class * HD_CAND_CAP * 8, 256) + dz_align_up((size_t)B * num_class * 4, 256) * 2;
+    return dz_carve_bytes(carve_decode, B, H, W, num_class, K);
 }
 
 extern "C" int dz_centerhead_decode(const float* head, int B, int H, int W, int ch, int ch_center, int ch_z, int ch_dim,
@@ -234,24 +246,19 @@ extern "C" int dz_centerhead_decode(const float* head, int B, int H, int W, int 
                                     int* d_cand_n, void* ws, size_t ws_bytes, dz_stream_t stream) {
     DZ_CHECK_ARG(head && cand_boxes && cand_scores && cand_labels && d_cand_n && ws);
     DZ_CHECK_ARG(K >= 1 && K <= 1024 && num_class >= 1 && num_class * K <= 4096);
-    if (ws_bytes < dz_centerhead_decode_ws_bytes(B, H, W, num_class, K)) { dz_set_error("dz_centerhead_decode: workspace too small"); return DZ_ERR_WORKSPACE; }
+    DZ_CHECK_WS(dz_centerhead_decode_ws_bytes(B, H, W, num_class, K));
     cudaStream_t st = (cudaStream_t)stream;
-    int Kp = 1; while (Kp < K) Kp <<= 1;
-    DzWs w(ws, ws_bytes);
-    float* score_ws = w.take<float>((size_t)B * num_class * H * W);
-    unsigned long long* cand_keys = w.take<unsigned long long>((size_t)B * num_class * Kp);
-    unsigned long long* cand = w.take<unsigned long long>((size_t)B * num_class * HD_CAND_CAP);
-    int* cand_cnt = w.take<int>((size_t)B * num_class);
-    int* overflow = w.take<int>((size_t)B * num_class);
-    if (!overflow) { dz_set_error("dz_centerhead_decode: workspace carve failed"); return DZ_ERR_WORKSPACE; }
+    DzCarve cv((char*)ws);
+    const DecodeWs w = carve_decode(cv, B, H, W, num_class, K);
+    const int Kp = w.Kp;
     if (K <= HD_CAND_CAP && score_thresh >= 0.f) {
-        DZ_CUDA(cudaMemsetAsync(cand_cnt, 0, (size_t)B * num_class * 4, st));
+        DZ_CUDA(cudaMemsetAsync(w.cand_cnt, 0, (size_t)B * num_class * 4, st));
         int blocks = max(1, min(dz_cdiv((long long)B * H * W, 256), DZ_NUM_SMS * 8));
-        k_score_prefilter<<<blocks, 256, 0, st>>>(head, H * W, ch, ch_hm, ch_iou, use_iou, num_class, B, score_thresh, cand, cand_cnt);
-        k_topk_from_candidates<<<B * num_class, HD_THREADS, 0, st>>>(cand, cand_cnt, K, Kp, cand_keys, overflow);
-        k_topk_class<<<B * num_class, HD_THREADS, 0, st>>>(head, H * W, ch, ch_hm, ch_iou, use_iou, num_class, K, Kp, score_ws, cand_keys, overflow);
+        k_score_prefilter<<<blocks, 256, 0, st>>>(head, H * W, ch, ch_hm, ch_iou, use_iou, num_class, B, score_thresh, w.cand, w.cand_cnt);
+        k_topk_from_candidates<<<B * num_class, HD_THREADS, 0, st>>>(w.cand, w.cand_cnt, K, Kp, w.cand_keys, w.overflow);
+        k_topk_class<<<B * num_class, HD_THREADS, 0, st>>>(head, H * W, ch, ch_hm, ch_iou, use_iou, num_class, K, Kp, w.score, w.cand_keys, w.overflow);
     } else {
-        k_topk_class<<<B * num_class, HD_THREADS, 0, st>>>(head, H * W, ch, ch_hm, ch_iou, use_iou, num_class, K, Kp, score_ws, cand_keys, nullptr);
+        k_topk_class<<<B * num_class, HD_THREADS, 0, st>>>(head, H * W, ch, ch_hm, ch_iou, use_iou, num_class, K, Kp, w.score, w.cand_keys, nullptr);
     }
     DecodeGeom g;
     for (int d = 0; d < 3; ++d) { g.lo[d] = range6[d]; g.vs[d] = vsize3[d]; }
@@ -259,7 +266,7 @@ extern "C" int dz_centerhead_decode(const float* head, int B, int H, int W, int 
     g.stride = (float)fmap_stride; g.thresh = score_thresh;
     int np2 = 1; while (np2 < num_class * K) np2 <<= 1;
     k_topk_merge_decode<<<B, HD_THREADS, (size_t)np2 * 8, st>>>(head, H, W, ch, ch_center, ch_z, ch_dim, ch_rot, num_class, K, Kp,
-                                                                 cand_keys, g, cand_boxes, cand_scores, cand_labels, d_cand_n);
+                                                                 w.cand_keys, g, cand_boxes, cand_scores, cand_labels, d_cand_n);
     DZ_LAUNCH_CHECK();
     return DZ_OK;
 }
@@ -382,18 +389,20 @@ __global__ void __launch_bounds__(256) k_nms_scan(const float* __restrict__ boxe
     if (threadIdx.x == 0) d_out_n[b] = nk;
 }
 
-extern "C" size_t dz_nms_bev_ws_bytes(int B, int cap) {
-    return dz_align_up((size_t)B * cap * ((cap + 63) / 64) * 8, 256);
-}
+// the suppression mask (B, cap, col_blocks)
+static unsigned long long* carve_nms(DzCarve& cv, int B, int cap) { return cv.take<unsigned long long>((size_t)B * cap * ((cap + 63) / 64)); }
+
+extern "C" size_t dz_nms_bev_ws_bytes(int B, int cap) { return dz_carve_bytes(carve_nms, B, cap); }
 
 extern "C" int dz_nms_bev(const float* boxes, const float* scores, const int32_t* labels, const int* d_n, int B, int cap,
                           float thresh, int post_max, int label_offset, float* out, int* d_out_n, void* ws,
                           size_t ws_bytes, dz_stream_t stream) {
     DZ_CHECK_ARG(boxes && scores && labels && d_n && out && d_out_n && ws && B >= 1 && cap >= 1 && cap <= 2048 && post_max >= 1);
-    if (ws_bytes < dz_nms_bev_ws_bytes(B, cap)) { dz_set_error("dz_nms_bev: workspace too small"); return DZ_ERR_WORKSPACE; }
+    DZ_CHECK_WS(dz_nms_bev_ws_bytes(B, cap));
     cudaStream_t st = (cudaStream_t)stream;
     int col_blocks = (cap + 63) / 64;
-    unsigned long long* mask = (unsigned long long*)ws;
+    DzCarve cv((char*)ws);
+    unsigned long long* mask = carve_nms(cv, B, cap);
     // refuse an unsupported cap before anything is enqueued: a rejected call leaves the workspace and the outputs as they were
     size_t smem = (size_t)cap * col_blocks * 8 + (size_t)cap * 4;
     if (smem > 200 * 1024) { dz_set_error("dz_nms_bev: cap too large for shared-memory scan"); return DZ_ERR_UNSUPPORTED; }

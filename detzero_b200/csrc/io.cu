@@ -86,19 +86,23 @@ __global__ void __launch_bounds__(256) k_prep_write(const float* __restrict__ ra
     }
 }
 
-extern "C" size_t dz_prepare_points_ws_bytes(int n) { return (size_t)dz_cdiv(max(n, 1), PREP_CHUNK) * 4 + 256; }
+// the per-chunk counts, scanned in place
+static int* carve_prep(DzCarve& cv, int n) { return cv.take<int>(dz_cdiv(max(n, 1), PREP_CHUNK)); }
+
+extern "C" size_t dz_prepare_points_ws_bytes(int n) { return dz_carve_bytes(carve_prep, n); }
 
 extern "C" int dz_prepare_points(const float* raw, int n, const double* transform12_host, float time_offset, int with_time, int batch_idx,
                                  float* out, int cap, int* d_count, void* ws, size_t ws_bytes, dz_stream_t stream) {
     DZ_CHECK_ARG(raw && out && d_count && n >= 0 && cap >= 1);
     if (n == 0) return DZ_OK;
-    if (ws_bytes < dz_prepare_points_ws_bytes(n)) { dz_set_error("dz_prepare_points: workspace too small"); return DZ_ERR_WORKSPACE; }
+    DZ_CHECK_WS(dz_prepare_points_ws_bytes(n));
     PrepXform xf;
     int identity = transform12_host == nullptr;
     for (int i = 0; i < 12; ++i) xf.m[i] = identity ? 0.0 : transform12_host[i];
     cudaStream_t st = (cudaStream_t)stream;
     const int n_chunks = dz_cdiv(n, PREP_CHUNK);
-    int* cc = (int*)ws;
+    DzCarve cv((char*)ws);
+    int* cc = carve_prep(cv, n);
     k_prep_count<<<n_chunks, 256, 0, st>>>(raw, n, cc);
     k_prep_scan<<<1, 1024, 0, st>>>(cc, n_chunks, d_count);
     k_prep_write<<<n_chunks, 256, 0, st>>>(raw, n, cc, xf, identity, time_offset, with_time, (float)batch_idx, out, cap);

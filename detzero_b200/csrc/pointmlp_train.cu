@@ -571,11 +571,10 @@ extern "C" int dz_pm_dgrad(int mode, int R, int gsize, int nseg,
     return DZ_OK;
 }
 
-extern "C" size_t dz_pm_wgrad_ws_bytes(int R, int N, int K) {
-    DzCarve cv(nullptr);
-    cv.take<float>((size_t)wgrad_splits(R, N, K) * N * K);
-    return cv.bytes;
-}
+// each row split's partial weight gradient (S, N, K)
+static float* carve_wgrad(DzCarve& cv, int R, int N, int K) { return cv.take<float>((size_t)wgrad_splits(R, N, K) * N * K); }
+
+extern "C" size_t dz_pm_wgrad_ws_bytes(int R, int N, int K) { return dz_carve_bytes(carve_wgrad, R, N, K); }
 
 extern "C" int dz_pm_wgrad(int mode, int R, int gsize, int N, const float* dhs, const int* sel, const float* dsel, const float* zs,
                            const float* tab, const float* x, int K, const float* tab_in, double* dw, void* ws, size_t ws_bytes,
@@ -588,10 +587,10 @@ extern "C" int dz_pm_wgrad(int mode, int R, int gsize, int N, const float* dhs, 
     WgradArgs a{};
     a.s = make_seg(N, dhs, sel, dsel, zs, tab, nullptr);
     if ((rc = check_seg("dz_pm_wgrad", a.s, false)) != DZ_OK) return rc;
-    if (ws_bytes < dz_pm_wgrad_ws_bytes(R, N, K)) { dz_set_error("dz_pm_wgrad: workspace too small"); return DZ_ERR_WORKSPACE; }
+    DZ_CHECK_WS(dz_pm_wgrad_ws_bytes(R, N, K));
     const int S = wgrad_splits(R, N, K);
     DzCarve cv((char*)ws);
-    a.part = cv.take<float>((size_t)S * N * K);
+    a.part = carve_wgrad(cv, R, N, K);
     a.R = R; a.gsize = gsize; a.x = x; a.K = K; a.tab_in = tab_in;
     a.rows_per_split = dz_cdiv(R / KC, S) * KC;
     dim3 grid(S, N / TM, dz_cdiv(K, TN));

@@ -397,10 +397,22 @@ __global__ void k_rd_fill(RdParams P) {
     emit_p2co(o, e, 0.f, P.bx[t], P.with_class, P.cls[b]);
 }
 
+// the RdParams arrays that live in the workspace; n and sel serve when the caller passes no counts / sel
+struct RdWs { RdBox* bx; int *cc, *n, *goff, *gtot, *qnum, *qidx, *sel, n_chunks; };
+
+static RdWs carve_rd(DzCarve& cv, int kind, int B, int L, int max_frame_points, int kq, int km, int nq) {
+    const size_t T = (size_t)B * L;
+    RdWs w;
+    w.n_chunks = dz_cdiv(max(max_frame_points, 1), RD_CHUNK);
+    w.bx = cv.take<RdBox>(T);
+    w.cc = cv.take<int>(T * w.n_chunks); w.n = cv.take<int>(T); w.goff = cv.take<int>(T);
+    w.gtot = cv.take<int>(B); w.qnum = cv.take<int>(B); w.qidx = cv.take<int>((size_t)B * nq);
+    w.sel = cv.take<int>(kind == RD_PRM ? T * (kq + km) : kind == RD_CRM ? T * kq : (size_t)B * (nq * kq + km));
+    return w;
+}
+
 extern "C" size_t dz_refine_inputs_ws_bytes(int kind, int B, int L, int max_frame_points, int kq, int km, int nq) {
-    const size_t T = (size_t)B * L, nch = dz_cdiv(max(max_frame_points, 1), RD_CHUNK);
-    const size_t sel = kind == RD_PRM ? T * (kq + km) : kind == RD_CRM ? T * kq : (size_t)B * (nq * kq + km);
-    return dz_align_up(T * sizeof(RdBox), 256) + dz_align_up((T * nch + 3 * T + 2 * B + (size_t)B * nq) * 4, 256) + sel * 4 + 256;
+    return dz_carve_bytes(carve_rd, kind, B, L, max_frame_points, kq, km, nq);
 }
 
 extern "C" int dz_refine_inputs(int kind, const float* points, int pt_stride, const int32_t* frame_offsets, int n_frames,
@@ -417,10 +429,7 @@ extern "C" int dz_refine_inputs(int kind, const float* points, int pt_stride, co
     DZ_CHECK_ARG(kind != RD_PRM || (m_pts && traj && track_f));
     DZ_CHECK_ARG(kind != RD_GRM || (m_pts && traj && query_num && nq >= 1 && nq <= 8 && q_out >= 0 && q_out <= nq));
     if (B == 0) return DZ_OK;
-    if (ws_bytes < dz_refine_inputs_ws_bytes(kind, B, L, max_frame_points, kq, km, nq)) {
-        dz_set_error("dz_refine_inputs: workspace too small");
-        return DZ_ERR_WORKSPACE;
-    }
+    DZ_CHECK_WS(dz_refine_inputs_ws_bytes(kind, B, L, max_frame_points, kq, km, nq));
     const int T = B * L;
     RdParams P;
     P.pts = points; P.pstride = pt_stride; P.foff = frame_offsets; P.F = n_frames;
@@ -429,19 +438,10 @@ extern "C" int dz_refine_inputs(int kind, const float* points, int pt_stride, co
     P.B = B; P.L = L; P.kind = kind; P.with_class = with_class ? 1 : 0; P.C = kind == RD_GRM ? 4 : 32 + 3 * P.with_class;
     P.kq = kq; P.km = kind == RD_CRM ? 0 : km; P.nq = nq; P.qout = q_out; P.crop = crop ? 1 : 0; P.bev = crop_on_bev ? 1 : 0;
     P.enlarge = enlarge_scale; P.seed = seed;
-    P.n_chunks = dz_cdiv(max(max_frame_points, 1), RD_CHUNK);
-    char* w = (char*)ws;
-    P.bx = (RdBox*)w; w += dz_align_up((size_t)T * sizeof(RdBox), 256);
-    int* iw = (int*)w;
-    P.cc = iw; iw += (size_t)T * P.n_chunks;
-    P.n = counts ? counts : iw; iw += T;
-    P.goff = iw; iw += T;
-    iw += T;
-    P.gtot = iw; iw += B;
-    P.qnum = iw; iw += B;
-    P.qidx = iw; iw += (size_t)B * nq;
-    w += dz_align_up(((size_t)T * P.n_chunks + 3 * (size_t)T + 2 * (size_t)B + (size_t)B * nq) * 4, 256);
-    P.sel = sel ? sel : (int*)w;
+    DzCarve cv((char*)ws);
+    const RdWs w = carve_rd(cv, kind, B, L, max_frame_points, kq, km, nq);
+    P.n_chunks = w.n_chunks; P.bx = w.bx; P.cc = w.cc; P.n = counts ? counts : w.n; P.goff = w.goff;
+    P.gtot = w.gtot; P.qnum = w.qnum; P.qidx = w.qidx; P.sel = sel ? sel : w.sel;
     P.q_pts = q_pts; P.m_pts = m_pts; P.traj = traj; P.box_f = box_f; P.track_f = track_f; P.query_num = query_num;
     cudaStream_t st = (cudaStream_t)stream;
     k_rd_prep<<<dz_cdiv(T, 128), 128, 0, st>>>(P);

@@ -410,13 +410,17 @@ __global__ void k_sum_rows_f64(const double* __restrict__ x, int rows, long long
 
 static int crm_point_grid(int crops) { return crops < DZ_NUM_SMS ? crops : DZ_NUM_SMS; }
 
-extern "C" size_t dz_crm_point_ws_bytes(int crops) {
-    DzCarve cv(nullptr);
+// each CTA's partials: its 512 BatchNorm sums and its slab
+struct CrmWs { double *stats, *slab; };
+
+static CrmWs carve_crm(DzCarve& cv, int crops) {
     const int G = crm_point_grid(crops);
-    cv.take<double>((size_t)G * 512);
-    cv.take<double>((size_t)G * SLAB);
-    return cv.bytes;
+    CrmWs w;
+    w.stats = cv.take<double>((size_t)G * 512); w.slab = cv.take<double>((size_t)G * SLAB);
+    return w;
 }
+
+extern "C" size_t dz_crm_point_ws_bytes(int crops) { return dz_carve_bytes(carve_crm, crops); }
 
 extern "C" int dz_crm_point_pass(int pass, int mode, const float* x, int crops, int P, int c0,
                                  const float* w1t, const float* w2t, const float* w3t, const float* w4pt,
@@ -433,12 +437,11 @@ extern "C" int dz_crm_point_pass(int pass, int mode, const float* x, int crops, 
     DZ_CHECK_ARG((pass != 3 && pass != 4) || (zext && iext));
     DZ_CHECK_ARG(pass != 4 || csum);
     DZ_CHECK_ARG(pass < 5 || (w2 && w3 && w4p && sel && dsel));
-    if (ws_bytes < dz_crm_point_ws_bytes(crops)) { dz_set_error("dz_crm_point_pass: workspace too small"); return DZ_ERR_WORKSPACE; }
+    DZ_CHECK_WS(dz_crm_point_ws_bytes(crops));
     const int G = crm_point_grid(crops);
     DzCarve cv((char*)ws);
-    Args a{x, crops, P, c0, w1t, w2t, w3t, w4pt, w2, w3, w4p, tab, shift4, sel, dsel, nullptr, zext, iext, csum, nullptr};
-    a.stats = cv.take<double>((size_t)G * 512);
-    a.slab = cv.take<double>((size_t)G * SLAB);
+    const CrmWs w = carve_crm(cv, crops);
+    Args a{x, crops, P, c0, w1t, w2t, w3t, w4pt, w2, w3, w4p, tab, shift4, sel, dsel, w.stats, zext, iext, csum, w.slab};
     cudaStream_t st = (cudaStream_t)stream;
     if (pass >= 5) DZ_CUDA(cudaMemsetAsync(a.slab, 0, (size_t)G * SLAB * sizeof(double), st));
     int rc = mode == DZ_F32 ? launch<DZ_F32>(pass, a, G, st) : launch<DZ_TF32>(pass, a, G, st);

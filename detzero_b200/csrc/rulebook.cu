@@ -127,20 +127,29 @@ __global__ void __launch_bounds__(256) k_subm_nbr(const int32_t* __restrict__ co
     table_finish(to, s_hist);
 }
 
-// workspace layout shared by the rulebook kernels (which emit digests + histogram) and dz_rulebook_schedule:
-// hist[SCHED_BINS] | tile_mask[tiles] | tickets[8] | masks[cap] | keys[cap] (u16)
-static TableOut table_out(int32_t* nbr, int32_t* tab, void* sched_ws, int cap) {
-    TableOut to{nbr, tab, nullptr, nullptr, nullptr, nullptr};
-    if (sched_ws) {
-        to.hist = reinterpret_cast<int*>(sched_ws);
-        to.ticket = to.hist + SCHED_BINS + dz_cdiv(cap, 128);
-        to.masks = to.ticket + 8;
-        to.keys = reinterpret_cast<uint16_t*>(to.masks + cap);
-    }
-    return to;
+// tile-schedule scratch, shared by the rulebook kernels (which emit digests + histogram) and dz_rulebook_schedule
+// hist[SCHED_BINS] | tile_mask[tiles] | ticket[2] | masks[cap] | keys[cap]: ticket[0] counts the rulebook kernel's blocks, ticket[1]
+// the scatter's; the rulebook call zeroes the first zero_bytes (histogram, tile masks, tickets)
+struct SchedWs { int *hist, *tile_mask, *ticket, *masks; uint16_t* keys; size_t zero_bytes; };
+
+static SchedWs carve_sched(DzCarve& cv, int cap) {
+    SchedWs w;
+    w.hist = cv.take<int>(SCHED_BINS); w.tile_mask = cv.take<int>(dz_cdiv(cap, 128)); w.ticket = cv.take<int>(2);
+    w.zero_bytes = cv.bytes;
+    w.masks = cv.take<int>(cap); w.keys = cv.take<uint16_t>(cap);
+    return w;
 }
-static size_t sched_zero_bytes(int cap) { return (size_t)(SCHED_BINS + dz_cdiv(cap, 128) + 8) * 4; }
-extern "C" size_t dz_rulebook_schedule_ws_bytes(int cap) { return sched_zero_bytes(cap) + (size_t)cap * 4 + (((size_t)cap * 2 + 255) & ~(size_t)255); }
+
+extern "C" size_t dz_rulebook_schedule_ws_bytes(int cap) { return dz_carve_bytes(carve_sched, cap); }
+
+// the table outputs and, given sched_ws, the digest outputs, with their histogram, tile masks and tickets zeroed on the stream
+static int table_out(TableOut& to, int32_t* nbr, int32_t* tab, void* sched_ws, int cap, cudaStream_t st) {
+    DzCarve cv((char*)sched_ws);
+    const SchedWs w = carve_sched(cv, cap);
+    to = sched_ws ? TableOut{nbr, tab, w.keys, w.masks, w.hist, w.ticket} : TableOut{nbr, tab, nullptr, nullptr, nullptr, nullptr};
+    if (sched_ws) DZ_CUDA(cudaMemsetAsync(sched_ws, 0, w.zero_bytes, st));
+    return DZ_OK;
+}
 
 extern "C" int dz_rulebook_subm(const int32_t* coords, const int* d_n, int cap, int B, int D, int H, int W,
                                 const int* ks, const uint32_t* bitmap, const uint32_t* prefix, const int32_t* perm,
@@ -148,8 +157,8 @@ extern "C" int dz_rulebook_subm(const int32_t* coords, const int* d_n, int cap, 
     DZ_CHECK_ARG(coords && d_n && bitmap && prefix && (nbr || tab) && cap >= 1);
     DZ_CHECK_ARG(ks[0] % 2 == 1 && ks[1] % 2 == 1 && ks[2] % 2 == 1 && ks[0] * ks[1] * ks[2] <= 27);
     DZ_CHECK_ARG(!sched_ws || tab);
-    TableOut to = table_out(nbr, tab, sched_ws, cap);
-    if (sched_ws) DZ_CUDA(cudaMemsetAsync(sched_ws, 0, sched_zero_bytes(cap), (cudaStream_t)stream));
+    TableOut to;
+    if (int rc = table_out(to, nbr, tab, sched_ws, cap, (cudaStream_t)stream)) return rc;
     GridIndex g{bitmap, prefix, perm, B, D, H, W, dz_cells_pad(D, H, W), cap};
     int blocks = max(1, min(dz_cdiv(cap, 256), DZ_NUM_SMS * 8));
     k_subm_nbr<<<blocks, 256, 0, (cudaStream_t)stream>>>(coords, d_n, cap, g, ks[0], ks[1], ks[2], to);
@@ -264,7 +273,7 @@ extern "C" int dz_rulebook_conv(const int32_t* in_coords, const int* d_n_in, int
     }
     cudaStream_t st = (cudaStream_t)stream;
     size_t out_words = dz_grid_index_words(B, cg.out_dhw[0], cg.out_dhw[1], cg.out_dhw[2]);
-    if (ws_bytes < dz_scan_ws_bytes(out_words)) { dz_set_error("dz_rulebook_conv: workspace too small"); return DZ_ERR_WORKSPACE; }
+    DZ_CHECK_WS(dz_scan_ws_bytes(out_words));
     long long out_cp = dz_cells_pad(cg.out_dhw[0], cg.out_dhw[1], cg.out_dhw[2]);
     int blocks_in = max(1, min(dz_cdiv(in_cap, 256), DZ_NUM_SMS * 8));
     k_conv_mark<<<blocks_in, 256, 0, st>>>(in_coords, d_n_in, in_cap, cg, out_cp, out_bitmap);
@@ -275,8 +284,8 @@ extern "C" int dz_rulebook_conv(const int32_t* in_coords, const int* d_n_in, int
                                                 out_cp, out_cap, out_coords);
     GridIndex gin{in_bitmap, in_prefix, in_perm, B, in_dhw[0], in_dhw[1], in_dhw[2], dz_cells_pad(in_dhw[0], in_dhw[1], in_dhw[2]), in_cap};
     int blocks_out = max(1, min(dz_cdiv(out_cap, 256), DZ_NUM_SMS * 8));
-    TableOut to = table_out(nbr, tab, sched_ws, out_cap);
-    if (sched_ws) DZ_CUDA(cudaMemsetAsync(sched_ws, 0, sched_zero_bytes(out_cap), st));
+    TableOut to;
+    if ((rc = table_out(to, nbr, tab, sched_ws, out_cap, st))) return rc;
     k_conv_nbr<<<blocks_out, 256, 0, st>>>(out_coords, d_n_out, out_cap, cg, gin, to);
     DZ_LAUNCH_CHECK();
     return DZ_OK;
@@ -394,14 +403,15 @@ __global__ void __launch_bounds__(256) k_sched_tiles(const int32_t* __restrict__
 extern "C" int dz_rulebook_schedule(const int32_t* tab, int cap, const int* d_n, int32_t* order, void* sched_ws, size_t ws_bytes,
                                     int K, int32_t* tab_tiles, dz_stream_t stream) {
     DZ_CHECK_ARG(tab && d_n && order && sched_ws && cap >= 1);
-    if (ws_bytes < dz_rulebook_schedule_ws_bytes(cap)) { dz_set_error("dz_rulebook_schedule: workspace too small"); return DZ_ERR_WORKSPACE; }
-    TableOut to = table_out(nullptr, const_cast<int32_t*>(tab), sched_ws, cap);
-    k_sched_scatter<<<dz_cdiv(cap, SCHED_CHUNK), 256, 0, (cudaStream_t)stream>>>(to.masks, cap, d_n, to.keys, to.hist, to.hist + SCHED_BINS, to.ticket + 1, order);
+    DZ_CHECK_WS(dz_rulebook_schedule_ws_bytes(cap));
+    DzCarve cv((char*)sched_ws);
+    const SchedWs w = carve_sched(cv, cap);
+    k_sched_scatter<<<dz_cdiv(cap, SCHED_CHUNK), 256, 0, (cudaStream_t)stream>>>(w.masks, cap, d_n, w.keys, w.hist, w.tile_mask, w.ticket + 1, order);
     DZ_LAUNCH_CHECK();
     if (tab_tiles) {
         DZ_CHECK_ARG(K >= 1 && K <= 27);
         const int blocks = max(1, min(dz_cdiv(cap, 256), DZ_NUM_SMS * 8));
-        k_sched_tiles<<<blocks, 256, 0, (cudaStream_t)stream>>>(tab, cap, d_n, K, order, to.hist + SCHED_BINS, tab_tiles);
+        k_sched_tiles<<<blocks, 256, 0, (cudaStream_t)stream>>>(tab, cap, d_n, K, order, w.tile_mask, tab_tiles);
         DZ_LAUNCH_CHECK();
     }
     return DZ_OK;

@@ -105,15 +105,21 @@ __global__ void k_crop_scan(int* __restrict__ chunk_counts, int n_chunks, int* _
     for (int k = min(s_tot, cap) + threadIdx.x; k < cap; k += blockDim.x) idx[(size_t)t * cap + k] = -1;      // padding
 }
 
-extern "C" size_t dz_crop_points_ws_bytes(int n_pts, int n_boxes) { return (size_t)n_boxes * dz_cdiv(max(n_pts, 1), CROP_CHUNK) * 4 + 256; }
+static int crop_chunks(int n_pts) { return dz_cdiv(max(n_pts, 1), CROP_CHUNK); }
+
+// the per-(box, chunk) counts, scanned in place
+static int* carve_crop(DzCarve& cv, int n_pts, int n_boxes) { return cv.take<int>((size_t)n_boxes * crop_chunks(n_pts)); }
+
+extern "C" size_t dz_crop_points_ws_bytes(int n_pts, int n_boxes) { return dz_carve_bytes(carve_crop, n_pts, n_boxes); }
 
 extern "C" int dz_crop_points_in_boxes(const float* points, int n_pts, int pt_stride, const float* boxes, int n_boxes, int ldb,
                                        int32_t* idx, int cap, int* num, void* ws, size_t ws_bytes, dz_stream_t stream) {
     DZ_CHECK_ARG(points && boxes && idx && num && n_pts >= 0 && n_boxes >= 0 && pt_stride >= 3 && ldb >= 7 && cap >= 1);
     if (n_boxes == 0) return DZ_OK;
-    if (ws_bytes < dz_crop_points_ws_bytes(n_pts, n_boxes)) { dz_set_error("dz_crop_points_in_boxes: workspace too small"); return DZ_ERR_WORKSPACE; }
-    const int n_chunks = dz_cdiv(max(n_pts, 1), CROP_CHUNK);
-    int* cc = (int*)ws;
+    DZ_CHECK_WS(dz_crop_points_ws_bytes(n_pts, n_boxes));
+    const int n_chunks = crop_chunks(n_pts);
+    DzCarve cv((char*)ws);
+    int* cc = carve_crop(cv, n_pts, n_boxes);
     cudaStream_t st = (cudaStream_t)stream;
     dim3 grid(n_chunks, n_boxes);
     k_crop<0><<<grid, 256, 0, st>>>(points, n_pts, pt_stride, boxes, n_boxes, ldb, cc, n_chunks, idx, cap, num);

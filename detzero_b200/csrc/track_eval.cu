@@ -100,11 +100,7 @@ __host__ __device__ Ws carve(DzCarve& c, int R, int G, int O, int P) {
     return w;
 }
 
-size_t block_ws_bytes(int R, int G, int O, int P) {
-    DzCarve c(nullptr);
-    carve(c, R, G, O, P);
-    return c.bytes;
-}
+size_t block_ws_bytes(int R, int G, int O, int P) { return dz_carve_bytes(carve, R, G, O, P); }
 
 // ground-truth row g matched to prediction row p in frame f by the chain of cutoff k: counts, then the chain state of g's object
 __device__ void record_match(Shared& sh, const Ws& w, int f, int k, int g, int p, float iou) {
@@ -374,10 +370,7 @@ extern "C" int dz_track_eval(const float* pred, const int* pred_id, const int* p
                  breakdown_mask <= 3 && max_pairs >= 1 && max_pairs <= (1 << 26) && G + (long long)R < INT_MAX &&
                  (long long)max_objects * NK < INT_MAX);
     if (S == 0 || breakdown_mask == 0) return DZ_OK;
-    if (ws_bytes < dz_track_eval_ws_bytes(S, R, G, max_objects, max_pairs)) {
-        dz_set_error("dz_track_eval: workspace too small");
-        return DZ_ERR_WORKSPACE;
-    }
+    DZ_CHECK_WS(dz_track_eval_ws_bytes(S, R, G, max_objects, max_pairs));
     TeIn in{pred, pred_id, pred_cnt, gt_box, gt_obj, gt_type, gt_level, gt_cnt, num_frames, n_obj, S, F, R, G, max_objects, max_pairs,
             breakdown_mask};
     char* base = (char*)dz_align_up((size_t)ws, 256);

@@ -128,11 +128,7 @@ static __host__ __device__ Ws carve_gt(DzCarve& c, int F, int O, int T, int E, i
     return w;
 }
 
-static size_t gt_seq_ws_bytes(int F, int O, int T, int E, int P, int H) {
-    DzCarve c(nullptr);
-    carve_gt(c, F, O, T, E, P, H);
-    return c.bytes + 256;
-}
+static size_t gt_seq_ws_bytes(int F, int O, int T, int E, int P, int H) { return dz_carve_bytes(carve_gt, F, O, T, E, P, H) + 256; }
 
 __global__ void __launch_bounds__(NT, 1)
 k_track_gt(GtIn gt, TkIn tk, GtPar pr, GtOut out, char* ws_base, size_t seq_bytes) {
@@ -355,8 +351,7 @@ static int table_slots(int P) {
 }
 
 extern "C" size_t dz_track_gt_ws_bytes(int S, int F, int max_objects, int max_tracks, int max_entries, int max_pairs) {
-    return (size_t)S * dz_align_up(gt_seq_ws_bytes(F, max_objects, max_tracks, max_entries, max_pairs, table_slots(max_pairs)), 256)
-           + 256;
+    return (size_t)S * gt_seq_ws_bytes(F, max_objects, max_tracks, max_entries, max_pairs, table_slots(max_pairs)) + 256;
 }
 
 extern "C" int dz_track_gt(const float* gt_box, const double* gt_world, const int* gt_cls, const int* gt_obj, const int* gt_diff,
@@ -370,10 +365,7 @@ extern "C" int dz_track_gt(const float* gt_box, const double* gt_world, const in
                  G >= 1 && max_objects >= 1 && max_tracks >= 1 && max_entries >= 1 && max_pairs >= 1 && max_pairs <= (1 << 28) &&
                  (long long)F * G < INT_MAX);
     if (S == 0) return DZ_OK;
-    if (ws_bytes < dz_track_gt_ws_bytes(S, F, max_objects, max_tracks, max_entries, max_pairs)) {
-        dz_set_error("dz_track_gt: workspace too small");
-        return DZ_ERR_WORKSPACE;
-    }
+    DZ_CHECK_WS(dz_track_gt_ws_bytes(S, F, max_objects, max_tracks, max_entries, max_pairs));
     GtPar pr;
     pr.thr[0] = 0.f;
     for (int c = 0; c < 3; ++c) pr.thr[c + 1] = (float)thresholds[c];
@@ -381,7 +373,7 @@ extern "C" int dz_track_gt(const float* gt_box, const double* gt_world, const in
     GtIn gi{gt_box, gt_world, gt_cls, gt_obj, gt_diff, gt_npts, gt_cnt, gt_num_frames, n_obj, F, G, max_objects};
     TkIn ti{trk, n_tracks, ent_box, ent_frame, poses, max_tracks, max_entries};
     GtOut go{obj_rec, trk_rec, ent_iou, overflow};
-    const size_t seq_bytes = dz_align_up(gt_seq_ws_bytes(F, max_objects, max_tracks, max_entries, max_pairs, pr.H), 256);
+    const size_t seq_bytes = gt_seq_ws_bytes(F, max_objects, max_tracks, max_entries, max_pairs, pr.H);
     char* base = (char*)dz_align_up((size_t)ws, 256);
     k_track_gt<<<S, NT, 0, (cudaStream_t)stream>>>(gi, ti, pr, go, base, seq_bytes);
     DZ_LAUNCH_CHECK();

@@ -420,11 +420,7 @@ __host__ __device__ Seq carve(DzCarve& c, int F, int K, int T, int E) {
     return s;
 }
 
-static size_t seq_ws_bytes(int F, int K, int T, int E) {
-    DzCarve c(nullptr);
-    carve(c, F, K, T, E);
-    return c.bytes + 256;
-}
+static size_t seq_ws_bytes(int F, int K, int T, int E) { return dz_carve_bytes(carve, F, K, T, E) + 256; }
 
 __global__ void __launch_bounds__(NT, 1)
 k_track_sequences(const float* __restrict__ boxes, const int* __restrict__ counts, const int* __restrict__ num_frames,
@@ -707,7 +703,7 @@ k_track_sequences(const float* __restrict__ boxes, const int* __restrict__ count
 static size_t track_smem(int K) { return (size_t)K * (7 * 8 + 8 + 7 * 4 * 2 + 4 * 6) + K + 16; }
 
 extern "C" size_t dz_track_sequences_ws_bytes(int S, int F, int K, int max_tracks, int max_entries) {
-    return (size_t)S * dz_align_up(seq_ws_bytes(F, K, max_tracks, max_entries), 256) + 256;
+    return (size_t)S * seq_ws_bytes(F, K, max_tracks, max_entries) + 256;
 }
 
 extern "C" int dz_track_sequences(const float* boxes, const int* counts, const int* num_frames, const double* poses, int S, int F, int K,
@@ -717,10 +713,7 @@ extern "C" int dz_track_sequences(const float* boxes, const int* counts, const i
     DZ_CHECK_ARG(boxes && counts && num_frames && poses && params && trk && n_tracks && ent_box && ent_score && ent_hit && ent_frame &&
                  kept && overflow && ws && S >= 0 && F >= 1 && K >= 1 && K <= 512 && max_tracks >= 1 && max_entries >= 1);
     if (S == 0) return DZ_OK;
-    if (ws_bytes < dz_track_sequences_ws_bytes(S, F, K, max_tracks, max_entries)) {
-        dz_set_error("dz_track_sequences: workspace too small");
-        return DZ_ERR_WORKSPACE;
-    }
+    DZ_CHECK_WS(dz_track_sequences_ws_bytes(S, F, K, max_tracks, max_entries));
     Params pr;
     for (int c = 0; c < 3; ++c) {
         pr.filt[c] = params[c]; pr.s1[c] = params[3 + c]; pr.s2[c] = params[6 + c]; pr.merge[c] = params[9 + c]; pr.score[c] = params[12 + c];
@@ -730,7 +723,7 @@ extern "C" int dz_track_sequences(const float* boxes, const int* counts, const i
     DzTrackOut out{trk, n_tracks, ent_box, ent_score, ent_hit, ent_frame, kept, overflow};
     const size_t smem = track_smem(K);
     DZ_CUDA(cudaFuncSetAttribute(k_track_sequences, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const size_t seq_bytes = dz_align_up(seq_ws_bytes(F, K, max_tracks, max_entries), 256);
+    const size_t seq_bytes = seq_ws_bytes(F, K, max_tracks, max_entries);
     char* base = (char*)dz_align_up((size_t)ws, 256);
     k_track_sequences<<<S, NT, smem, (cudaStream_t)stream>>>(boxes, counts, num_frames, poses, F, K, pr, max_tracks, max_entries, out,
                                                              base, seq_bytes);

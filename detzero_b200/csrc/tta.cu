@@ -110,14 +110,12 @@ struct WbfWs {                                    // per frame F = V*K slots; cl
     int* slot_of;                                 // (B, F) first member (v*K + r) -> cluster slot
 };
 
-static WbfWs carve(void* ws, size_t bytes, int B, int F, int L, bool& ok) {
-    DzWs w(ws, bytes);
+static WbfWs carve_wbf(DzCarve& cv, int B, int F, int L) {
     WbfWs r;
     const size_t BF = (size_t)B * F;
-    r.order = w.take<int>(BF); r.seg = w.take<int>((size_t)B * (L + 1)); r.ncl = w.take<int>((size_t)B * L);
-    r.fused = w.take<float>(BF * 8); r.acc = w.take<float>(BF * 8); r.conf = w.take<double>(BF); r.cnt = w.take<int>(BF);
-    r.first = w.take<int>(BF); r.slot_of = w.take<int>(BF);
-    ok = r.order && r.seg && r.ncl && r.fused && r.acc && r.conf && r.cnt && r.first && r.slot_of;
+    r.order = cv.take<int>(BF); r.seg = cv.take<int>((size_t)B * (L + 1)); r.ncl = cv.take<int>((size_t)B * L);
+    r.fused = cv.take<float>(BF * 8); r.acc = cv.take<float>(BF * 8); r.conf = cv.take<double>(BF); r.cnt = cv.take<int>(BF);
+    r.first = cv.take<int>(BF); r.slot_of = cv.take<int>(BF);
     return r;
 }
 
@@ -338,10 +336,7 @@ static int wbf_pow2(int F) {
     return P;
 }
 
-extern "C" size_t dz_wbf_3d_ws_bytes(int B, int V, int K, int L) {
-    const size_t BF = (size_t)B * V * K;
-    return 9 * 256 + BF * (4 + 32 + 32 + 8 + 4 + 4 + 4) + (size_t)B * (2 * L + 1) * 4;
-}
+extern "C" size_t dz_wbf_3d_ws_bytes(int B, int V, int K, int L) { return dz_carve_bytes(carve_wbf, B, V * K, L); }
 
 extern "C" int dz_wbf_3d(const float* boxes, const int* counts, int B, int V, int K, const double* h_iou_thr, const double* h_skip_thr,
                          int L, float* out, int* out_count, void* ws, size_t ws_bytes, dz_stream_t stream) {
@@ -359,9 +354,9 @@ extern "C" int dz_wbf_3d(const float* boxes, const int* counts, int B, int V, in
         prm.skip_thr[l] = h_skip_thr[l];
     }
     if (B == 0) return DZ_OK;
-    bool ok;
-    WbfWs w = carve(ws, ws_bytes, B, F, L, ok);
-    if (!ok) { dz_set_error("dz_wbf_3d: workspace too small"); return DZ_ERR_WORKSPACE; }
+    DZ_CHECK_WS(dz_wbf_3d_ws_bytes(B, V, K, L));
+    DzCarve cv((char*)ws);
+    const WbfWs w = carve_wbf(cv, B, F, L);
     const int P = wbf_pow2(F);
     const size_t sort_smem = (size_t)P * 12, circ_smem = (size_t)F * sizeof(float3);
     static bool configured = false;

@@ -114,15 +114,17 @@ extern "C" size_t dz_grid_index_words(int B, int D, int H, int W) {
     return (size_t)((long long)B * dz_cells_pad(D, H, W) / 32);
 }
 
-extern "C" size_t dz_scan_ws_bytes(size_t n_words) {
-    return dz_align_up((size_t)(dz_cdiv((long long)n_words, SCAN_CHUNK) + 1) * sizeof(int), 256);
-}
+// the scan's block sums
+static int* carve_scan(DzCarve& cv, size_t n_words) { return cv.take<int>(dz_cdiv((long long)n_words, SCAN_CHUNK) + 1); }
+
+extern "C" size_t dz_scan_ws_bytes(size_t n_words) { return dz_carve_bytes(carve_scan, n_words); }
 
 extern "C" int dz_grid_index_scan(const uint32_t* bitmap, uint32_t* prefix, size_t n_words, const int* d_base,
                                   int* d_total, void* ws, size_t ws_bytes, dz_stream_t stream) {
     DZ_CHECK_ARG(bitmap && prefix && ws);
-    if (ws_bytes < dz_scan_ws_bytes(n_words)) { dz_set_error("dz_grid_index_scan: workspace too small"); return DZ_ERR_WORKSPACE; }
-    return scan_launch(bitmap, prefix, n_words, d_base, d_total, (int*)ws, (cudaStream_t)stream);
+    DZ_CHECK_WS(dz_scan_ws_bytes(n_words));
+    DzCarve cv((char*)ws);
+    return scan_launch(bitmap, prefix, n_words, d_base, d_total, carve_scan(cv, n_words), (cudaStream_t)stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -158,11 +160,12 @@ extern "C" int dz_grid_index_from_coords(const int32_t* coords, const int* d_n, 
     DZ_CHECK_ARG(coords && d_n && bitmap && prefix && cap >= 0);
     cudaStream_t st = (cudaStream_t)stream;
     size_t n_words = dz_grid_index_words(B, D, H, W);
-    if (ws_bytes < dz_scan_ws_bytes(n_words)) { dz_set_error("dz_grid_index_from_coords: workspace too small"); return DZ_ERR_WORKSPACE; }
+    DZ_CHECK_WS(dz_scan_ws_bytes(n_words));
     long long cp = dz_cells_pad(D, H, W);
     int blocks = max(1, min(dz_cdiv(cap, 256), DZ_NUM_SMS * 8));
+    DzCarve cv((char*)ws);
     k_coords_mark<<<blocks, 256, 0, st>>>(coords, d_n, cap, D, H, W, cp, bitmap);
-    int rc = scan_launch(bitmap, prefix, n_words, nullptr, d_total, (int*)ws, st);
+    int rc = scan_launch(bitmap, prefix, n_words, nullptr, d_total, carve_scan(cv, n_words), st);
     if (rc) return rc;
     if (perm) k_coords_perm<<<blocks, 256, 0, st>>>(coords, d_n, cap, D, H, W, cp, bitmap, prefix, perm);
     DZ_LAUNCH_CHECK();
@@ -372,18 +375,23 @@ __global__ void k_vox_finish(const int* __restrict__ d_tmp, int max_voxels, int 
     }
 }
 
-// scan of the leader block sums (single block) writing the total into d_tmp[1]
+// one frame of n points (a frame of no points still gets one slot of each array) and at most max_voxels point lists;
+// d_tmp: [0] occupied cells up to this frame, [1] voxels of this frame
+struct VoxWs { uint32_t *cell, *rnk; int *first_idx, *lists, *scan_sums, *lead_sums, *d_tmp; size_t nn; int L, lead_blocks; };
+
+static VoxWs carve_vox(DzCarve& cv, int n, int max_pts, int max_voxels, size_t frame_words) {
+    VoxWs w;
+    w.nn = (size_t)max(n, 1); w.L = n < max_voxels ? max(n, 1) : max_voxels; w.lead_blocks = max(1, dz_cdiv(n, LEAD_CHUNK));
+    w.cell = cv.take<uint32_t>(w.nn); w.rnk = cv.take<uint32_t>(w.nn); w.first_idx = cv.take<int>(w.nn);
+    w.lists = cv.take<int>((size_t)w.L * max_pts);
+    w.scan_sums = carve_scan(cv, frame_words);
+    w.lead_sums = cv.take<int>(w.lead_blocks + 1);
+    w.d_tmp = cv.take<int>(4);
+    return w;
+}
+
 extern "C" size_t dz_voxelize_hard_ws_bytes(int n_points, int max_pts, int max_voxels, int iD, int iH, int iW) {
-    size_t n = (size_t)(n_points > 0 ? n_points : 1);
-    size_t L = (size_t)(n_points < max_voxels ? (n_points > 0 ? n_points : 1) : max_voxels);
-    size_t frame_words = (size_t)(dz_cells_pad(iD, iH, iW) / 32);
-    size_t b = 0;
-    b += dz_align_up(n * 4, 256) * 3;                            // cell, rnk, first_idx
-    b += dz_align_up(L * max_pts * 4, 256);                      // lists
-    b += dz_scan_ws_bytes(frame_words);                          // bitmap scan block sums
-    b += dz_align_up((size_t)(dz_cdiv((long long)n, LEAD_CHUNK) + 1) * 4, 256);
-    b += 256;                                                    // tmp ints
-    return b;
+    return dz_carve_bytes(carve_vox, n_points, max_pts, max_voxels, (size_t)(dz_cells_pad(iD, iH, iW) / 32));
 }
 
 extern "C" int dz_voxelize_hard(const float* points, int n, int point_stride, int xyz_off, int c,
@@ -397,49 +405,36 @@ extern "C" int dz_voxelize_hard(const float* points, int n, int point_stride, in
     DZ_CHECK_ARG(n >= 0 && c >= 1 && xyz_off >= 0 && xyz_off + c <= point_stride && point_stride <= VOX_MAX_STRIDE && c >= 3);
     DZ_CHECK_ARG(max_pts >= 1 && max_voxels >= 1 && batch_idx >= 0 && batch_idx < B);
     DZ_CHECK_ARG(grid_zyx3[0] <= iD && grid_zyx3[1] <= iH && grid_zyx3[2] <= iW);
-    if (ws_bytes < dz_voxelize_hard_ws_bytes(n, max_pts, max_voxels, iD, iH, iW)) {
-        dz_set_error("dz_voxelize_hard: workspace too small"); return DZ_ERR_WORKSPACE;
-    }
+    DZ_CHECK_WS(dz_voxelize_hard_ws_bytes(n, max_pts, max_voxels, iD, iH, iW));
     cudaStream_t st = (cudaStream_t)stream;
     VoxGeom g;
     for (int d = 0; d < 3; ++d) { g.lo[d] = range6[d]; g.vs[d] = vsize3[d]; g.grid[d] = grid_zyx3[2 - d]; }
     g.iD = iD; g.iH = iH; g.iW = iW; g.cells_pad = dz_cells_pad(iD, iH, iW);
     size_t frame_words = (size_t)(g.cells_pad / 32);
-    size_t nn = (size_t)(n > 0 ? n : 1);
-    int L = n < max_voxels ? (n > 0 ? n : 1) : max_voxels;
+    DzCarve cv((char*)ws);
+    const VoxWs w = carve_vox(cv, n, max_pts, max_voxels, frame_words);
 
-    DzWs w(ws, ws_bytes);
-    uint32_t* cell = w.take<uint32_t>(nn);
-    uint32_t* rnk = w.take<uint32_t>(nn);
-    int* first_idx = w.take<int>(nn);
-    int* lists = w.take<int>((size_t)L * max_pts);
-    int* scan_sums = (int*)w.take<char>(dz_scan_ws_bytes(frame_words));
-    int n_lead_blocks = max(1, dz_cdiv(n, LEAD_CHUNK));
-    int* lead_sums = w.take<int>(n_lead_blocks + 1);
-    int* d_tmp = w.take<int>(4);
-    if (!d_tmp) { dz_set_error("dz_voxelize_hard: workspace carve failed"); return DZ_ERR_WORKSPACE; }
-
-    DZ_CUDA(cudaMemsetAsync(first_idx, 0x7f, nn * 4, st));
-    DZ_CUDA(cudaMemsetAsync(lists, 0x7f, (size_t)L * max_pts * 4, st));
+    DZ_CUDA(cudaMemsetAsync(w.first_idx, 0x7f, w.nn * 4, st));
+    DZ_CUDA(cudaMemsetAsync(w.lists, 0x7f, (size_t)w.L * max_pts * 4, st));
     int pblocks = max(1, dz_cdiv(n, VOX_THREADS));
     uint32_t* bm_frame = index_bitmap + (size_t)batch_idx * frame_words;
     uint32_t* pf_frame = index_prefix + (size_t)batch_idx * frame_words;
 
-    k_vox_mark<<<pblocks, VOX_THREADS, 0, st>>>(points, n, point_stride, xyz_off, g, batch_idx, index_bitmap, cell);
+    k_vox_mark<<<pblocks, VOX_THREADS, 0, st>>>(points, n, point_stride, xyz_off, g, batch_idx, index_bitmap, w.cell);
     // prefix of this frame's words, continuing the rank count of previous frames (d_counters[1])
-    int rc = scan_launch(bm_frame, pf_frame, frame_words, d_counters + 1, d_tmp + 0, scan_sums, st);
+    int rc = scan_launch(bm_frame, pf_frame, frame_words, d_counters + 1, w.d_tmp + 0, w.scan_sums, st);
     if (rc) return rc;
-    k_vox_first<<<pblocks, VOX_THREADS, 0, st>>>(cell, n, (long long)batch_idx * g.cells_pad, index_bitmap, index_prefix,
-                                                 d_counters, first_idx, rnk);
-    k_vox_lead_count<<<n_lead_blocks, VOX_THREADS, 0, st>>>(cell, rnk, first_idx, n, lead_sums);
-    k_scan_offsets<<<1, 1024, 0, st>>>(lead_sums, n_lead_blocks, nullptr, d_tmp + 1);
-    k_vox_lead_emit<<<n_lead_blocks, VOX_THREADS, 0, st>>>(cell, rnk, first_idx, n, lead_sums, g, batch_idx, max_voxels, cap,
+    k_vox_first<<<pblocks, VOX_THREADS, 0, st>>>(w.cell, n, (long long)batch_idx * g.cells_pad, index_bitmap, index_prefix,
+                                                 d_counters, w.first_idx, w.rnk);
+    k_vox_lead_count<<<w.lead_blocks, VOX_THREADS, 0, st>>>(w.cell, w.rnk, w.first_idx, n, w.lead_sums);
+    k_scan_offsets<<<1, 1024, 0, st>>>(w.lead_sums, w.lead_blocks, nullptr, w.d_tmp + 1);
+    k_vox_lead_emit<<<w.lead_blocks, VOX_THREADS, 0, st>>>(w.cell, w.rnk, w.first_idx, n, w.lead_sums, g, batch_idx, max_voxels, cap,
                                                            d_counters, coords, index_perm);
-    k_vox_slots<<<pblocks, VOX_THREADS, 0, st>>>(cell, rnk, n, index_perm, d_counters, max_pts, L, lists);
-    k_vox_write<<<max(1, dz_cdiv(L, VOX_THREADS)), VOX_THREADS, 0, st>>>(points, point_stride, xyz_off, c, lists, L, max_pts,
-                                                                         max_voxels, cap, d_tmp, d_counters, voxels,
+    k_vox_slots<<<pblocks, VOX_THREADS, 0, st>>>(w.cell, w.rnk, n, index_perm, d_counters, max_pts, w.L, w.lists);
+    k_vox_write<<<max(1, dz_cdiv(w.L, VOX_THREADS)), VOX_THREADS, 0, st>>>(points, point_stride, xyz_off, c, w.lists, w.L, max_pts,
+                                                                         max_voxels, cap, w.d_tmp, d_counters, voxels,
                                                                          num_per_voxel, mean);
-    k_vox_finish<<<1, 32, 0, st>>>(d_tmp, max_voxels, cap, d_counters);
+    k_vox_finish<<<1, 32, 0, st>>>(w.d_tmp, max_voxels, cap, d_counters);
     DZ_LAUNCH_CHECK();
     return DZ_OK;
 }
@@ -471,8 +466,19 @@ __global__ void k_vb_pub_vid(const int* __restrict__ d_tmp, const int* __restric
     }
 }
 
+// B frame slices of frame_bytes each (a frame is carved in its slice with its own point count), then the running totals
+// ctr: (B+1) x {row base, rank base, rows wanted, pad}
+struct VbWs { char* frames; int* ctr; };
+
+static VbWs carve_vb(DzCarve& cv, int B, size_t frame_bytes) {
+    VbWs w;
+    w.frames = cv.take<char>((size_t)B * frame_bytes);
+    w.ctr = cv.take<int>((size_t)(B + 1) * 4);
+    return w;
+}
+
 extern "C" size_t dz_voxelize_hard_batch_ws_bytes(int n_max, int B, int max_pts, int max_voxels, int iD, int iH, int iW) {
-    return (size_t)B * dz_align_up(dz_voxelize_hard_ws_bytes(n_max, max_pts, max_voxels, iD, iH, iW), 256) + dz_align_up((size_t)(B + 1) * 16, 256);
+    return dz_carve_bytes(carve_vb, B, dz_voxelize_hard_ws_bytes(n_max, max_pts, max_voxels, iD, iH, iW));
 }
 
 extern "C" int dz_voxelize_hard_batch(const float* const* points_host, const int* n_host, int B, int point_stride, int xyz_off, int c,
@@ -485,9 +491,7 @@ extern "C" int dz_voxelize_hard_batch(const float* const* points_host, const int
     DZ_CHECK_ARG(max_pts >= 1 && max_voxels >= 1 && grid_zyx3[0] <= iD && grid_zyx3[1] <= iH && grid_zyx3[2] <= iW);
     int n_max = 0;
     for (int b = 0; b < B; ++b) { DZ_CHECK_ARG(n_host[b] >= 0 && (points_host[b] || n_host[b] == 0)); n_max = max(n_max, n_host[b]); }
-    if (ws_bytes < dz_voxelize_hard_batch_ws_bytes(n_max, B, max_pts, max_voxels, iD, iH, iW)) {
-        dz_set_error("dz_voxelize_hard_batch: workspace too small"); return DZ_ERR_WORKSPACE;
-    }
+    DZ_CHECK_WS(dz_voxelize_hard_batch_ws_bytes(n_max, B, max_pts, max_voxels, iD, iH, iW));
     cudaStream_t st = (cudaStream_t)stream;
     if (!g_vb.init) {
         for (int i = 0; i < VB_STREAMS; ++i) {
@@ -505,10 +509,10 @@ extern "C" int dz_voxelize_hard_batch(const float* const* points_host, const int
     for (int d = 0; d < 3; ++d) { g.lo[d] = range6[d]; g.vs[d] = vsize3[d]; g.grid[d] = grid_zyx3[2 - d]; }
     g.iD = iD; g.iH = iH; g.iW = iW; g.cells_pad = dz_cells_pad(iD, iH, iW);
     const size_t frame_words = (size_t)(g.cells_pad / 32);
-    const size_t per_frame = dz_align_up(dz_voxelize_hard_ws_bytes(n_max, max_pts, max_voxels, iD, iH, iW), 256);
-    unsigned char* wsb = reinterpret_cast<unsigned char*>(ws);
-    int* ctr = reinterpret_cast<int*>(wsb + (size_t)B * per_frame);          // (B+1) x {row base, rank base, rows wanted, pad}
-    DZ_CUDA(cudaMemcpyAsync(ctr, d_counters, 12, cudaMemcpyDeviceToDevice, st));
+    const size_t frame_bytes = dz_voxelize_hard_ws_bytes(n_max, max_pts, max_voxels, iD, iH, iW);
+    DzCarve cv((char*)ws);
+    const VbWs vw = carve_vb(cv, B, frame_bytes);
+    DZ_CUDA(cudaMemcpyAsync(vw.ctr, d_counters, 12, cudaMemcpyDeviceToDevice, st));
     DZ_CUDA(cudaEventRecord(g_vb.fork, st));
     const int S = min(B, VB_STREAMS);
     for (int i = 0; i < S; ++i) DZ_CUDA(cudaStreamWaitEvent(g_vb.s[i], g_vb.fork, 0));
@@ -516,47 +520,37 @@ extern "C" int dz_voxelize_hard_batch(const float* const* points_host, const int
         cudaStream_t s = g_vb.s[b % S];
         const float* points = points_host[b];
         const int n = n_host[b];
-        const size_t nn = (size_t)(n > 0 ? n : 1);
-        const int L = n < max_voxels ? (n > 0 ? n : 1) : max_voxels;
-        DzWs w(wsb + (size_t)b * per_frame, per_frame);
-        uint32_t* cell = w.take<uint32_t>(nn);
-        uint32_t* rnk = w.take<uint32_t>(nn);
-        int* first_idx = w.take<int>(nn);
-        int* lists = w.take<int>((size_t)L * max_pts);
-        int* scan_sums = (int*)w.take<char>(dz_scan_ws_bytes(frame_words));
-        const int n_lead_blocks = max(1, dz_cdiv(n, LEAD_CHUNK));
-        int* lead_sums = w.take<int>(n_lead_blocks + 1);
-        int* d_tmp = w.take<int>(4);
-        if (!d_tmp) { dz_set_error("dz_voxelize_hard_batch: workspace carve failed"); return DZ_ERR_WORKSPACE; }
-        int* ctr_b = ctr + 4 * b;
-        int* ctr_n = ctr + 4 * (b + 1);
-        DZ_CUDA(cudaMemsetAsync(first_idx, 0x7f, nn * 4, s));
-        DZ_CUDA(cudaMemsetAsync(lists, 0x7f, (size_t)L * max_pts * 4, s));
+        DzCarve fc(vw.frames + (size_t)b * frame_bytes);
+        const VoxWs w = carve_vox(fc, n, max_pts, max_voxels, frame_words);
+        int* ctr_b = vw.ctr + 4 * b;
+        int* ctr_n = vw.ctr + 4 * (b + 1);
+        DZ_CUDA(cudaMemsetAsync(w.first_idx, 0x7f, w.nn * 4, s));
+        DZ_CUDA(cudaMemsetAsync(w.lists, 0x7f, (size_t)w.L * max_pts * 4, s));
         const int pblocks = max(1, dz_cdiv(n, VOX_THREADS));
         uint32_t* bm_frame = index_bitmap + (size_t)b * frame_words;
         uint32_t* pf_frame = index_prefix + (size_t)b * frame_words;
-        k_vox_mark<<<pblocks, VOX_THREADS, 0, s>>>(points, n, point_stride, xyz_off, g, b, index_bitmap, cell);
+        k_vox_mark<<<pblocks, VOX_THREADS, 0, s>>>(points, n, point_stride, xyz_off, g, b, index_bitmap, w.cell);
         if (b > 0) DZ_CUDA(cudaStreamWaitEvent(s, g_vb.rank_ev[b - 1], 0));       // ctr_b[1] = cells of the frames before
-        int rc = scan_launch(bm_frame, pf_frame, frame_words, ctr_b + 1, d_tmp + 0, scan_sums, s);
+        int rc = scan_launch(bm_frame, pf_frame, frame_words, ctr_b + 1, w.d_tmp + 0, w.scan_sums, s);
         if (rc) return rc;
-        k_vb_pub_rank<<<1, 32, 0, s>>>(d_tmp, ctr_n);
+        k_vb_pub_rank<<<1, 32, 0, s>>>(w.d_tmp, ctr_n);
         DZ_CUDA(cudaEventRecord(g_vb.rank_ev[b], s));
-        k_vox_first<<<pblocks, VOX_THREADS, 0, s>>>(cell, n, (long long)b * g.cells_pad, index_bitmap, index_prefix, ctr_b, first_idx, rnk);
-        k_vox_lead_count<<<n_lead_blocks, VOX_THREADS, 0, s>>>(cell, rnk, first_idx, n, lead_sums);
-        k_scan_offsets<<<1, 1024, 0, s>>>(lead_sums, n_lead_blocks, nullptr, d_tmp + 1);
+        k_vox_first<<<pblocks, VOX_THREADS, 0, s>>>(w.cell, n, (long long)b * g.cells_pad, index_bitmap, index_prefix, ctr_b, w.first_idx, w.rnk);
+        k_vox_lead_count<<<w.lead_blocks, VOX_THREADS, 0, s>>>(w.cell, w.rnk, w.first_idx, n, w.lead_sums);
+        k_scan_offsets<<<1, 1024, 0, s>>>(w.lead_sums, w.lead_blocks, nullptr, w.d_tmp + 1);
         if (b > 0) DZ_CUDA(cudaStreamWaitEvent(s, g_vb.vid_ev[b - 1], 0));        // ctr_b[0], ctr_b[2] = rows of the frames before
-        k_vb_pub_vid<<<1, 32, 0, s>>>(d_tmp, ctr_b, max_voxels, cap, ctr_n);
+        k_vb_pub_vid<<<1, 32, 0, s>>>(w.d_tmp, ctr_b, max_voxels, cap, ctr_n);
         DZ_CUDA(cudaEventRecord(g_vb.vid_ev[b], s));
-        k_vox_lead_emit<<<n_lead_blocks, VOX_THREADS, 0, s>>>(cell, rnk, first_idx, n, lead_sums, g, b, max_voxels, cap, ctr_b, coords, index_perm);
-        k_vox_slots<<<pblocks, VOX_THREADS, 0, s>>>(cell, rnk, n, index_perm, ctr_b, max_pts, L, lists);
-        k_vox_write<<<max(1, dz_cdiv(L, VOX_THREADS)), VOX_THREADS, 0, s>>>(points, point_stride, xyz_off, c, lists, L, max_pts, max_voxels, cap,
-                                                                           d_tmp, ctr_b, voxels, num_per_voxel, mean);
+        k_vox_lead_emit<<<w.lead_blocks, VOX_THREADS, 0, s>>>(w.cell, w.rnk, w.first_idx, n, w.lead_sums, g, b, max_voxels, cap, ctr_b, coords, index_perm);
+        k_vox_slots<<<pblocks, VOX_THREADS, 0, s>>>(w.cell, w.rnk, n, index_perm, ctr_b, max_pts, w.L, w.lists);
+        k_vox_write<<<max(1, dz_cdiv(w.L, VOX_THREADS)), VOX_THREADS, 0, s>>>(points, point_stride, xyz_off, c, w.lists, w.L, max_pts, max_voxels, cap,
+                                                                           w.d_tmp, ctr_b, voxels, num_per_voxel, mean);
     }
     for (int i = 0; i < S; ++i) {
         DZ_CUDA(cudaEventRecord(g_vb.done[i], g_vb.s[i]));
         DZ_CUDA(cudaStreamWaitEvent(st, g_vb.done[i], 0));
     }
-    DZ_CUDA(cudaMemcpyAsync(d_counters, ctr + 4 * B, 12, cudaMemcpyDeviceToDevice, st));
+    DZ_CUDA(cudaMemcpyAsync(d_counters, vw.ctr + 4 * B, 12, cudaMemcpyDeviceToDevice, st));
     DZ_LAUNCH_CHECK();
     return DZ_OK;
 }
@@ -679,12 +673,25 @@ static size_t dyn_sort_bytes(int n) {
     return bytes;
 }
 
+struct DynWs { uint32_t *bitmap, *prefix; long long* cell; uint32_t *key, *key_sorted; int *idx, *idx_sorted, *beg, *end, *sums;
+                void* sort_tmp; size_t sort_bytes; };
+
+static DynWs carve_dyn(DzCarve& cv, int n, int cap, size_t words) {
+    const size_t nn = (size_t)max(n, 1);
+    DynWs w;
+    w.bitmap = cv.take<uint32_t>(words); w.prefix = cv.take<uint32_t>(words);
+    w.cell = cv.take<long long>(nn);
+    w.key = cv.take<uint32_t>(nn); w.key_sorted = cv.take<uint32_t>(nn);
+    w.idx = cv.take<int>(nn); w.idx_sorted = cv.take<int>(nn);
+    w.beg = cv.take<int>(cap); w.end = cv.take<int>(cap);
+    w.sort_bytes = dyn_sort_bytes(max(n, 0));
+    w.sort_tmp = cv.take<char>(max(w.sort_bytes, (size_t)1));
+    w.sums = carve_scan(cv, words);
+    return w;
+}
+
 extern "C" size_t dz_voxelize_dynamic_ws_bytes(int n_points, int cap, int B, int X, int Y, int Z) {
-    size_t words = (size_t)((long long)B * dz_cells_pad(X, Y, Z) / 32);
-    size_t n = (size_t)(n_points > 0 ? n_points : 1);
-    return dz_align_up(words * 4, 256) * 2 + dz_align_up(n * 8, 256) + dz_align_up(n * 4, 256) * 4 +
-           dz_align_up((size_t)cap * 4, 256) * 2 + dz_align_up(dyn_sort_bytes(n_points > 0 ? n_points : 0), 256) +
-           dz_scan_ws_bytes(words) + 256;
+    return dz_carve_bytes(carve_dyn, n_points, cap, (size_t)((long long)B * dz_cells_pad(X, Y, Z) / 32));
 }
 
 // Every voxel's mean is summed in ascending point index, so the result does not depend on launch timing: the same frame gives
@@ -694,40 +701,25 @@ extern "C" int dz_voxelize_dynamic_mean(const float* points, int n, int c, int B
                                         const int* grid_xyz3, float* feats, int32_t* coords, int cap, int* d_m,
                                         void* ws, size_t ws_bytes, dz_stream_t stream) {
     DZ_CHECK_ARG((points || n == 0) && feats && coords && d_m && n >= 0 && c >= 3 && 1 + c <= VOX_MAX_STRIDE && B >= 1 && cap >= 1);
-    if (ws_bytes < dz_voxelize_dynamic_ws_bytes(n, cap, B, grid_xyz3[0], grid_xyz3[1], grid_xyz3[2])) {
-        dz_set_error("dz_voxelize_dynamic_mean: workspace too small"); return DZ_ERR_WORKSPACE;
-    }
+    DZ_CHECK_WS(dz_voxelize_dynamic_ws_bytes(n, cap, B, grid_xyz3[0], grid_xyz3[1], grid_xyz3[2]));
     cudaStream_t st = (cudaStream_t)stream;
     DynGeom g;
     for (int d = 0; d < 3; ++d) { g.lo[d] = range6[d]; g.vs[d] = vsize3[d]; g.grid[d] = grid_xyz3[d]; }
     g.cells_pad = dz_cells_pad(g.grid[0], g.grid[1], g.grid[2]);
     size_t words = (size_t)((long long)B * g.cells_pad / 32);
-    size_t nn = (size_t)(n > 0 ? n : 1);
-    size_t sort_bytes = dyn_sort_bytes(n);
-    DzWs w(ws, ws_bytes);
-    uint32_t* bitmap = w.take<uint32_t>(words);
-    uint32_t* prefix = w.take<uint32_t>(words);
-    long long* cell = w.take<long long>(nn);
-    uint32_t* key = w.take<uint32_t>(nn);
-    uint32_t* key_sorted = w.take<uint32_t>(nn);
-    int* idx = w.take<int>(nn);
-    int* idx_sorted = w.take<int>(nn);
-    int* beg = w.take<int>(cap);
-    int* end = w.take<int>(cap);
-    void* sort_tmp = w.take<char>(sort_bytes > 0 ? sort_bytes : 1);
-    int* sums = (int*)w.take<char>(dz_scan_ws_bytes(words));
-    if (!sums) { dz_set_error("dz_voxelize_dynamic_mean: workspace carve failed"); return DZ_ERR_WORKSPACE; }
-    DZ_CUDA(cudaMemsetAsync(bitmap, 0, words * 4, st));
+    DzCarve cv((char*)ws);
+    DynWs w = carve_dyn(cv, n, cap, words);
+    DZ_CUDA(cudaMemsetAsync(w.bitmap, 0, words * 4, st));
     int pblocks = max(1, dz_cdiv(n, VOX_THREADS));
-    k_dyn_mark<<<pblocks, VOX_THREADS, 0, st>>>(points, n, 1 + c, g, B, bitmap, cell);
-    int rc = scan_launch(bitmap, prefix, words, nullptr, d_m, sums, st);
+    k_dyn_mark<<<pblocks, VOX_THREADS, 0, st>>>(points, n, 1 + c, g, B, w.bitmap, w.cell);
+    int rc = scan_launch(w.bitmap, w.prefix, words, nullptr, d_m, w.sums, st);
     if (rc) return rc;
     if (n > 0) {
-        k_dyn_key<<<pblocks, VOX_THREADS, 0, st>>>(cell, n, bitmap, prefix, key, idx);
-        DZ_CUDA(cub::DeviceRadixSort::SortPairs(sort_tmp, sort_bytes, key, key_sorted, idx, idx_sorted, n, 0, dyn_key_bits(n), st));
-        k_dyn_runs<<<pblocks, VOX_THREADS, 0, st>>>(key_sorted, idx_sorted, n, cell, g, d_m, cap, beg, end, coords);
+        k_dyn_key<<<pblocks, VOX_THREADS, 0, st>>>(w.cell, n, w.bitmap, w.prefix, w.key, w.idx);
+        DZ_CUDA(cub::DeviceRadixSort::SortPairs(w.sort_tmp, w.sort_bytes, w.key, w.key_sorted, w.idx, w.idx_sorted, n, 0, dyn_key_bits(n), st));
+        k_dyn_runs<<<pblocks, VOX_THREADS, 0, st>>>(w.key_sorted, w.idx_sorted, n, w.cell, g, d_m, cap, w.beg, w.end, coords);
     }
-    k_dyn_mean<<<DZ_NUM_SMS * 4, 256, 0, st>>>(points, 1 + c, c, idx_sorted, beg, end, d_m, cap, feats);
+    k_dyn_mean<<<DZ_NUM_SMS * 4, 256, 0, st>>>(points, 1 + c, c, w.idx_sorted, w.beg, w.end, d_m, cap, feats);
     DZ_LAUNCH_CHECK();
     return DZ_OK;
 }
