@@ -75,6 +75,14 @@ _SIGS = {
     'dz_refine_inputs': (ci, [ci, vp, ci, vp, ci, ci, vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, ctypes.c_double, ci, ci,
                               ctypes.c_uint64, vp, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]),
     'dz_refine_revert': (ci, [ci, vp, vp, ci, vp, vp, vp, ci, ci, vp, vp, vp]),
+    'dz_crop_tracks_ws_bytes': (sz, [ci, ci, ci]),
+    'dz_crop_tracks': (ci, [vp, ci, ci, vp, ci, ci, vp, vp, vp, vp, ci, ci, ctypes.c_double, ci, vp, vp, vp, vp, sz, vp]),
+    'dz_refine_train_draw_ws_bytes': (sz, [ci, ci]),
+    'dz_refine_train_draw': (ci, [ci, vp, vp, vp, ci, ci, ci, ctypes.c_uint64, ctypes.c_longlong, vp, vp, vp, vp, vp, vp, sz, vp]),
+    'dz_refine_train_inputs_ws_bytes': (sz, [ci, ci, ci, ci, ci, ci, ci]),
+    'dz_refine_train_inputs': (ci, [ci, vp, ci, vp, ci, ci, vp, vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ctypes.c_double,
+                                    ci, ci, ctypes.c_uint64, ctypes.c_longlong, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp,
+                                    vp, vp, vp, sz, vp]),
     'dz_combine_frames_ws_bytes': (sz, [ci, ci, ci]),
     'dz_combine_frames': (ci, [vp, vp, vp, vp, vp, vp, vp, ci, ci, vp, vp, vp, ci, ci, ci, vp, vp, vp, vp, vp, sz, vp]),
     'dz_refine_targets': (ci, [vp, vp, vp, ci, ci, vp, vp, vp, vp, vp, vp, ci, ci, vp, vp, vp, vp, vp, vp]),

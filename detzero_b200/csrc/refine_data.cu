@@ -32,12 +32,32 @@
 //   3. GRM's query count is min(nq, L) per track (the reference lowers self.query_num for every later track).
 //   4. The crop tests each point in float64 world coordinates relative to the box centre (rounded to float32 for the shared
 //      float32 test), where the reference tests float32 world points: only points within ~1e-3 m of an enlarged face can differ.
+//
+// Training samples (the training branch of WaymoGeometryDataset / WaymoConfidenceDataset.extract_track_feature, with
+// geometry_augment.py:65-77 augment_single_box for the GRM; restated in oracle/refine_train_data_ref.py):
+//   crop    dz_crop_tracks runs prep / count / scan / write once and copies every in-box point row to a frame of its own (one pose
+//           per box), the layout the builders read with crop = 0, so the crop leaves the epoch loop.
+//   draw    k_rd_draw, one block per track, keyed on (epoch_seed(seed, epoch), track_uid) with the streams ST_TR_*:
+//             eligible slots: the matched ones (GRM), every valid one (CRM); m of them
+//             kept count n = lo + key mod (m - lo + 1), lo = min(5, m), key = mix64(key_base(.., 0, ST_TR_COUNT)): the bias of a
+//               64-bit key reduced mod at most 200 is below 200 / 2^64 < 2^-56
+//             kept: the k-subset rule of select (k = n of the m eligible ranks), in ascending slot order
+//             GRM queries: min(nq, n) kept positions by the same rule; CRM init box: a kept position, key mod n (ST_TR_INIT)
+//             GRM flip bits: the top bit of key(i) of ST_TR_FLIP per kept position i
+//           epoch_seed(seed, epoch) = mix64(mix64(seed) + epoch); the point samples of a training build use it as their seed.
+//   build   dz_refine_train_inputs gathers the kept slots into a derived track table and runs the passes above on it, with the
+//           drawn query positions in k_rd_track (GRM), the drawn init box in k_rd_prep (CRM) and the flip applied to box-local y
+//           of the memory rows in the write pass (GRM; the query points are never flipped, as the reference copies them first).
+//   Deviation 5: the reference keeps random.sample's order of the kept boxes; here they are in ascending slot order.  Every
+//   consumer is invariant to the order of a track's boxes (per-box encoders, max-pools, BatchNorm statistics, decoder attention
+//   over the memory, summed losses), so no distribution the model sees changes.
 #include "common.cuh"
 #include "boxgeom.cuh"
 #include "refine_frame.cuh"
 
-enum { RD_PRM = 0, RD_CRM = 1, RD_GRM = 2 };
+enum { RD_PRM = 0, RD_CRM = 1, RD_GRM = 2, RD_CROP = 3 };
 enum { ST_PRM_Q = 0, ST_PRM_M = 1, ST_CRM = 2, ST_GRM_Q = 3, ST_GRM_M = 4 };
+enum { ST_TR_COUNT = 5, ST_TR_KEEP = 6, ST_TR_QUERY = 7, ST_TR_INIT = 8, ST_TR_FLIP = 9 };
 static constexpr int RD_CHUNK = 4096;              // points of a frame per count / write block
 
 struct RdBox {
@@ -57,6 +77,11 @@ struct RdParams {
     int B, L, kind, with_class, C, kq, km, nq, qout, crop, bev; double enlarge; unsigned long long seed;
     RdBox* bx; int* cc; int n_chunks; int* n; int* goff; int* gtot; int* qidx; int* qnum; int* sel;
     float* q_pts; float* m_pts; float* traj; float* box_f; float* track_f; int* query_num;
+    // training builds (NULL otherwise): drawn GRM query positions (B, nq), CRM init positions (B), GRM flip bits (B, L); the
+    // derived gt_geo_trajectory (B, L, 7) f32 and gt_geo_query_boxes (B, qout, 7)
+    const int* qsel; const int* init; const unsigned char* flip; const float* gt_traj; float* gt_box_f;
+    // dz_crop_tracks: the first output row of each box slot, the output rows (width C)
+    const int* rbase; float* rows;
 };
 
 __host__ __device__ __forceinline__ unsigned long long mix64(unsigned long long z) {
@@ -64,6 +89,10 @@ __host__ __device__ __forceinline__ unsigned long long mix64(unsigned long long 
     z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
     z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
     return z ^ (z >> 31);
+}
+
+__host__ __device__ __forceinline__ unsigned long long epoch_seed(unsigned long long seed, long long epoch) {
+    return mix64(mix64(seed) + (unsigned long long)epoch);
 }
 
 __device__ __forceinline__ unsigned long long key_base(unsigned long long seed, long long uid, int slot, int stream) {
@@ -107,8 +136,9 @@ __global__ void k_rd_prep(RdParams P) {
     o.crop[6] = (float)bw[6];
     o.p0 = P.foff[f];
     o.p1 = P.foff[f + 1];
-    o.score = P.scores[t];
+    o.score = P.scores ? P.scores[t] : 0.f;
     for (int d = 0; d < 12; ++d) o.E[d] = 0.0;
+    if (P.kind == RD_CROP) return;
     if (P.kind == RD_GRM) {                                              // local_coords_transform: rotate by -heading
         const double c = cos(bw[6]), s = sin(bw[6]);
         o.E[0] = c; o.E[1] = s; o.E[4] = -s; o.E[5] = c; o.E[10] = 1.0;
@@ -116,8 +146,9 @@ __global__ void k_rd_prep(RdParams P) {
         for (int d = 0; d < 7; ++d) P.traj[(size_t)t * 7 + d] = (float)bw[d];
         return;
     }
-    // init_coords_transform: init box = traj[L // 2] (heading wrapped); trajectory into its frame
-    const double* bi = P.boxes + ((size_t)b * P.L + L / 2) * 7;
+    // init_coords_transform: init box = traj[L // 2] (heading wrapped), or the drawn one of a training build; trajectory into its frame
+    const int ii = P.init ? min(max(P.init[b], 0), L - 1) : L / 2;
+    const double* bi = P.boxes + ((size_t)b * P.L + ii) * 7;
     const InitFrame fr = init_frame(bi);
     const double yi = fr.yaw, c = fr.c, s = fr.s;
     o.E[0] = c; o.E[1] = s; o.E[4] = -s; o.E[5] = c; o.E[10] = 1.0;
@@ -168,6 +199,11 @@ __device__ __forceinline__ int find_rank(const int* list, int m, int r) {       
 __device__ void write_point(const RdParams& P, const RdBox& bx, int t, int r, int p, int qi, int goff) {
     const int b = t / P.L, j = t % P.L, n = P.n[t];
     const float* q = P.pts + (size_t)p * P.pstride;
+    if (P.kind == RD_CROP) {
+        float* o = P.rows + ((size_t)P.rbase[t] + r) * P.C;
+        for (int d = 0; d < P.C; ++d) o[d] = q[d];
+        return;
+    }
     const double x = q[1], y = q[2], z = q[3];
     double g[3], e[3];
     for (int d = 0; d < 3; ++d) g[d] = bx.G[d * 4] * x + bx.G[d * 4 + 1] * y + bx.G[d * 4 + 2] * z + bx.G[d * 4 + 3];
@@ -181,6 +217,7 @@ __device__ void write_point(const RdParams& P, const RdBox& bx, int t, int r, in
                 o[0] = (float)e[0]; o[1] = (float)e[1]; o[2] = (float)e[2]; o[3] = inten;
             }
         }
+        if (P.flip && P.flip[t]) e[1] = -e[1];                               // augment_single_box, after the query copy
         const int s = find_rank(sel_list(P, b, 0, ST_GRM_M), min(P.gtot[b], P.km), goff + r);
         if (s >= 0) {
             float* o = P.m_pts + ((size_t)b * P.km + s) * 11;
@@ -276,6 +313,7 @@ __global__ void k_rd_track(RdParams P) {
     const int nq = min(P.nq, L);
     int taken[8];
     for (int i = 0; i < nq; ++i) {
+        if (P.qsel) { taken[i] = P.qidx[b * P.nq + i] = P.qsel[b * P.nq + i]; continue; }
         int best = -1;
         for (int j = L - 1; j >= 0; --j) {
             bool used = false;
@@ -291,39 +329,19 @@ __global__ void k_rd_track(RdParams P) {
         for (int d = 0; d < 7; ++d)
             P.box_f[((size_t)b * P.qout + i) * 7 + d] =
                 (i < nq && d >= 3 && d < 6) ? (float)P.boxes[((size_t)b * P.L + taken[i]) * 7 + d] : 0.f;
+    if (P.gt_box_f)
+        for (int i = 0; i < P.qout; ++i)
+            for (int d = 0; d < 7; ++d)
+                P.gt_box_f[((size_t)b * P.qout + i) * 7 + d] =
+                    (i < nq && d >= 3 && d < 6) ? P.gt_traj[((size_t)b * P.L + taken[i]) * 7 + d] : 0.f;
 }
 
-// ---- select: one block per selection ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_rd_select(RdParams P) {
-    const int id = blockIdx.x;
-    int b, slot, stream, n, k;
-    int* out;
-    if (P.kind == RD_GRM) {
-        b = id / (P.nq + 1);
-        const int i = id % (P.nq + 1);
-        if (i < P.nq) {
-            if (i >= P.qnum[b]) return;
-            slot = P.qidx[b * P.nq + i]; stream = ST_GRM_Q; k = P.kq; n = P.n[(size_t)b * P.L + slot];
-            out = sel_list(P, b, i, ST_GRM_Q);
-        } else {
-            slot = 0; stream = ST_GRM_M; k = P.km; n = P.gtot[b];
-            out = sel_list(P, b, 0, ST_GRM_M);
-        }
-    } else {
-        const int per = P.kind == RD_PRM ? 2 : 1;
-        const int t = id / per;
-        b = t / P.L; slot = t % P.L;
-        if (slot >= track_len(P, b)) return;
-        stream = P.kind == RD_CRM ? ST_CRM : (id % per ? ST_PRM_M : ST_PRM_Q);
-        k = stream == ST_PRM_M ? P.km : P.kq;
-        n = P.n[t];
-        out = sel_list(P, b, slot, stream);
-    }
+// ---- select: the k ranks of 0..n-1 with the smallest keys mix64(base + r), sorted, into out; called by a whole 256-thread block ----
+__device__ void select_k(unsigned long long base, int n, int k, int* out) {
     if (n <= k) {
         for (int r = threadIdx.x; r < n; r += blockDim.x) out[r] = r;
         return;
     }
-    const unsigned long long base = key_base(P.seed, P.uid[b], slot, stream);
     __shared__ unsigned hist[256];
     __shared__ unsigned long long s_prefix, s_mask;
     __shared__ int s_need, s_done, s_warp[8];
@@ -365,6 +383,35 @@ __global__ void __launch_bounds__(256) k_rd_select(RdParams P) {
         run += total;
         __syncthreads();
     }
+}
+
+// ---- select: one block per selection ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_rd_select(RdParams P) {
+    const int id = blockIdx.x;
+    int b, slot, stream, n, k;
+    int* out;
+    if (P.kind == RD_GRM) {
+        b = id / (P.nq + 1);
+        const int i = id % (P.nq + 1);
+        if (i < P.nq) {
+            if (i >= P.qnum[b]) return;
+            slot = P.qidx[b * P.nq + i]; stream = ST_GRM_Q; k = P.kq; n = P.n[(size_t)b * P.L + slot];
+            out = sel_list(P, b, i, ST_GRM_Q);
+        } else {
+            slot = 0; stream = ST_GRM_M; k = P.km; n = P.gtot[b];
+            out = sel_list(P, b, 0, ST_GRM_M);
+        }
+    } else {
+        const int per = P.kind == RD_PRM ? 2 : 1;
+        const int t = id / per;
+        b = t / P.L; slot = t % P.L;
+        if (slot >= track_len(P, b)) return;
+        stream = P.kind == RD_CRM ? ST_CRM : (id % per ? ST_PRM_M : ST_PRM_Q);
+        k = stream == ST_PRM_M ? P.km : P.kq;
+        n = P.n[t];
+        out = sel_list(P, b, slot, stream);
+    }
+    select_k(key_base(P.seed, P.uid[b], slot, stream), n, k, out);
 }
 
 // ---- fill: every row no point lands in -----------------------------------------------------------------------------------------
@@ -411,6 +458,21 @@ static RdWs carve_rd(DzCarve& cv, int kind, int B, int L, int max_frame_points, 
     return w;
 }
 
+// the passes of one build: prep, count, scan, (GRM: per track), select, fill, write
+static void launch_rd(const RdParams& P, cudaStream_t st) {
+    const int T = P.B * P.L;
+    k_rd_prep<<<dz_cdiv(T, 128), 128, 0, st>>>(P);
+    dim3 grid(T, P.n_chunks);
+    k_rd_crop<0><<<grid, 256, 0, st>>>(P);
+    k_rd_scan<<<dz_cdiv(T, 128), 128, 0, st>>>(P);
+    if (P.kind == RD_GRM) k_rd_track<<<dz_cdiv(P.B, 64), 64, 0, st>>>(P);
+    const int n_sel = P.kind == RD_GRM ? P.B * (P.nq + 1) : T * (P.kind == RD_PRM ? 2 : 1);
+    k_rd_select<<<n_sel, 256, 0, st>>>(P);
+    const long long rows = P.kind == RD_GRM ? (long long)P.B * (P.qout * P.kq + P.km) : (long long)T * (P.kq + P.km);
+    k_rd_fill<<<(unsigned)((rows + 255) / 256), 256, 0, st>>>(P);
+    k_rd_crop<1><<<grid, 256, 0, st>>>(P);
+}
+
 extern "C" size_t dz_refine_inputs_ws_bytes(int kind, int B, int L, int max_frame_points, int kq, int km, int nq) {
     return dz_carve_bytes(carve_rd, kind, B, L, max_frame_points, kq, km, nq);
 }
@@ -430,8 +492,7 @@ extern "C" int dz_refine_inputs(int kind, const float* points, int pt_stride, co
     DZ_CHECK_ARG(kind != RD_GRM || (m_pts && traj && query_num && nq >= 1 && nq <= 8 && q_out >= 0 && q_out <= nq));
     if (B == 0) return DZ_OK;
     DZ_CHECK_WS(dz_refine_inputs_ws_bytes(kind, B, L, max_frame_points, kq, km, nq));
-    const int T = B * L;
-    RdParams P;
+    RdParams P = {};
     P.pts = points; P.pstride = pt_stride; P.foff = frame_offsets; P.F = n_frames;
     P.poses = poses; P.boxes = boxes; P.fob = frame_of_box; P.scores = scores; P.box_num = box_num; P.cls = cls;
     P.uid = (const long long*)track_uid;
@@ -443,17 +504,189 @@ extern "C" int dz_refine_inputs(int kind, const float* points, int pt_stride, co
     P.n_chunks = w.n_chunks; P.bx = w.bx; P.cc = w.cc; P.n = counts ? counts : w.n; P.goff = w.goff;
     P.gtot = w.gtot; P.qnum = w.qnum; P.qidx = w.qidx; P.sel = sel ? sel : w.sel;
     P.q_pts = q_pts; P.m_pts = m_pts; P.traj = traj; P.box_f = box_f; P.track_f = track_f; P.query_num = query_num;
+    launch_rd(P, (cudaStream_t)stream);
+    DZ_LAUNCH_CHECK();
+    return DZ_OK;
+}
+
+// ---- training samples ------------------------------------------------------------------------------------------------------------
+// the draw of one track: one block of 256 threads
+struct RdDraw {
+    const int* box_num; const unsigned char* matched; const long long* uid;
+    int B, L, kind, nq; unsigned long long seed;
+    int* elig; int* kept; int* n_kept; int* qsel; int* init; unsigned char* flip;
+};
+
+__global__ void __launch_bounds__(256) k_rd_draw(RdDraw D) {
+    const int b = blockIdx.x;
+    const int L = min(max(D.box_num[b], 0), D.L);
+    const long long uid = D.uid[b];
+    int* elig = D.elig + (size_t)b * D.L;
+    int* kept = D.kept + (size_t)b * D.L;
+    __shared__ int s_m, s_n;
+    if (threadIdx.x == 0) {                                                  // eligible slots, ascending
+        int m = 0;
+        for (int j = 0; j < L; ++j)
+            if (!D.matched || D.matched[(size_t)b * D.L + j]) elig[m++] = j;
+        const int lo = min(5, m);
+        const int n = m ? lo + (int)(mix64(key_base(D.seed, uid, 0, ST_TR_COUNT)) % (unsigned long long)(m - lo + 1)) : 0;
+        s_m = m; s_n = n;
+        D.n_kept[b] = n;
+        if (D.init) D.init[b] = n ? (int)(mix64(key_base(D.seed, uid, 0, ST_TR_INIT)) % (unsigned long long)n) : 0;
+    }
+    __syncthreads();
+    const int m = s_m, n = s_n;
+    select_k(key_base(D.seed, uid, 0, ST_TR_KEEP), m, n, kept);              // ranks among the eligible slots
+    __syncthreads();
+    for (int i = threadIdx.x; i < D.L; i += blockDim.x) kept[i] = i < n ? elig[kept[i]] : -1;
+    if (D.qsel) {
+        int* q = D.qsel + (size_t)b * D.nq;
+        const int nq = min(D.nq, n);
+        select_k(key_base(D.seed, uid, 0, ST_TR_QUERY), n, nq, q);
+        __syncthreads();
+        for (int i = nq + threadIdx.x; i < D.nq; i += blockDim.x) q[i] = -1;
+    }
+    if (D.flip) {
+        const unsigned long long base = key_base(D.seed, uid, 0, ST_TR_FLIP);
+        for (int i = threadIdx.x; i < D.L; i += blockDim.x)
+            D.flip[(size_t)b * D.L + i] = i < n ? (unsigned char)(mix64(base + (unsigned long long)i) >> 63) : 0;
+    }
+}
+
+static int* carve_draw(DzCarve& cv, int B, int L) { return cv.take<int>((size_t)B * L); }
+
+extern "C" size_t dz_refine_train_draw_ws_bytes(int B, int L) { return dz_carve_bytes(carve_draw, B, L); }
+
+extern "C" int dz_refine_train_draw(int kind, const int32_t* box_num, const uint8_t* matched, const int64_t* track_uid, int B, int L,
+                                    int nq, unsigned long long seed, long long epoch, int32_t* kept, int32_t* n_kept,
+                                    int32_t* query_slots, int32_t* init_slot, uint8_t* flip, void* ws, size_t ws_bytes,
+                                    dz_stream_t stream) {
+    DZ_CHECK_ARG((kind == RD_CRM || kind == RD_GRM) && box_num && track_uid && B >= 0 && L >= 1 && kept && n_kept);
+    DZ_CHECK_ARG(kind != RD_GRM || (matched && query_slots && flip && nq >= 1 && nq <= 8));
+    DZ_CHECK_ARG(kind != RD_CRM || init_slot);
+    if (B == 0) return DZ_OK;
+    DZ_CHECK_WS(dz_refine_train_draw_ws_bytes(B, L));
+    DzCarve cv((char*)ws);
+    RdDraw D;
+    D.box_num = box_num; D.matched = kind == RD_GRM ? matched : nullptr; D.uid = (const long long*)track_uid;
+    D.B = B; D.L = L; D.kind = kind; D.nq = nq; D.seed = epoch_seed(seed, epoch);
+    D.elig = carve_draw(cv, B, L); D.kept = kept; D.n_kept = n_kept;
+    D.qsel = kind == RD_GRM ? query_slots : nullptr; D.init = kind == RD_CRM ? init_slot : nullptr;
+    D.flip = kind == RD_GRM ? flip : nullptr;
+    k_rd_draw<<<B, 256, 0, (cudaStream_t)stream>>>(D);
+    DZ_LAUNCH_CHECK();
+    return DZ_OK;
+}
+
+// the kept slots of each track -> the derived track table (boxes, frame_of_box, scores) and the kept targets: gt_geo_trajectory
+// (GRM, f32 world, zero padded) and iou (CRM, -1 padded).  One thread per derived slot.
+__global__ void k_rd_gather(const double* __restrict__ boxes, const int* __restrict__ fob, const float* __restrict__ scores,
+                            const int* __restrict__ kept, const int* __restrict__ n_kept, const double* __restrict__ gt_boxes,
+                            const float* __restrict__ iou, int B, int L, double* __restrict__ dboxes, int* __restrict__ dfob,
+                            float* __restrict__ dscores, float* __restrict__ gt_traj, float* __restrict__ iou_out) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= B * L) return;
+    const int b = t / L, i = t % L;
+    const bool live = i < min(max(n_kept[b], 0), L);
+    const size_t s = live ? (size_t)b * L + kept[t] : 0;
+    for (int d = 0; d < 7; ++d) dboxes[(size_t)t * 7 + d] = live ? boxes[s * 7 + d] : 0.0;
+    dfob[t] = live ? fob[s] : 0;
+    dscores[t] = live ? scores[s] : 0.f;
+    if (gt_traj) for (int d = 0; d < 7; ++d) gt_traj[(size_t)t * 7 + d] = live ? (float)gt_boxes[s * 7 + d] : 0.f;
+    if (iou_out) iou_out[t] = live ? iou[s] : -1.f;
+}
+
+struct RdTrainWs { double* boxes; int* fob; float* scores; RdWs rd; };
+
+static RdTrainWs carve_rd_train(DzCarve& cv, int kind, int B, int L, int max_frame_points, int kq, int km, int nq) {
+    RdTrainWs w;
+    w.boxes = cv.take<double>((size_t)B * L * 7);
+    w.fob = cv.take<int>((size_t)B * L);
+    w.scores = cv.take<float>((size_t)B * L);
+    w.rd = carve_rd(cv, kind, B, L, max_frame_points, kq, km, nq);
+    return w;
+}
+
+extern "C" size_t dz_refine_train_inputs_ws_bytes(int kind, int B, int L, int max_frame_points, int kq, int km, int nq) {
+    return dz_carve_bytes(carve_rd_train, kind, B, L, max_frame_points, kq, km, nq);
+}
+
+extern "C" int dz_refine_train_inputs(int kind, const float* points, int pt_stride, const int32_t* frame_offsets, int n_frames,
+                                      int max_frame_points, const double* poses, const double* boxes, const int32_t* frame_of_box,
+                                      const float* scores, const int32_t* cls, const int64_t* track_uid, const double* gt_boxes,
+                                      const float* iou, int B, int L, int kq, int km, int nq, int q_out, double enlarge_scale,
+                                      int crop_on_bev, int crop, unsigned long long seed, long long epoch, const int32_t* kept,
+                                      const int32_t* n_kept, const int32_t* query_slots, const int32_t* init_slot,
+                                      const uint8_t* flip, float* q_pts, float* m_pts, float* traj, float* box_f, float* gt_box_f,
+                                      float* gt_traj, float* iou_out, int32_t* query_num, int32_t* counts, int32_t* sel, void* ws,
+                                      size_t ws_bytes, dz_stream_t stream) {
+    DZ_CHECK_ARG((kind == RD_CRM || kind == RD_GRM) && pt_stride >= 5 && frame_offsets && n_frames >= 1 && max_frame_points >= 0 &&
+                 poses && boxes && frame_of_box && scores && cls && track_uid && B >= 0 && L >= 1 && kq >= 1 && kept && n_kept &&
+                 q_pts && box_f && (points || max_frame_points == 0));
+    DZ_CHECK_ARG(kind != RD_GRM || (gt_boxes && query_slots && m_pts && traj && gt_box_f && gt_traj && query_num && km >= 1 &&
+                                    nq >= 1 && nq <= 8 && q_out >= 0 && q_out <= nq));
+    DZ_CHECK_ARG(kind != RD_CRM || (iou && init_slot && iou_out));
+    if (B == 0) return DZ_OK;
+    DZ_CHECK_WS(dz_refine_train_inputs_ws_bytes(kind, B, L, max_frame_points, kq, km, nq));
+    DzCarve cv((char*)ws);
+    const RdTrainWs w = carve_rd_train(cv, kind, B, L, max_frame_points, kq, km, nq);
     cudaStream_t st = (cudaStream_t)stream;
-    k_rd_prep<<<dz_cdiv(T, 128), 128, 0, st>>>(P);
+    k_rd_gather<<<dz_cdiv(B * L, 128), 128, 0, st>>>(boxes, frame_of_box, scores, kept, n_kept, gt_boxes, iou, B, L, w.boxes, w.fob,
+                                                     w.scores, kind == RD_GRM ? gt_traj : nullptr, kind == RD_CRM ? iou_out : nullptr);
+    RdParams P = {};
+    P.pts = points; P.pstride = pt_stride; P.foff = frame_offsets; P.F = n_frames;
+    P.poses = poses; P.boxes = w.boxes; P.fob = w.fob; P.scores = w.scores; P.box_num = n_kept; P.cls = cls;
+    P.uid = (const long long*)track_uid;
+    P.B = B; P.L = L; P.kind = kind; P.with_class = 0; P.C = kind == RD_GRM ? 4 : 32;
+    P.kq = kq; P.km = kind == RD_CRM ? 0 : km; P.nq = nq; P.qout = q_out; P.crop = crop ? 1 : 0; P.bev = crop_on_bev ? 1 : 0;
+    P.enlarge = enlarge_scale; P.seed = epoch_seed(seed, epoch);
+    P.n_chunks = w.rd.n_chunks; P.bx = w.rd.bx; P.cc = w.rd.cc; P.n = counts ? counts : w.rd.n; P.goff = w.rd.goff;
+    P.gtot = w.rd.gtot; P.qnum = w.rd.qnum; P.qidx = w.rd.qidx; P.sel = sel ? sel : w.rd.sel;
+    P.q_pts = q_pts; P.m_pts = m_pts; P.traj = kind == RD_GRM ? traj : nullptr; P.box_f = box_f; P.query_num = query_num;
+    if (kind == RD_GRM) { P.qsel = query_slots; P.flip = flip; P.gt_traj = gt_traj; P.gt_box_f = gt_box_f; }
+    else P.init = init_slot;
+    launch_rd(P, st);
+    DZ_LAUNCH_CHECK();
+    return DZ_OK;
+}
+
+// ---- crop once: every in-box point row of every box slot, copied to rows[rbase[t] + rank] --------------------------------------
+static RdWs carve_crop(DzCarve& cv, int B, int L, int max_frame_points) {
+    const size_t T = (size_t)B * L;
+    RdWs w = {};
+    w.n_chunks = dz_cdiv(max(max_frame_points, 1), RD_CHUNK);
+    w.bx = cv.take<RdBox>(T);
+    w.cc = cv.take<int>(T * w.n_chunks);
+    return w;
+}
+
+extern "C" size_t dz_crop_tracks_ws_bytes(int B, int L, int max_frame_points) {
+    return dz_carve_bytes(carve_crop, B, L, max_frame_points);
+}
+
+extern "C" int dz_crop_tracks(const float* points, int pt_stride, int width, const int32_t* frame_offsets, int n_frames,
+                              int max_frame_points, const double* poses, const double* boxes, const int32_t* frame_of_box,
+                              const int32_t* box_num, int B, int L, double enlarge_scale, int crop_on_bev, int32_t* counts,
+                              const int32_t* row_base, float* rows, void* ws, size_t ws_bytes, dz_stream_t stream) {
+    DZ_CHECK_ARG(pt_stride >= 5 && width >= 5 && width <= pt_stride && frame_offsets && n_frames >= 1 && max_frame_points >= 0 &&
+                 poses && boxes && frame_of_box && box_num && B >= 0 && L >= 1 && counts && (points || max_frame_points == 0) &&
+                 (!rows == !row_base));
+    if (B == 0) return DZ_OK;
+    DZ_CHECK_WS(dz_crop_tracks_ws_bytes(B, L, max_frame_points));
+    DzCarve cv((char*)ws);
+    const RdWs w = carve_crop(cv, B, L, max_frame_points);
+    RdParams P = {};
+    P.pts = points; P.pstride = pt_stride; P.foff = frame_offsets; P.F = n_frames;
+    P.poses = poses; P.boxes = boxes; P.fob = frame_of_box; P.box_num = box_num;
+    P.B = B; P.L = L; P.kind = RD_CROP; P.C = width; P.crop = 1; P.bev = crop_on_bev ? 1 : 0; P.enlarge = enlarge_scale;
+    P.n_chunks = w.n_chunks; P.bx = w.bx; P.cc = w.cc; P.n = counts; P.rbase = row_base; P.rows = rows;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int T = B * L;
     dim3 grid(T, P.n_chunks);
+    k_rd_prep<<<dz_cdiv(T, 128), 128, 0, st>>>(P);
     k_rd_crop<0><<<grid, 256, 0, st>>>(P);
     k_rd_scan<<<dz_cdiv(T, 128), 128, 0, st>>>(P);
-    if (kind == RD_GRM) k_rd_track<<<dz_cdiv(B, 64), 64, 0, st>>>(P);
-    const int n_sel = kind == RD_GRM ? B * (nq + 1) : T * (kind == RD_PRM ? 2 : 1);
-    k_rd_select<<<n_sel, 256, 0, st>>>(P);
-    const long long rows = kind == RD_GRM ? (long long)B * (q_out * kq + km) : (long long)T * (kq + P.km);
-    k_rd_fill<<<(unsigned)((rows + 255) / 256), 256, 0, st>>>(P);
-    k_rd_crop<1><<<grid, 256, 0, st>>>(P);
+    if (rows) k_rd_crop<1><<<grid, 256, 0, st>>>(P);
     DZ_LAUNCH_CHECK();
     return DZ_OK;
 }

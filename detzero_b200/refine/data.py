@@ -9,6 +9,10 @@ that function and the other deliberate deviations (float64 geometry, per-track G
 ``combine_frames`` puts the refined tracks of a sequence together into per-frame result rows (csrc/combine.cu), replacing
 daemon/combine_output.py's convert_frame_format and combine_det.  ``track_targets`` attaches the ground truth of an assignment
 (track.assign_track_target) to a TrackBatch (csrc/refine_gt.cu); refine.score turns it into the recall records and IoU labels.
+Training samples: ``crop_tracks`` crops every box once into per-box frames; ``geometry_training_inputs`` /
+``confidence_training_inputs`` build the training branch of the GRM / CRM datasets from them each epoch, with every random draw keyed
+on (seed, epoch, track_uid) (csrc/refine_data.cu); ``training_order`` is the epoch's shuffled track list (streams 10 and 11 of the
+same key function, on the host).
 """
 import zlib
 
@@ -241,6 +245,232 @@ def geometry_inputs(frames, frame_offsets, poses, tracks, cfg=None, seed=0, crop
     geo_query_num (dataset.py:239-256); 'geo_trajectory' is the world trajectory.  'selection' (B, nq * kq + km): the kept ranks of
     each query box, then of the memory sample over the concatenation of every box's points."""
     return _build(GRM, frames, frame_offsets, poses, tracks, _cfg(cfg, grm_data_cfg()), seed, crop, return_selection)
+
+
+def crop_tracks(frames, frame_offsets, poses, tracks, cfg=None):
+    """Crop every box of ``tracks`` from its frame once (the crop of the builders: ENLARGE_SCALE, CROP_ON_BEV) and return the points
+    as one frame per box, the layout tracks_from_object_infos packs: (box_frames (N, C) f32, the in-box rows of ``frames`` copied in
+    frame order, box_offsets (n_boxes + 1) int64 (device), box_poses (n_boxes, 4, 4) f64, TrackBatch with frame_of_box re-pointed
+    at the box frames, track by track, 0 past box_num).  The builders run on the result with crop=False and give, bit for bit, what
+    they give with crop=True on the original frames.  One device-to-host read sizes the output."""
+    cfg = _cfg(cfg, {'ENLARGE_SCALE': 1.1, 'CROP_ON_BEV': False})
+    off, F, max_pts, poses = _frames_args(frames, frame_offsets, poses)
+    dev = frames.device
+    B, L = len(tracks), tracks.L
+    if B == 0:
+        raise ValueError('crop_tracks needs at least one track')
+    W = int(frames.shape[1])
+    counts = torch.empty((B, L), dtype=torch.int32, device=dev)
+    ws = ops.workspace(lib().dz_crop_tracks_ws_bytes(B, L, max_pts), dev, 'refine_data')
+    enlarge, bev = float(cfg['ENLARGE_SCALE']), int(bool(cfg['CROP_ON_BEV']))
+
+    def run(row_base, rows):
+        check(lib().dz_crop_tracks(ops._p(frames), frames.stride(0), W, ops._p(off), F, max_pts, ops._p(poses), ops._p(tracks.boxes),
+                                   ops._p(tracks.frame_of_box), ops._p(tracks.box_num), B, L, enlarge, bev, ops._p(counts),
+                                   ops._p(row_base), ops._p(rows), ops._p(ws), ws.numel(), ops._stream()), 'crop_tracks')
+        ops._count(4 if rows is not None else 3)
+    run(None, None)
+    valid = torch.arange(L, device=dev)[None, :] < tracks.box_num[:, None]
+    box_offsets = torch.zeros(int(valid.sum()) + 1, dtype=torch.int64, device=dev)
+    torch.cumsum(counts[valid].long(), 0, out=box_offsets[1:])
+    total = int(box_offsets[-1])
+    if total >= 1 << 31:
+        raise ValueError('crop_tracks: %d cropped rows do not fit int32 row offsets' % total)
+    row_base = torch.zeros((B, L), dtype=torch.int32, device=dev)
+    row_base[valid] = box_offsets[:-1].to(torch.int32)
+    rows = torch.empty((total, W), dtype=torch.float32, device=dev)
+    run(row_base, rows)
+    fob = torch.zeros((B, L), dtype=torch.int32, device=dev)
+    fob[valid] = torch.arange(box_offsets.numel() - 1, dtype=torch.int32, device=dev)
+    box_poses = poses[tracks.frame_of_box[valid].long()].contiguous()
+    return rows, box_offsets, box_poses, TrackBatch(tracks.boxes, fob, tracks.scores, tracks.box_num, tracks.cls, tracks.track_uid, dev)
+
+
+def grm_train_cfg():
+    """waymo_grm_dataset.yaml in training: AUGMENT_SINGLE on (its AUGMENT_ALL is a key the dataset never reads)"""
+    return dict(grm_data_cfg(), AUGMENTOR={'AUGMENT_SINGLE': True, 'AUGMENT_FULL': False})
+
+
+def crm_train_cfg():
+    """waymo_crm_dataset.yaml in training (the CRM dataset applies no augmentation)"""
+    return dict(crm_data_cfg(), AUGMENTOR={'AUGMENT_SINGLE': True, 'AUGMENT_FULL': False})
+
+
+def _check_train_cfg(kind, cfg):
+    enc = list(cfg['ENCODING'])
+    if enc != (P2S if kind == GRM else P2CO):
+        raise ValueError('unsupported ENCODING %r (the shipped lists only)' % (enc,))
+    aug = cfg.get('AUGMENTOR') or {}
+    if aug.get('AUGMENT_FULL', False):
+        raise ValueError('AUGMENT_FULL (augment_full_track) is not supported; the shipped configs never enable it')
+    return bool(aug.get('AUGMENT_SINGLE', False))
+
+
+def _train_build(kind, frames, frame_offsets, poses, tracks, cfg, seed, epoch, crop, return_selection, gt_boxes=None, iou=None,
+                 matched=None):
+    augment_single = _check_train_cfg(kind, cfg)
+    off, F, max_pts, poses = _frames_args(frames, frame_offsets, poses)
+    dev = frames.device
+    B, L = len(tracks), tracks.L
+    if kind == CRM and int(cfg['QUERY_NUM']) != L:
+        raise ValueError('QUERY_NUM %d != the track tables\' %d box slots' % (cfg['QUERY_NUM'], L))
+    kq = int(cfg['QUERY_POINTS_NUM'])
+    km = int(cfg['MEMORY_POINTS_NUM']) if kind == GRM else 0
+    nq = int(cfg['QUERY_NUM']) if kind == GRM else 1
+    seed, epoch = int(seed) & ((1 << 64) - 1), int(epoch)
+    i32 = dict(dtype=torch.int32, device=dev)
+    f32 = dict(dtype=torch.float32, device=dev)
+    kept = torch.empty((B, L), **i32)
+    n_kept = torch.empty((B,), **i32)
+    qsel = torch.empty((B, nq), **i32) if kind == GRM else None
+    init = torch.empty((B,), **i32) if kind == CRM else None
+    flip = torch.empty((B, L), dtype=torch.uint8, device=dev) if kind == GRM else None
+    if B:
+        ws = ops.workspace(lib().dz_refine_train_draw_ws_bytes(B, L), dev, 'refine_data')
+        check(lib().dz_refine_train_draw(kind, ops._p(tracks.box_num), ops._p(matched), ops._p(tracks.track_uid), B, L, nq, seed, epoch,
+                                         ops._p(kept), ops._p(n_kept), ops._p(qsel), ops._p(init), ops._p(flip), ops._p(ws),
+                                         ws.numel(), ops._stream()), 'refine_train_draw')
+        ops._count(1)
+        if kind == GRM and not augment_single:
+            flip.zero_()
+    q_out = min(nq, int(n_kept.max())) if kind == GRM and B else 0
+    gt_traj = gt_box_f = iou_out = qn = m = traj = None
+    if kind == GRM:
+        q = torch.empty((B, q_out, kq, 4), **f32)
+        m = torch.empty((B, km, 11), **f32)
+        traj = torch.empty((B, L, 7), **f32)
+        box_f = torch.empty((B, q_out, 7), **f32)
+        gt_box_f = torch.empty((B, q_out, 7), **f32)
+        gt_traj = torch.empty((B, L, 7), **f32)
+        qn = torch.empty((B,), **i32)
+        nsel = nq * kq + km
+    else:
+        q = torch.empty((B, L, kq, 32), **f32)
+        box_f = torch.empty((B, L), **f32)
+        iou_out = torch.empty((B, L), **f32)
+        nsel = L * kq
+    counts = torch.empty((B, L), **i32) if return_selection else None
+    sel = torch.full((B, nsel), -1, **i32) if return_selection else None
+    if B:
+        ws = ops.workspace(lib().dz_refine_train_inputs_ws_bytes(kind, B, L, max_pts, kq, km, nq), dev, 'refine_data')
+        check(lib().dz_refine_train_inputs(kind, ops._p(frames), frames.stride(0), ops._p(off), F, max_pts, ops._p(poses),
+                                           ops._p(tracks.boxes), ops._p(tracks.frame_of_box), ops._p(tracks.scores), ops._p(tracks.cls),
+                                           ops._p(tracks.track_uid), ops._p(gt_boxes), ops._p(iou), B, L, kq, km, nq, q_out,
+                                           float(cfg.get('ENLARGE_SCALE', 1.1)), int(bool(cfg.get('CROP_ON_BEV', False))),
+                                           int(bool(crop)), seed, epoch, ops._p(kept), ops._p(n_kept), ops._p(qsel), ops._p(init),
+                                           ops._p(flip), ops._p(q), ops._p(m), ops._p(traj), ops._p(box_f), ops._p(gt_box_f),
+                                           ops._p(gt_traj), ops._p(iou_out), ops._p(qn), ops._p(counts), ops._p(sel), ops._p(ws),
+                                           ws.numel(), ops._stream()), 'refine_train_inputs')
+        ops._count(8)
+    if kind == GRM:
+        out = {'geo_query_points': q, 'geo_query_boxes': box_f, 'gt_geo_query_boxes': gt_box_f, 'geo_memory_points': m,
+               'geo_query_num': qn, 'geo_trajectory': traj, 'gt_geo_trajectory': gt_traj}
+    else:
+        out = {'conf_points': q, 'conf_score': box_f, 'iou': iou_out, 'box_num': n_kept}
+    if return_selection:
+        out.update({'kept': kept, 'crop_counts': counts, 'selection': sel})
+        if kind == GRM:
+            out.update({'kept_num': n_kept, 'query_slots': qsel, 'flip': flip})
+        else:
+            out['init_slot'] = init
+    return out
+
+
+def _grm_trainable(targets, box_num):
+    """per track: matched, with at least one matched box among its valid slots"""
+    L = targets.matched.shape[1]
+    valid = torch.arange(L, device=targets.matched.device)[None, :] < box_num.to(targets.matched.device)[:, None]
+    return (targets.matched_tracklet != 0) & ((targets.matched != 0) & valid).any(1)
+
+
+def geometry_training_inputs(frames, frame_offsets, poses, tracks, targets, cfg=None, seed=0, epoch=0, crop=True,
+                             return_selection=False):
+    """GRM training samples (WaymoGeometryDataset.extract_track_feature, training, with augment_single_box) of every track:
+    per track a random subset of its matched boxes (n uniform on min(5, m) .. m of m), min(QUERY_NUM, n) random query boxes and
+    one random y flip per kept box's memory points, all keyed on (seed, epoch, track_uid) (csrc/refine_data.cu).  targets: the
+    TrackTargets of ``tracks`` (track_targets); every track must be a matched tracklet with a matched box.  Returns the dict
+    GeometryTransformer.forward_train reads: geo_query_points, geo_query_boxes, gt_geo_query_boxes (sizes only, padded to the
+    batch's largest geo_query_num), geo_memory_points, geo_query_num, and geo_trajectory / gt_geo_trajectory (B, L, 7) the kept world
+    boxes and their ground truth, zero padded.  Kept boxes are in ascending slot order.  return_selection adds kept (B, L) source
+    slots (-1 padding), kept_num (B), query_slots (B, QUERY_NUM) kept positions (-1 padding), flip (B, L) per kept position,
+    crop_counts and selection (geometry_inputs' layout, on the kept positions).  crop=False: frames are per-box (crop_tracks)."""
+    cfg = _cfg(cfg, grm_train_cfg())
+    if len(tracks) and not bool(_grm_trainable(targets, tracks.box_num).all()):
+        raise ValueError('geometry_training_inputs: every track must be a matched tracklet with at least one matched box '
+                         '(training_order excludes the others)')
+    return _train_build(GRM, frames, frame_offsets, poses, tracks, cfg, seed, epoch, crop, return_selection,
+                        gt_boxes=targets.gt_boxes.to(torch.float64).contiguous(), matched=targets.matched.to(torch.uint8).contiguous())
+
+
+def confidence_training_inputs(frames, frame_offsets, poses, tracks, iou, cfg=None, seed=0, epoch=0, crop=True,
+                               return_selection=False):
+    """CRM training samples (WaymoConfidenceDataset.extract_track_feature, training) of every track: a random subset of its boxes
+    (n uniform on min(5, L) .. L) and a random init box among them in place of L // 2, keyed on (seed, epoch, track_uid).
+    iou: (B, L) refine_iou_labels.  Returns conf_points, conf_score (-1 padding), iou (the kept labels, -1 padding) and box_num (the
+    kept count).  return_selection adds kept, init_slot (B) (a kept position), crop_counts and selection (on the kept positions)."""
+    cfg = _cfg(cfg, crm_train_cfg())
+    dev = tracks.boxes.device
+    iou = torch.as_tensor(iou).to(device=dev, dtype=torch.float32).contiguous()
+    if iou.shape != (len(tracks), tracks.L):
+        raise ValueError('iou must be (B, L) = %r, got %r' % ((len(tracks), tracks.L), tuple(iou.shape)))
+    return _train_build(CRM, frames, frame_offsets, poses, tracks, cfg, seed, epoch, crop, return_selection, iou=iou)
+
+
+ST_ORDER, ST_NEG = 10, 11
+
+
+def training_order(targets, kind, seed=0, epoch=0):
+    """The track indices of one training epoch (host int64), keyed on (seed, epoch) as the samples are: the dataset's list shuffled
+    as the DataLoader does.  'grm': every matched tracklet with at least one matched box (load_infos_worker drops unmatched tracks
+    without IOU_NAME), once.  'crm': every positive (matched) track once, each paired with a negative drawn uniformly with
+    replacement (WaymoConfidenceDataset.__getitem__), 2 x positives in all.  Raises when the CRM has no negative track."""
+    es = epoch_seed(seed, epoch)
+    mt = targets.matched_tracklet.cpu().numpy() != 0
+    if kind == 'grm':
+        ok = mt & (targets.matched.cpu().numpy() != 0).any(1)
+        items = np.nonzero(ok)[0]
+    elif kind == 'crm':
+        pos, neg = np.nonzero(mt)[0], np.nonzero(~mt)[0]
+        if len(pos) and not len(neg):
+            raise ValueError('training_order: CRM training pairs every positive track with a negative one, and there is none')
+        with np.errstate(over='ignore'):
+            pick = _mix64(np.uint64(_key_base(es, 0, 0, ST_NEG)) + np.arange(len(pos), dtype=np.uint64)) % np.uint64(max(len(neg), 1))
+        items = np.stack([pos, neg[pick.astype(np.int64)] if len(pos) else pos], 1).reshape(-1)
+    else:
+        raise ValueError("kind must be 'grm' or 'crm'")
+    with np.errstate(over='ignore'):
+        keys = _mix64(np.uint64(_key_base(es, 0, 0, ST_ORDER)) + np.arange(len(items), dtype=np.uint64))
+    return items[np.argsort(keys, kind='stable')].astype(np.int64)
+
+
+_M64 = (1 << 64) - 1
+
+
+def _mix64_int(z):
+    """splitmix64's output step (csrc/refine_data.cu mix64) on a Python int"""
+    z = (int(z) + 0x9E3779B97F4A7C15) & _M64
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & _M64
+    return z ^ (z >> 31)
+
+
+def _mix64(z):
+    """the same on uint64 arrays"""
+    z = np.asarray(z, np.uint64)
+    with np.errstate(over='ignore'):
+        z = z + np.uint64(0x9E3779B97F4A7C15)
+        z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+        z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+        return z ^ (z >> np.uint64(31))
+
+
+def _key_base(seed, uid, slot, stream):
+    return _mix64_int(_mix64_int(_mix64_int(seed) ^ (int(uid) & _M64)) ^ ((int(slot) << 8) | int(stream)))
+
+
+def epoch_seed(seed, epoch):
+    """the seed a training epoch keys its draws on: mix64(mix64(seed) + epoch) mod 2^64 (csrc/refine_data.cu epoch_seed)"""
+    return _mix64_int((_mix64_int(int(seed) & _M64) + int(epoch)) & _M64)
 
 
 def _revert(kind, pred, poses, tracks):

@@ -312,6 +312,36 @@ int dz_refine_inputs(int kind, const float* points, int pt_stride, const int32_t
  * (waymo_geometry_dataset.py:160-186).  lidar, world (B, L, 7) f64, rows past box_num zero. */
 int dz_refine_revert(int kind, const float* pred, const double* poses, int n_frames, const double* boxes, const int32_t* frame_of_box,
                      const int32_t* box_num, int B, int L, double* lidar, double* world, dz_stream_t stream);
+/* Training samples (the training branch of WaymoGeometryDataset / WaymoConfidenceDataset.extract_track_feature), csrc/refine_data.cu.
+ * dz_crop_tracks: the crop of dz_refine_inputs once, copying the first `width` floats of every in-box point row; box slot t's points go
+ *   to rows[row_base[t] ..] in frame order.  Called with rows = row_base = NULL it writes only counts (B, L), the in-box point count
+ *   of every slot (0 past box_num); the caller sizes rows from them and calls again.
+ * dz_refine_train_draw: per track, keyed on (seed, epoch, track_uid) only.  kind 2 (GRM): eligible slots are the matched ones
+ *   (matched (B, L) u8); kind 1 (CRM): every valid slot.  kept (B, L) source slots in ascending order, -1 padded; n_kept (B) uniform on
+ *   min(5, m) .. m of m eligible; GRM: query_slots (B, nq) min(nq, n_kept) distinct kept positions ascending, -1 padded, and flip
+ *   (B, L) u8 bits per kept position; CRM: init_slot (B), a kept position.
+ * dz_refine_train_inputs: dz_refine_inputs on the kept slots of each track (a derived table of n_kept boxes) with the drawn query
+ *   positions (GRM), init box (CRM) and flips (GRM, memory rows only), point samples keyed on the epoch's seed.  Outputs as
+ *   dz_refine_inputs kinds 1 / 2, plus GRM: gt_box_f (B, q_out, 7) gt_geo_query_boxes (sizes of gt_boxes), gt_traj (B, L, 7) f32 kept
+ *   gt_boxes; CRM: iou_out (B, L) the kept iou, -1 padded.  counts / sel as dz_refine_inputs, on the derived slots. */
+size_t dz_crop_tracks_ws_bytes(int B, int L, int max_frame_points);
+int dz_crop_tracks(const float* points, int pt_stride, int width, const int32_t* frame_offsets, int n_frames, int max_frame_points,
+                   const double* poses, const double* boxes, const int32_t* frame_of_box, const int32_t* box_num, int B, int L,
+                   double enlarge_scale, int crop_on_bev, int32_t* counts, const int32_t* row_base, float* rows, void* ws,
+                   size_t ws_bytes, dz_stream_t stream);
+size_t dz_refine_train_draw_ws_bytes(int B, int L);
+int dz_refine_train_draw(int kind, const int32_t* box_num, const uint8_t* matched, const int64_t* track_uid, int B, int L, int nq,
+                         unsigned long long seed, long long epoch, int32_t* kept, int32_t* n_kept, int32_t* query_slots,
+                         int32_t* init_slot, uint8_t* flip, void* ws, size_t ws_bytes, dz_stream_t stream);
+size_t dz_refine_train_inputs_ws_bytes(int kind, int B, int L, int max_frame_points, int kq, int km, int nq);
+int dz_refine_train_inputs(int kind, const float* points, int pt_stride, const int32_t* frame_offsets, int n_frames,
+                           int max_frame_points, const double* poses, const double* boxes, const int32_t* frame_of_box,
+                           const float* scores, const int32_t* cls, const int64_t* track_uid, const double* gt_boxes, const float* iou,
+                           int B, int L, int kq, int km, int nq, int q_out, double enlarge_scale, int crop_on_bev, int crop,
+                           unsigned long long seed, long long epoch, const int32_t* kept, const int32_t* n_kept,
+                           const int32_t* query_slots, const int32_t* init_slot, const uint8_t* flip, float* q_pts, float* m_pts,
+                           float* traj, float* box_f, float* gt_box_f, float* gt_traj, float* iou_out, int32_t* query_num,
+                           int32_t* counts, int32_t* sel, void* ws, size_t ws_bytes, dz_stream_t stream);
 
 /* ---- combine: refined tracks -> per-frame result rows (csrc/combine.cu) ------------------------------------------------------- */
 /* convert_frame_format + combine_det as combine_final drives them (daemon/combine_output.py:27-41,44-99,102-167), for the B tracks
