@@ -526,7 +526,8 @@ class GeometryTransformer(nn.Module):
         self.preds_dict = {}
         self.targets_dict = {}
         self.loss_weight = [0.1, 2]
-        self.pooled_rows = {}           # the rows the last training step's max-pools picked: 'memory' (B, 512), 'query' (B*Q, 256)
+        self.pooled_rows = {}           # the rows the last training step's max-pools picked: 'memory' (B, 512), 'query' (B*Q, 256);
+        #                                 'memory_pool' (B, 512) the pooled memory_encoder output
 
     def forward(self, data_dict):
         if self.training:

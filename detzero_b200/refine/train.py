@@ -180,7 +180,8 @@ def _w(w):
 
 class GrmMemoryPath(torch.autograd.Function):
     """memory_encoder (11 -> 128 -> 128 -> 512, max over the track's N points: g) -> memory_mlp on cat([y2, g]) (640 -> 512 -> 256):
-    x (B*N, c0) -> y5 (B*N, 256).  ``rows`` (a dict) receives the pooled row of each (track, channel) under 'memory'.  Arguments
+    x (B*N, c0) -> y5 (B*N, 256).  ``rows`` (a dict) receives the pooled row of each (track, channel) under 'memory' and the pooled
+    output g under 'memory_pool'.  Arguments
     after ``bns`` (the five BatchNorm1d modules): per layer conv weight, BN weight, BN bias."""
 
     @staticmethod
@@ -197,7 +198,7 @@ class GrmMemoryPath(torch.autograd.Function):
         z3, ps, ev, ei = ops.pm_fwd(z2, W3, mode, t2, gsize=N, ext=True)
         t3, s3 = _bn_table(ps, g3, b3, bns[2], R)
         g, sel3, zsel3 = _pool(*ops.pm_group_ext(ev, ei, B), t3, s3)
-        rows['memory'] = sel3
+        rows['memory'], rows['memory_pool'] = sel3, g                    # the pooled output too, for the tests
         shift4 = ops.linear(g.contiguous(), W4g)                          # (B, 512) = g W4g^T, once per track
         z4, ps4, _, _ = ops.pm_fwd(z2, W4p, mode, t2, shift=shift4, gsize=N)
         t4, s4 = _bn_table(ps4, g4, b4, bns[3], R)

@@ -32,8 +32,9 @@ def grm_train_inputs(seed, B, **kw):
 
 
 class _Net:
-    def __init__(self, sd, stats, dropout, generator):
+    def __init__(self, sd, stats, dropout, generator, relu_masks=None):
         self.sd, self.stats, self.p, self.gen = sd, stats, dropout, generator
+        self.masks = relu_masks or {}
 
     def conv(self, x, name):
         w = self.sd[name + '.weight']
@@ -46,7 +47,10 @@ class _Net:
                             training=True, momentum=momentum, eps=eps)
 
     def cbr(self, x, conv, bn, eps=1e-3, momentum=0.01):
-        return torch.relu(self.bn(self.conv(x, conv), bn, eps, momentum))
+        h = self.bn(self.conv(x, conv), bn, eps, momentum)
+        if bn in self.masks:                                  # the ReLU taken at a given mask: h where the mask is set, else 0
+            return torch.where(self.masks[bn].to(h.device), h, torch.zeros_like(h))
+        return torch.relu(h)
 
     def drop(self, x):
         return F.dropout(x, self.p, training=True) if self.p > 0 else x
@@ -77,16 +81,22 @@ def _pool(y, groups, rows):
     return y.gather(1, rows.long().to(y.device).unsqueeze(1)).squeeze(1)
 
 
-def grm_train_step(state_dict, inputs, device='cpu', pooled_rows=None, dropout=0.0, generator=None, dtype=torch.float64, record=None):
+def grm_train_step(state_dict, inputs, device='cpu', pooled_rows=None, dropout=0.0, generator=None, dtype=torch.float64, record=None,
+                   relu_masks=None, path_outputs=None):
     """one training forward + backward in float64 (or ``dtype``).  state_dict: GeometryTransformer keys (no 'reg.' prefix); inputs: the data-dict
     keys geo_memory_points, geo_query_points, geo_query_boxes, geo_query_num, gt_geo_query_boxes.  Returns (losses {name: float},
     grads {param: tensor}, running stats after the step {buffer: tensor}).  ``record`` (a dict) receives the inputs of the two
-    max-pools: 'memory' (B, N, 512) and 'query' (B*Q, P, 256)"""
+    max-pools: 'memory' (B, N, 512) and 'query' (B*Q, P, 256), and the outputs of the two point paths: 'memory_out' (B*N, 256), the
+    memory_mlp output, 'memory_pool' (B, 512) the pooled memory_encoder output, and 'query_pool' (B*Q, 256) the pooled
+    query_encoder output.  ``relu_masks`` {BatchNorm name: bool (rows, C)} takes that layer's ReLU at the given mask instead of at
+    the sign of its input, so that a test can restate a step at the masks the device took.  ``path_outputs`` {'memory_out',
+    'query_pool'} replaces the two point paths' outputs by given tensors (constants: the point layers then get no gradient and are
+    left out of grads), so that a test can restate the rest of the step from the device's point-path outputs"""
     stat_keys = ('running_mean', 'running_var', 'num_batches_tracked')
     sd = {k: v.to(device, dtype).clone().requires_grad_(True) for k, v in state_dict.items() if not k.endswith(stat_keys)}
     stats = {k: v.to(device).clone().to(dtype) if not k.endswith('num_batches_tracked') else v.to(device).clone()
              for k, v in state_dict.items() if k.endswith(stat_keys)}
-    net = _Net(sd, stats, dropout, generator)
+    net = _Net(sd, stats, dropout, generator, relu_masks)
     pr = pooled_rows or {}
     m = inputs['geo_memory_points'].to(device, dtype)
     B, N, _ = m.shape
@@ -97,8 +107,13 @@ def grm_train_step(state_dict, inputs, device='cpu', pooled_rows=None, dropout=0
     g = _pool(y3, B, pr.get('memory'))
     if record is not None:
         record['memory'] = y3.detach().view(B, N, -1)
+        record['memory_pool'] = g.detach()
     x4 = torch.cat([y2.view(B, N, -1), g.unsqueeze(1).expand(B, N, g.shape[1])], dim=2).reshape(B * N, -1)
     mem = net.cbr(net.cbr(x4, 'memory_mlp.0', 'memory_mlp.1'), 'memory_mlp.3', 'memory_mlp.4')
+    if record is not None:
+        record['memory_out'] = mem.detach()
+    if path_outputs is not None:
+        mem = path_outputs['memory_out'].to(device, dtype)
     qp = inputs['geo_query_points'].to(device, dtype)
     _, Q, P, _ = qp.shape
     h = qp.reshape(B * Q * P, -1)
@@ -107,6 +122,9 @@ def grm_train_step(state_dict, inputs, device='cpu', pooled_rows=None, dropout=0
     q = _pool(h, B * Q, pr.get('query'))
     if record is not None:
         record['query'] = h.detach().view(B * Q, P, -1)
+        record['query_pool'] = q.detach()
+    if path_outputs is not None:
+        q = path_outputs['query_pool'].to(device, dtype)
     q = net.cbr(net.cbr(q, 'query_mlp.0', 'query_mlp.1'), 'query_mlp.3', 'query_mlp.4')
     E = q.shape[1]
     query, key = q.view(B, Q, E), mem.view(B, N, E)
@@ -140,7 +158,7 @@ def grm_train_step(state_dict, inputs, device='cpu', pooled_rows=None, dropout=0
     loss = 0.1 * cls_loss + 2 * reg_loss
     loss.backward()
     losses = {'cls_loss': cls_loss.item(), 'reg_loss': reg_loss.item(), 'geometry_loss': loss.item()}
-    return losses, {k: v.grad.detach() for k, v in sd.items()}, stats
+    return losses, {k: v.grad.detach() for k, v in sd.items() if v.grad is not None}, stats
 
 
 def probe(name, shape, seed):

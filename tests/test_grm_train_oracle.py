@@ -45,6 +45,26 @@ def test_restatement_matches_reference_golden():
             assert torch.allclose(v, ref.double(), rtol=1e-6, atol=1e-7), k
 
 
+def test_pooling_at_the_argmax_rows_is_the_default_path():
+    """pooled_rows at the float64 argmax of each group and channel reproduces the max-pooled step bit for bit (the device tests pool
+    the restatement at the device's rows through this hook); record holds the inputs of both maxes"""
+    B = 2
+    sd = seeded_state_dict()
+    inp = grm_train_ref.grm_train_inputs(SEED, B)
+    rec = {}
+    losses, grads, stats = grm_train_ref.grm_train_step(sd, inp, record=rec)
+    Q, P = inp['geo_query_points'].shape[1:3]
+    assert rec['memory'].shape == (B, 4096, 512) and rec['query'].shape == (B * Q, P, 256)
+    rows = {k: rec[k].max(dim=1)[1].int() for k in ('memory', 'query')}
+    l2, g2, s2 = grm_train_ref.grm_train_step(sd, inp, pooled_rows=rows)
+    assert l2 == losses
+    assert set(g2) == set(grads)
+    for k in grads:
+        assert torch.equal(g2[k], grads[k]), k
+    for k in stats:
+        assert torch.equal(s2[k], stats[k]), k
+
+
 def test_targets_pick_the_nearest_anchor():
     gt = grm_train_ref.grm_train_gt(SEED, 4, 3)
     from detzero_b200.refine.modules import TargetAssigner
