@@ -33,24 +33,30 @@
 //   4. The crop tests each point in float64 world coordinates relative to the box centre (rounded to float32 for the shared
 //      float32 test), where the reference tests float32 world points: only points within ~1e-3 m of an enlarged face can differ.
 //
-// Training samples (the training branch of WaymoGeometryDataset / WaymoConfidenceDataset.extract_track_feature, with
-// geometry_augment.py:65-77 augment_single_box for the GRM; restated in oracle/refine_train_data_ref.py):
+// Training samples (the training branch of WaymoPositionDataset / WaymoGeometryDataset / WaymoConfidenceDataset
+// .extract_track_feature, with geometry_augment.py:65-77 augment_single_box for the GRM; restated in oracle/refine_train_data_ref.py,
+// and for the PRM in tests/prm_train_data_ref.py):
 //   crop    dz_crop_tracks runs prep / count / scan / write once and copies every in-box point row to a frame of its own (one pose
 //           per box), the layout the builders read with crop = 0, so the crop leaves the epoch loop.
 //   draw    k_rd_draw, one block per track, keyed on (epoch_seed(seed, epoch), track_uid) with the streams ST_TR_*:
-//             eligible slots: the matched ones (GRM), every valid one (CRM); m of them
+//             eligible slots: the matched ones (PRM, GRM), every valid one (CRM); m of them
 //             kept count n = lo + key mod (m - lo + 1), lo = min(5, m), key = mix64(key_base(.., 0, ST_TR_COUNT)): the bias of a
 //               64-bit key reduced mod at most 200 is below 200 / 2^64 < 2^-56
 //             kept: the k-subset rule of select (k = n of the m eligible ranks), in ascending slot order
-//             GRM queries: min(nq, n) kept positions by the same rule; CRM init box: a kept position, key mod n (ST_TR_INIT)
+//             GRM queries: min(nq, n) kept positions by the same rule; PRM / CRM init box: a kept position, key mod n (ST_TR_INIT)
 //             GRM flip bits: the top bit of key(i) of ST_TR_FLIP per kept position i
 //           epoch_seed(seed, epoch) = mix64(mix64(seed) + epoch); the point samples of a training build use it as their seed.
-//   build   dz_refine_train_inputs gathers the kept slots into a derived track table and runs the passes above on it, with the
-//           drawn query positions in k_rd_track (GRM), the drawn init box in k_rd_prep (CRM) and the flip applied to box-local y
-//           of the memory rows in the write pass (GRM; the query points are never flipped, as the reference copies them first).
+//   build   dz_refine_train_inputs (GRM, CRM) and dz_position_train_inputs (PRM) gather the kept slots into a derived track table and
+//           run the passes above on it, with the drawn query positions in k_rd_track (GRM), the drawn init box in k_rd_prep (PRM,
+//           CRM) and the flip applied to box-local y of the memory rows in the write pass (GRM; the query points are never flipped,
+//           as the reference copies them first).  The PRM's gt_pos_trajectory is the kept ground truth taken into the drawn init
+//           box's frame by k_rd_prep, through the same float64 to_init_frame as pos_trajectory (init_coords_transform: heading
+//           limited to [-pi, pi) before and after the rotation).
+//   The PRM build keeps deviations 1 (keyed sampling, streams 0 and 1 on the kept positions), 2 (float64 geometry) and 5 unchanged.
 //   Deviation 5: the reference keeps random.sample's order of the kept boxes; here they are in ascending slot order.  Every
 //   consumer is invariant to the order of a track's boxes (per-box encoders, max-pools, BatchNorm statistics, decoder attention
-//   over the memory, summed losses), so no distribution the model sees changes.
+//   over the memory, summed losses), so no distribution the model sees changes.  The PRM decoder uses no order-dependent mask
+//   (PositionHead.forward passes attn_mask = None), so its ascending order changes nothing the model sees either.
 #include "common.cuh"
 #include "boxgeom.cuh"
 #include "refine_frame.cuh"
@@ -80,6 +86,8 @@ struct RdParams {
     // training builds (NULL otherwise): drawn GRM query positions (B, nq), CRM init positions (B), GRM flip bits (B, L); the
     // derived gt_geo_trajectory (B, L, 7) f32 and gt_geo_query_boxes (B, qout, 7)
     const int* qsel; const int* init; const unsigned char* flip; const float* gt_traj; float* gt_box_f;
+    // PRM training builds (NULL otherwise): the kept ground truth (B, L, 7) f64 world, and gt_pos_trajectory (B, L, 7) f32
+    const double* gt_w; float* gt_pos;
     // dz_crop_tracks: the first output row of each box slot, the output rows (width C)
     const int* rbase; float* rows;
 };
@@ -118,6 +126,7 @@ __global__ void k_rd_prep(RdParams P) {
     if (j >= L) {
         o.p0 = o.p1 = 0;
         if (P.traj) for (int d = 0; d < 7; ++d) P.traj[(size_t)t * 7 + d] = 0.f;
+        if (P.gt_pos) for (int d = 0; d < 7; ++d) P.gt_pos[(size_t)t * 7 + d] = 0.f;
         if (P.kind == RD_PRM) P.box_f[t] = 1.f;                          // padding_mask
         if (P.kind == RD_CRM) P.box_f[t] = -1.f;                         // conf_score padding
         return;
@@ -167,6 +176,11 @@ __global__ void k_rd_prep(RdParams P) {
     for (int d = 0; d < 3; ++d) o.cc[24 + d] = loc[d];
     if (P.kind == RD_PRM) {
         for (int d = 0; d < 7; ++d) P.traj[(size_t)t * 7 + d] = (float)loc[d];
+        if (P.gt_pos) {
+            double g[7];
+            to_init_frame(fr, bi, P.gt_w + (size_t)t * 7, g);
+            for (int d = 0; d < 7; ++d) P.gt_pos[(size_t)t * 7 + d] = (float)g[d];
+        }
         P.box_f[t] = 0.f;
         if (j == 0) {
             for (int d = 0; d < 6; ++d) P.track_f[(size_t)b * 7 + d] = (float)bi[d];
@@ -561,17 +575,18 @@ extern "C" int dz_refine_train_draw(int kind, const int32_t* box_num, const uint
                                     int nq, unsigned long long seed, long long epoch, int32_t* kept, int32_t* n_kept,
                                     int32_t* query_slots, int32_t* init_slot, uint8_t* flip, void* ws, size_t ws_bytes,
                                     dz_stream_t stream) {
-    DZ_CHECK_ARG((kind == RD_CRM || kind == RD_GRM) && box_num && track_uid && B >= 0 && L >= 1 && kept && n_kept);
+    DZ_CHECK_ARG(kind >= RD_PRM && kind <= RD_GRM && box_num && track_uid && B >= 0 && L >= 1 && kept && n_kept);
     DZ_CHECK_ARG(kind != RD_GRM || (matched && query_slots && flip && nq >= 1 && nq <= 8));
+    DZ_CHECK_ARG(kind != RD_PRM || (matched && init_slot));
     DZ_CHECK_ARG(kind != RD_CRM || init_slot);
     if (B == 0) return DZ_OK;
     DZ_CHECK_WS(dz_refine_train_draw_ws_bytes(B, L));
     DzCarve cv((char*)ws);
     RdDraw D;
-    D.box_num = box_num; D.matched = kind == RD_GRM ? matched : nullptr; D.uid = (const long long*)track_uid;
+    D.box_num = box_num; D.matched = kind != RD_CRM ? matched : nullptr; D.uid = (const long long*)track_uid;
     D.B = B; D.L = L; D.kind = kind; D.nq = nq; D.seed = epoch_seed(seed, epoch);
     D.elig = carve_draw(cv, B, L); D.kept = kept; D.n_kept = n_kept;
-    D.qsel = kind == RD_GRM ? query_slots : nullptr; D.init = kind == RD_CRM ? init_slot : nullptr;
+    D.qsel = kind == RD_GRM ? query_slots : nullptr; D.init = kind != RD_GRM ? init_slot : nullptr;
     D.flip = kind == RD_GRM ? flip : nullptr;
     k_rd_draw<<<B, 256, 0, (cudaStream_t)stream>>>(D);
     DZ_LAUNCH_CHECK();
@@ -579,11 +594,13 @@ extern "C" int dz_refine_train_draw(int kind, const int32_t* box_num, const uint
 }
 
 // the kept slots of each track -> the derived track table (boxes, frame_of_box, scores) and the kept targets: gt_geo_trajectory
-// (GRM, f32 world, zero padded) and iou (CRM, -1 padded).  One thread per derived slot.
+// (GRM, f32 world, zero padded), the kept ground truth (PRM, f64 world, zero padded) and iou (CRM, -1 padded).  One thread per
+// derived slot.
 __global__ void k_rd_gather(const double* __restrict__ boxes, const int* __restrict__ fob, const float* __restrict__ scores,
                             const int* __restrict__ kept, const int* __restrict__ n_kept, const double* __restrict__ gt_boxes,
                             const float* __restrict__ iou, int B, int L, double* __restrict__ dboxes, int* __restrict__ dfob,
-                            float* __restrict__ dscores, float* __restrict__ gt_traj, float* __restrict__ iou_out) {
+                            float* __restrict__ dscores, float* __restrict__ gt_traj, double* __restrict__ dgt,
+                            float* __restrict__ iou_out) {
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= B * L) return;
     const int b = t / L, i = t % L;
@@ -593,22 +610,48 @@ __global__ void k_rd_gather(const double* __restrict__ boxes, const int* __restr
     dfob[t] = live ? fob[s] : 0;
     dscores[t] = live ? scores[s] : 0.f;
     if (gt_traj) for (int d = 0; d < 7; ++d) gt_traj[(size_t)t * 7 + d] = live ? (float)gt_boxes[s * 7 + d] : 0.f;
+    if (dgt) for (int d = 0; d < 7; ++d) dgt[(size_t)t * 7 + d] = live ? gt_boxes[s * 7 + d] : 0.0;
     if (iou_out) iou_out[t] = live ? iou[s] : -1.f;
 }
 
-struct RdTrainWs { double* boxes; int* fob; float* scores; RdWs rd; };
+struct RdTrainWs { double* boxes; int* fob; float* scores; double* gt; RdWs rd; };
 
 static RdTrainWs carve_rd_train(DzCarve& cv, int kind, int B, int L, int max_frame_points, int kq, int km, int nq) {
     RdTrainWs w;
     w.boxes = cv.take<double>((size_t)B * L * 7);
     w.fob = cv.take<int>((size_t)B * L);
     w.scores = cv.take<float>((size_t)B * L);
+    w.gt = kind == RD_PRM ? cv.take<double>((size_t)B * L * 7) : nullptr;
     w.rd = carve_rd(cv, kind, B, L, max_frame_points, kq, km, nq);
     return w;
 }
 
 extern "C" size_t dz_refine_train_inputs_ws_bytes(int kind, int B, int L, int max_frame_points, int kq, int km, int nq) {
     return dz_carve_bytes(carve_rd_train, kind, B, L, max_frame_points, kq, km, nq);
+}
+
+// what every training build shares: the gather of the kept slots (with the kind's kept targets) and the RdParams of the passes on
+// the derived table; the caller adds the kind's own outputs and launches
+static RdParams rd_train_params(const RdTrainWs& w, int kind, const float* points, int pt_stride, const int32_t* frame_offsets,
+                                int n_frames, const double* poses, const double* boxes, const int32_t* frame_of_box,
+                                const float* scores, const int32_t* cls, const int64_t* track_uid, const double* gt_boxes,
+                                const float* iou, int B, int L, int kq, int km, int nq, int q_out, double enlarge_scale,
+                                int crop_on_bev, int crop, unsigned long long seed, long long epoch, const int32_t* kept,
+                                const int32_t* n_kept, float* gt_traj, float* iou_out, int32_t* counts, int32_t* sel,
+                                cudaStream_t st) {
+    k_rd_gather<<<dz_cdiv(B * L, 128), 128, 0, st>>>(boxes, frame_of_box, scores, kept, n_kept, gt_boxes, iou, B, L, w.boxes, w.fob,
+                                                     w.scores, kind == RD_GRM ? gt_traj : nullptr, w.gt,
+                                                     kind == RD_CRM ? iou_out : nullptr);
+    RdParams P = {};
+    P.pts = points; P.pstride = pt_stride; P.foff = frame_offsets; P.F = n_frames;
+    P.poses = poses; P.boxes = w.boxes; P.fob = w.fob; P.scores = w.scores; P.box_num = n_kept; P.cls = cls;
+    P.uid = (const long long*)track_uid;
+    P.B = B; P.L = L; P.kind = kind; P.with_class = 0; P.C = kind == RD_GRM ? 4 : 32;
+    P.kq = kq; P.km = kind == RD_CRM ? 0 : km; P.nq = nq; P.qout = q_out; P.crop = crop ? 1 : 0; P.bev = crop_on_bev ? 1 : 0;
+    P.enlarge = enlarge_scale; P.seed = epoch_seed(seed, epoch);
+    P.n_chunks = w.rd.n_chunks; P.bx = w.rd.bx; P.cc = w.rd.cc; P.n = counts ? counts : w.rd.n; P.goff = w.rd.goff;
+    P.gtot = w.rd.gtot; P.qnum = w.rd.qnum; P.qidx = w.rd.qidx; P.sel = sel ? sel : w.rd.sel;
+    return P;
 }
 
 extern "C" int dz_refine_train_inputs(int kind, const float* points, int pt_stride, const int32_t* frame_offsets, int n_frames,
@@ -631,20 +674,42 @@ extern "C" int dz_refine_train_inputs(int kind, const float* points, int pt_stri
     DzCarve cv((char*)ws);
     const RdTrainWs w = carve_rd_train(cv, kind, B, L, max_frame_points, kq, km, nq);
     cudaStream_t st = (cudaStream_t)stream;
-    k_rd_gather<<<dz_cdiv(B * L, 128), 128, 0, st>>>(boxes, frame_of_box, scores, kept, n_kept, gt_boxes, iou, B, L, w.boxes, w.fob,
-                                                     w.scores, kind == RD_GRM ? gt_traj : nullptr, kind == RD_CRM ? iou_out : nullptr);
-    RdParams P = {};
-    P.pts = points; P.pstride = pt_stride; P.foff = frame_offsets; P.F = n_frames;
-    P.poses = poses; P.boxes = w.boxes; P.fob = w.fob; P.scores = w.scores; P.box_num = n_kept; P.cls = cls;
-    P.uid = (const long long*)track_uid;
-    P.B = B; P.L = L; P.kind = kind; P.with_class = 0; P.C = kind == RD_GRM ? 4 : 32;
-    P.kq = kq; P.km = kind == RD_CRM ? 0 : km; P.nq = nq; P.qout = q_out; P.crop = crop ? 1 : 0; P.bev = crop_on_bev ? 1 : 0;
-    P.enlarge = enlarge_scale; P.seed = epoch_seed(seed, epoch);
-    P.n_chunks = w.rd.n_chunks; P.bx = w.rd.bx; P.cc = w.rd.cc; P.n = counts ? counts : w.rd.n; P.goff = w.rd.goff;
-    P.gtot = w.rd.gtot; P.qnum = w.rd.qnum; P.qidx = w.rd.qidx; P.sel = sel ? sel : w.rd.sel;
+    RdParams P = rd_train_params(w, kind, points, pt_stride, frame_offsets, n_frames, poses, boxes, frame_of_box, scores, cls,
+                                 track_uid, gt_boxes, iou, B, L, kq, km, nq, q_out, enlarge_scale, crop_on_bev, crop, seed, epoch,
+                                 kept, n_kept, gt_traj, iou_out, counts, sel, st);
     P.q_pts = q_pts; P.m_pts = m_pts; P.traj = kind == RD_GRM ? traj : nullptr; P.box_f = box_f; P.query_num = query_num;
     if (kind == RD_GRM) { P.qsel = query_slots; P.flip = flip; P.gt_traj = gt_traj; P.gt_box_f = gt_box_f; }
     else P.init = init_slot;
+    launch_rd(P, st);
+    DZ_LAUNCH_CHECK();
+    return DZ_OK;
+}
+
+extern "C" size_t dz_position_train_inputs_ws_bytes(int B, int L, int max_frame_points, int kq, int km) {
+    return dz_carve_bytes(carve_rd_train, (int)RD_PRM, B, L, max_frame_points, kq, km, 1);
+}
+
+extern "C" int dz_position_train_inputs(const float* points, int pt_stride, const int32_t* frame_offsets, int n_frames,
+                                        int max_frame_points, const double* poses, const double* boxes, const int32_t* frame_of_box,
+                                        const float* scores, const int32_t* cls, const int64_t* track_uid, const double* gt_boxes,
+                                        int B, int L, int kq, int km, double enlarge_scale, int crop_on_bev, int crop,
+                                        unsigned long long seed, long long epoch, const int32_t* kept, const int32_t* n_kept,
+                                        const int32_t* init_slot, float* q_pts, float* m_pts, float* traj, float* gt_traj,
+                                        float* padding_mask, float* init_box, int32_t* counts, int32_t* sel, void* ws,
+                                        size_t ws_bytes, dz_stream_t stream) {
+    DZ_CHECK_ARG(pt_stride >= 5 && frame_offsets && n_frames >= 1 && max_frame_points >= 0 && poses && boxes && frame_of_box &&
+                 scores && cls && track_uid && gt_boxes && B >= 0 && L >= 1 && kq >= 1 && km >= 1 && kept && n_kept && init_slot &&
+                 q_pts && m_pts && traj && gt_traj && padding_mask && init_box && (points || max_frame_points == 0));
+    if (B == 0) return DZ_OK;
+    DZ_CHECK_WS(dz_position_train_inputs_ws_bytes(B, L, max_frame_points, kq, km));
+    DzCarve cv((char*)ws);
+    const RdTrainWs w = carve_rd_train(cv, RD_PRM, B, L, max_frame_points, kq, km, 1);
+    cudaStream_t st = (cudaStream_t)stream;
+    RdParams P = rd_train_params(w, RD_PRM, points, pt_stride, frame_offsets, n_frames, poses, boxes, frame_of_box, scores, cls,
+                                 track_uid, gt_boxes, nullptr, B, L, kq, km, 1, 0, enlarge_scale, crop_on_bev, crop, seed, epoch,
+                                 kept, n_kept, nullptr, nullptr, counts, sel, st);
+    P.q_pts = q_pts; P.m_pts = m_pts; P.traj = traj; P.box_f = padding_mask; P.track_f = init_box;
+    P.init = init_slot; P.gt_w = w.gt; P.gt_pos = gt_traj;
     launch_rd(P, st);
     DZ_LAUNCH_CHECK();
     return DZ_OK;

@@ -9,10 +9,10 @@ that function and the other deliberate deviations (float64 geometry, per-track G
 ``combine_frames`` puts the refined tracks of a sequence together into per-frame result rows (csrc/combine.cu), replacing
 daemon/combine_output.py's convert_frame_format and combine_det.  ``track_targets`` attaches the ground truth of an assignment
 (track.assign_track_target) to a TrackBatch (csrc/refine_gt.cu); refine.score turns it into the recall records and IoU labels.
-Training samples: ``crop_tracks`` crops every box once into per-box frames; ``geometry_training_inputs`` /
-``confidence_training_inputs`` build the training branch of the GRM / CRM datasets from them each epoch, with every random draw keyed
-on (seed, epoch, track_uid) (csrc/refine_data.cu); ``training_order`` is the epoch's shuffled track list (streams 10 and 11 of the
-same key function, on the host).
+Training samples: ``crop_tracks`` crops every box once into per-box frames; ``position_training_inputs`` /
+``geometry_training_inputs`` / ``confidence_training_inputs`` build the training branch of the PRM / GRM / CRM datasets from them
+each epoch, with every random draw keyed on (seed, epoch, track_uid) (csrc/refine_data.cu); ``training_order`` is the epoch's
+shuffled track list (streams 10 and 11 of the same key function, on the host).
 """
 import zlib
 
@@ -291,6 +291,11 @@ def grm_train_cfg():
     return dict(grm_data_cfg(), AUGMENTOR={'AUGMENT_SINGLE': True, 'AUGMENT_FULL': False})
 
 
+def prm_train_cfg():
+    """waymo_prm_dataset.yaml in training (AUGMENT_FULL off, as shipped; LOCAL_SCALE and the rest feed only augment_full_track)"""
+    return dict(prm_data_cfg(), AUGMENTOR={'AUGMENT_FULL': False})
+
+
 def crm_train_cfg():
     """waymo_crm_dataset.yaml in training (the CRM dataset applies no augmentation)"""
     return dict(crm_data_cfg(), AUGMENTOR={'AUGMENT_SINGLE': True, 'AUGMENT_FULL': False})
@@ -312,10 +317,10 @@ def _train_build(kind, frames, frame_offsets, poses, tracks, cfg, seed, epoch, c
     off, F, max_pts, poses = _frames_args(frames, frame_offsets, poses)
     dev = frames.device
     B, L = len(tracks), tracks.L
-    if kind == CRM and int(cfg['QUERY_NUM']) != L:
+    if kind != GRM and int(cfg['QUERY_NUM']) != L:
         raise ValueError('QUERY_NUM %d != the track tables\' %d box slots' % (cfg['QUERY_NUM'], L))
     kq = int(cfg['QUERY_POINTS_NUM'])
-    km = int(cfg['MEMORY_POINTS_NUM']) if kind == GRM else 0
+    km = int(cfg['MEMORY_POINTS_NUM']) if kind != CRM else 0
     nq = int(cfg['QUERY_NUM']) if kind == GRM else 1
     seed, epoch = int(seed) & ((1 << 64) - 1), int(epoch)
     i32 = dict(dtype=torch.int32, device=dev)
@@ -323,7 +328,7 @@ def _train_build(kind, frames, frame_offsets, poses, tracks, cfg, seed, epoch, c
     kept = torch.empty((B, L), **i32)
     n_kept = torch.empty((B,), **i32)
     qsel = torch.empty((B, nq), **i32) if kind == GRM else None
-    init = torch.empty((B,), **i32) if kind == CRM else None
+    init = torch.empty((B,), **i32) if kind != GRM else None
     flip = torch.empty((B, L), dtype=torch.uint8, device=dev) if kind == GRM else None
     if B:
         ws = ops.workspace(lib().dz_refine_train_draw_ws_bytes(B, L), dev, 'refine_data')
@@ -334,7 +339,7 @@ def _train_build(kind, frames, frame_offsets, poses, tracks, cfg, seed, epoch, c
         if kind == GRM and not augment_single:
             flip.zero_()
     q_out = min(nq, int(n_kept.max())) if kind == GRM and B else 0
-    gt_traj = gt_box_f = iou_out = qn = m = traj = None
+    gt_traj = gt_box_f = iou_out = qn = m = traj = init_box = None
     if kind == GRM:
         q = torch.empty((B, q_out, kq, 4), **f32)
         m = torch.empty((B, km, 11), **f32)
@@ -344,6 +349,14 @@ def _train_build(kind, frames, frame_offsets, poses, tracks, cfg, seed, epoch, c
         gt_traj = torch.empty((B, L, 7), **f32)
         qn = torch.empty((B,), **i32)
         nsel = nq * kq + km
+    elif kind == PRM:
+        q = torch.empty((B, L, kq, 32), **f32)
+        m = torch.empty((B, L, km, 32), **f32)
+        traj = torch.empty((B, L, 7), **f32)
+        gt_traj = torch.empty((B, L, 7), **f32)
+        box_f = torch.empty((B, L), **f32)
+        init_box = torch.empty((B, 7), **f32)
+        nsel = L * (kq + km)
     else:
         q = torch.empty((B, L, kq, 32), **f32)
         box_f = torch.empty((B, L), **f32)
@@ -351,7 +364,18 @@ def _train_build(kind, frames, frame_offsets, poses, tracks, cfg, seed, epoch, c
         nsel = L * kq
     counts = torch.empty((B, L), **i32) if return_selection else None
     sel = torch.full((B, nsel), -1, **i32) if return_selection else None
-    if B:
+    if B and kind == PRM:
+        enlarge, bev = float(cfg.get('ENLARGE_SCALE', 1.1)), int(bool(cfg.get('CROP_ON_BEV', False)))
+        ws = ops.workspace(lib().dz_position_train_inputs_ws_bytes(B, L, max_pts, kq, km), dev, 'refine_data')
+        check(lib().dz_position_train_inputs(ops._p(frames), frames.stride(0), ops._p(off), F, max_pts, ops._p(poses),
+                                             ops._p(tracks.boxes), ops._p(tracks.frame_of_box), ops._p(tracks.scores),
+                                             ops._p(tracks.cls), ops._p(tracks.track_uid), ops._p(gt_boxes), B, L, kq, km, enlarge,
+                                             bev, int(bool(crop)), seed, epoch, ops._p(kept), ops._p(n_kept), ops._p(init), ops._p(q),
+                                             ops._p(m), ops._p(traj), ops._p(gt_traj), ops._p(box_f), ops._p(init_box),
+                                             ops._p(counts), ops._p(sel), ops._p(ws), ws.numel(), ops._stream()),
+              'position_train_inputs')
+        ops._count(8)
+    elif B:
         ws = ops.workspace(lib().dz_refine_train_inputs_ws_bytes(kind, B, L, max_pts, kq, km, nq), dev, 'refine_data')
         check(lib().dz_refine_train_inputs(kind, ops._p(frames), frames.stride(0), ops._p(off), F, max_pts, ops._p(poses),
                                            ops._p(tracks.boxes), ops._p(tracks.frame_of_box), ops._p(tracks.scores), ops._p(tracks.cls),
@@ -365,6 +389,9 @@ def _train_build(kind, frames, frame_offsets, poses, tracks, cfg, seed, epoch, c
     if kind == GRM:
         out = {'geo_query_points': q, 'geo_query_boxes': box_f, 'gt_geo_query_boxes': gt_box_f, 'geo_memory_points': m,
                'geo_query_num': qn, 'geo_trajectory': traj, 'gt_geo_trajectory': gt_traj}
+    elif kind == PRM:
+        out = {'pos_query_points': q, 'pos_memory_points': m, 'pos_trajectory': traj, 'gt_pos_trajectory': gt_traj,
+               'padding_mask': box_f, 'pos_init_box': init_box, 'box_num': n_kept}
     else:
         out = {'conf_points': q, 'conf_score': box_f, 'iou': iou_out, 'box_num': n_kept}
     if return_selection:
@@ -402,6 +429,27 @@ def geometry_training_inputs(frames, frame_offsets, poses, tracks, targets, cfg=
                         gt_boxes=targets.gt_boxes.to(torch.float64).contiguous(), matched=targets.matched.to(torch.uint8).contiguous())
 
 
+def position_training_inputs(frames, frame_offsets, poses, tracks, targets, cfg=None, seed=0, epoch=0, crop=True,
+                             return_selection=False):
+    """PRM training samples (WaymoPositionDataset.extract_track_feature, training) of every track: a random subset of its matched
+    boxes (n uniform on min(5, m) .. m of m) and a random init box among them in place of n // 2, keyed on (seed, epoch,
+    track_uid) (csrc/refine_data.cu).  targets: the TrackTargets of ``tracks`` (track_targets); every track must be a matched
+    tracklet with a matched box.  Returns the dict PositionTransformer reads in training: pos_query_points (B, L, 256, 32),
+    pos_memory_points (B, L, 48, 32), pos_trajectory and gt_pos_trajectory (B, L, 7) (the kept boxes and their ground truth in the
+    init box's frame), pos_init_box (B, 7), padding_mask (B, L) and box_num (B) the kept count.  Padded boxes are zero rows.  Kept
+    boxes are in ascending slot order.  return_selection adds kept (B, L) source slots (-1 padding), init_slot (B) (a kept
+    position), crop_counts and selection (position_inputs' layout, on the kept positions).  crop=False: frames are per-box
+    (crop_tracks)."""
+    cfg = _cfg(cfg, prm_train_cfg())
+    if int(cfg['MEMORY_POINTS_NUM']) != 48:
+        raise ValueError('MEMORY_POINTS_NUM must be 48 (PositionHead.forward builds its cross-attention mask for 48 memory points)')
+    if len(tracks) and not bool(_grm_trainable(targets, tracks.box_num).all()):
+        raise ValueError('position_training_inputs: every track must be a matched tracklet with at least one matched box '
+                         '(training_order excludes the others)')
+    return _train_build(PRM, frames, frame_offsets, poses, tracks, cfg, seed, epoch, crop, return_selection,
+                        gt_boxes=targets.gt_boxes.to(torch.float64).contiguous(), matched=targets.matched.to(torch.uint8).contiguous())
+
+
 def confidence_training_inputs(frames, frame_offsets, poses, tracks, iou, cfg=None, seed=0, epoch=0, crop=True,
                                return_selection=False):
     """CRM training samples (WaymoConfidenceDataset.extract_track_feature, training) of every track: a random subset of its boxes
@@ -421,12 +469,13 @@ ST_ORDER, ST_NEG = 10, 11
 
 def training_order(targets, kind, seed=0, epoch=0):
     """The track indices of one training epoch (host int64), keyed on (seed, epoch) as the samples are: the dataset's list shuffled
-    as the DataLoader does.  'grm': every matched tracklet with at least one matched box (load_infos_worker drops unmatched tracks
-    without IOU_NAME), once.  'crm': every positive (matched) track once, each paired with a negative drawn uniformly with
-    replacement (WaymoConfidenceDataset.__getitem__), 2 x positives in all.  Raises when the CRM has no negative track."""
+    as the DataLoader does.  'grm' and 'prm': every matched tracklet with at least one matched box (load_infos_worker drops
+    unmatched tracks without IOU_NAME, and the PRM's extract_track_feature cannot run on a track without one), once.  'crm': every
+    positive (matched) track once, each paired with a negative drawn uniformly with replacement (WaymoConfidenceDataset.__getitem__),
+    2 x positives in all.  Raises when the CRM has no negative track."""
     es = epoch_seed(seed, epoch)
     mt = targets.matched_tracklet.cpu().numpy() != 0
-    if kind == 'grm':
+    if kind in ('grm', 'prm'):
         ok = mt & (targets.matched.cpu().numpy() != 0).any(1)
         items = np.nonzero(ok)[0]
     elif kind == 'crm':
@@ -437,7 +486,7 @@ def training_order(targets, kind, seed=0, epoch=0):
             pick = _mix64(np.uint64(_key_base(es, 0, 0, ST_NEG)) + np.arange(len(pos), dtype=np.uint64)) % np.uint64(max(len(neg), 1))
         items = np.stack([pos, neg[pick.astype(np.int64)] if len(pos) else pos], 1).reshape(-1)
     else:
-        raise ValueError("kind must be 'grm' or 'crm'")
+        raise ValueError("kind must be 'prm', 'grm' or 'crm'")
     with np.errstate(over='ignore'):
         keys = _mix64(np.uint64(_key_base(es, 0, 0, ST_ORDER)) + np.arange(len(items), dtype=np.uint64))
     return items[np.argsort(keys, kind='stable')].astype(np.int64)

@@ -12,7 +12,7 @@ token-major on libdetzero_b200:
 Layout: activations are (tokens, channels) row-major; the reference's (B,C,P) <-> (P,B,C) permute copies disappear.
 Every 1x1 Conv / Linear (+BatchNorm eval +ReLU) is one fused GEMM launch; attention streams keys with an online
 softmax and never materialises the (B*H, Pq, Pk) score tensor; the query scaling head_dim**-0.5 is folded into the
-in-projection epilogue.  ConfidencePointnet and GeometryTransformer also train (refine/train.py); the PRM is eval only.
+in-projection epilogue.  All three refiners also train (refine/train.py).
 The ``forward_train`` methods follow the reference op for op through torch autograd, dropout included, token-major."""
 import copy
 import math
@@ -216,8 +216,9 @@ class MultiheadAttention(nn.Module):
                          None if self.out_proj.bias is None else self.out_proj.bias.detach().float(), False, mode=mode)
         return out.view(B, Pq, E)
 
-    def forward_train(self, query, key, self_attention):
-        """multi_head_attention_forward (:120-295) through autograd, no masks: query (B,Pq,E), key == value (B,Pk,E) -> (B,Pq,E)"""
+    def forward_train(self, query, key, self_attention, key_padding_mask=None):
+        """multi_head_attention_forward (:120-295) through autograd: query (B,Pq,E), key == value (B,Pk,E) -> (B,Pq,E).
+        key_padding_mask (B,Pk) bool or None: masked keys get -inf before the softmax, then dropout (:266-283)"""
         B, Pq, E = query.shape
         Pk, H = key.shape[1], self.num_heads
         W, b = self.in_proj_weight, self.in_proj_bias
@@ -228,7 +229,10 @@ class MultiheadAttention(nn.Module):
             k, v = F.linear(key, W[E:], None if b is None else b[E:]).chunk(2, dim=-1)
         q = q * float(self.head_dim) ** -0.5
         heads = lambda t, P: t.reshape(B, P, H, self.head_dim).transpose(1, 2).reshape(B * H, P, self.head_dim)    # noqa: E731
-        w = F.softmax(torch.bmm(heads(q, Pq), heads(k, Pk).transpose(1, 2)), dim=-1)
+        w = torch.bmm(heads(q, Pq), heads(k, Pk).transpose(1, 2))
+        if key_padding_mask is not None:
+            w = w.view(B, H, Pq, Pk).masked_fill(key_padding_mask.view(B, 1, 1, Pk), float('-inf')).view(B * H, Pq, Pk)
+        w = F.softmax(w, dim=-1)
         w = F.dropout(w, p=self.dropout, training=self.training)
         out = torch.bmm(w, heads(v, Pk)).view(B, H, Pq, self.head_dim).transpose(1, 2).reshape(B, Pq, E)
         return F.linear(out, self.out_proj.weight, self.out_proj.bias)
@@ -278,8 +282,9 @@ class TransformerDecoderLayer(nn.Module):
         x = self._ln(self.norm3, x, h)
         return x.view(B, Pq, E)
 
-    def forward_train(self, query, key, query_pos):
-        """decoder.py:48-92 in training (no masks, no key position embedding): query (B,Pq,E), key (B,Pk,E) -> (B,Pq,E)"""
+    def forward_train(self, query, key, query_pos, sa_mask=None, ca_mask=None):
+        """decoder.py:48-92 in training (no key position embedding): query (B,Pq,E), key (B,Pk,E) -> (B,Pq,E); sa_mask (B,Pq) and
+        ca_mask (B,Pk) bool key padding masks of the self- and cross-attention, or None"""
         B, Pq, E = query.shape
         qpe = None
         if self.self_posembed is not None:
@@ -287,8 +292,8 @@ class TransformerDecoderLayer(nn.Module):
         pos = (lambda t: t) if qpe is None else (lambda t: t + qpe)      # noqa: E731
         if not self.cross_only:
             q = pos(query)
-            query = self.norm1(query + self.dropout1(self.self_attn.forward_train(q, q, True)))
-        query = self.norm2(query + self.dropout2(self.multihead_attn.forward_train(pos(query), key, False)))
+            query = self.norm1(query + self.dropout1(self.self_attn.forward_train(q, q, True, sa_mask)))
+        query = self.norm2(query + self.dropout2(self.multihead_attn.forward_train(pos(query), key, False, ca_mask)))
         h = self.linear2(self.dropout(F.relu(self.linear1(query))))
         return self.norm3(query + self.dropout3(h))
 
@@ -384,6 +389,17 @@ class PositionHead(_HeadBase):
             rets.append(self.prediction_heads[i].forward_tokens(query.reshape(-1, query.shape[-1]), mode))
         return rets[-1] if self.auxiliary is False else rets[0]
 
+    def forward_train(self, query, memory, query_pos, padding_mask, mem_per_box):
+        """position_head.py:83-114 in training: the same masks as bool key padding masks, through autograd"""
+        B, L = padding_mask.shape
+        sa = padding_mask != 0
+        ca = sa.view(B, L, 1).expand(B, L, mem_per_box).reshape(B, -1)
+        rets = []
+        for i in range(self.num_decoder_layers):
+            query = self.decoder[i].forward_train(query, memory, query_pos, sa, ca)
+            rets.append(self.prediction_heads[i].forward_train(query.reshape(-1, query.shape[-1])))
+        return rets[-1] if self.auxiliary is False else rets[0]
+
 
 class GeometryHead(_HeadBase):
     POS_DIMS = 3
@@ -432,9 +448,22 @@ class TargetAssigner:
             anchors = self.anchor_sizes.to(gt.device, gt.dtype).unsqueeze(0)
             delta = (gt[:, 3:6].unsqueeze(1) - anchors) / anchors
             return {'geometry_reg': delta.reshape(gt.shape[0], -1), 'geometry_cls': torch.min(delta.abs().sum(-1), dim=-1)[1]}
+        if self.mode == 'position':
+            # target_assign.py:32-53: gt heading folded into [-pi, pi], centre residual, heading residual against every bin's anchor
+            # and the heading bin.  Deviation: floor((yaw + pi) / (pi / 6)) is 12 for yaw = pi and for float32 headings a few ulps
+            # below it, a bin that does not exist (cross_entropy rejects it; on the device, a device-side assert).  +pi closes bin
+            # 11, so 12 becomes 11.
+            traj, gt = data_dict['pos_trajectory'], data_dict['gt_pos_trajectory']
+            h = gt[..., 6]
+            h = torch.where(h < -np.pi, h + 2 * np.pi, h)
+            h = torch.where(h > np.pi, h - 2 * np.pi, h)
+            anchors = self.anchor_angles.to(h.device, h.dtype)
+            return {'center_reg': gt[..., :3] - traj[..., :3],
+                    'heading_reg': (h.unsqueeze(-1) - anchors) / (np.pi / self.dir_bin_num),
+                    'heading_cls': torch.floor((h + np.pi) / (np.pi / 6.)).long().clamp(0, self.dir_bin_num - 1),
+                    'boxes_gt': torch.cat([gt[..., :6], h.unsqueeze(-1)], -1), 'box_num': data_dict['box_num']}
         if self.mode != 'confidence':
-            raise NotImplementedError('TargetAssigner.encode_torch: the geometry and confidence modes are implemented (GRM and CRM '
-                                      'training)')
+            raise NotImplementedError('TargetAssigner.encode_torch: mode %r' % (self.mode,))
         iou = torch.clamp(data_dict['iou'], 0, 1).reshape(-1)
         pos = iou >= self.score_thresh[1]
         return {'score_gt': pos.to(iou.dtype), 'iou_gt': iou, 'mask': (iou < self.score_thresh[0]) | pos}
@@ -473,11 +502,63 @@ class PositionTransformer(nn.Module):
         assert dec.pop('NAME') == 'PositionHead'
         self.decoder = PositionHead(**dec)
         self.preds_dict = {}
+        self.targets_dict = {}
+        self.loss_weight = [0.1, 2]
+        self.pooled_rows = {}           # the rows the last training step's max-pools picked: 'memory' (B, 256), 'query' (B*L, 256);
+        #                                 'memory_pool' (B, 256) the pooled memory_encoder output
 
-    @torch.no_grad()
     def forward(self, data_dict):
         if self.training:
-            raise NotImplementedError('refiner training is a next row (SURVEY.md §8f)')
+            return self.forward_train(data_dict)
+        return self.forward_eval(data_dict)
+
+    def forward_train(self, data_dict):
+        """position_transformer.py:98-139 in training: the query encoder and the memory path on the train-mode point layers
+        (refine/train.py), the query MLP, position embedding, decoder and heads through autograd on this module's own layers,
+        token-major, dropout included"""
+        if self.mode == _lib.DZ_F32 and torch.backends.cuda.matmul.allow_tf32:
+            raise RuntimeError('PositionTransformer with COMPUTE_MODE fp32 trains in fp32, but torch.backends.cuda.matmul.allow_tf32 is '
+                               'set: the query MLP and the decoder would run TF32')
+        local, glob, traj = data_dict['pos_query_points'].float(), data_dict['pos_memory_points'].float(), data_dict['pos_trajectory']
+        B, L, P, C = local.shape
+        Pm = glob.shape[2]
+        if Pm != 48 or glob.shape[:2] != (B, L):
+            raise ValueError('train-mode PositionTransformer needs pos_memory_points (B, L, 48, C) beside pos_query_points (B, L, P, C) '
+                             '(position_head.py builds its cross-attention mask for 48 memory points per box); got %s and %s'
+                             % (tuple(glob.shape), tuple(local.shape)))
+        q = _train_mlp(self.query_mlp, train.prm_query(self, local))                    # (B*L, E)
+        mem = train.prm_memory(self, glob)                                              # (B*L*Pm, E)
+        E = q.shape[1]
+        query_pos = torch.cat([traj[..., :3], traj[..., 6:]], dim=-1).float()
+        preds = self.decoder.forward_train(q.view(B, L, E), mem.view(B, L * Pm, E), query_pos, data_dict['padding_mask'], Pm)
+        preds = {k: v.view(B, L, -1) for k, v in preds.items()}
+        preds['size_reg'] = traj[:, :, 3:6]
+        self.preds_dict.update(preds)
+        self.targets_dict.update(self.target_assigner.encode_torch(data_dict))
+        return data_dict
+
+    def get_loss(self, tb_dict=None):
+        """position_transformer.py:143-186: per track over its first box_num boxes, the centre L1 summed / (bs * num), the heading
+        cross entropy (mean) / bs and the L1 of the target bin's heading residual summed / (bs * num); center + 0.1 cls + 2 reg"""
+        tb_dict = {} if tb_dict is None else tb_dict
+        p, t = self.preds_dict, self.targets_dict
+        B, L, _ = p['center_reg'].shape
+        num = t['box_num'].to(p['center_reg'].device).long().clamp(1, L)
+        valid = torch.arange(L, device=num.device).unsqueeze(0) < num.unsqueeze(1)                         # (B, L)
+        cent = (p['center_reg'] - t['center_reg'].float()).abs().sum(-1)
+        center_loss = (torch.where(valid, cent, 0).sum(1) / num).sum() / B
+        ce = F.cross_entropy(p['heading_cls'].reshape(B * L, -1), t['heading_cls'].reshape(-1), reduction='none').view(B, L)
+        cls_loss = (torch.where(valid, ce, 0).sum(1) / num).sum() / B
+        reg = torch.gather((p['heading_reg'] - t['heading_reg'].float()).abs(), 2, t['heading_cls'].unsqueeze(-1)).squeeze(-1)
+        reg_loss = (torch.where(valid, reg, 0).sum(1) / num).sum() / B
+        tb_dict.update({'center_reg_loss': center_loss, 'heading_cls_loss': cls_loss, 'heading_reg_loss': reg_loss})
+        w1, w2 = self.loss_weight
+        loss = center_loss + w1 * cls_loss + w2 * reg_loss
+        tb_dict['position_loss'] = loss
+        return loss, tb_dict
+
+    @torch.no_grad()
+    def forward_eval(self, data_dict):
         local, glob, traj = data_dict['pos_query_points'], data_dict['pos_memory_points'], data_dict['pos_trajectory']
         B, L, P, C = local.shape
         Pm = glob.shape[2]

@@ -179,18 +179,23 @@ def _w(w):
 
 
 class GrmMemoryPath(torch.autograd.Function):
-    """memory_encoder (11 -> 128 -> 128 -> 512, max over the track's N points: g) -> memory_mlp on cat([y2, g]) (640 -> 512 -> 256):
-    x (B*N, c0) -> y5 (B*N, 256).  ``rows`` (a dict) receives the pooled row of each (track, channel) under 'memory' and the pooled
-    output g under 'memory_pool'.  Arguments
-    after ``bns`` (the five BatchNorm1d modules): per layer conv weight, BN weight, BN bias."""
+    """memory_encoder (c0 -> C1 -> C2 -> C3, max over the track's N points: g) -> memory_mlp on the concatenation of y2 and g
+    (-> C4 -> 256): x (B*N, c0) -> y5 (B*N, 256).  GRM: 11 -> 128 -> 128 -> 512, cat([y2, g]) 640 -> 512 -> 256
+    (geometry_transformer.py:128); PRM: 32 -> 128 -> 128 -> 256, cat([g, y2]) 384 -> 512 -> 256 (position_transformer.py:120), so
+    ``glob_first`` names the concatenation order.  ``rows`` (a dict) receives the pooled row of each (track, channel) under
+    'memory' and the pooled output g under 'memory_pool'.  Arguments after ``glob_first`` (``bns``: the five BatchNorm modules):
+    per layer conv weight, BN weight, BN bias.  Weight gradients come back in each weight's own shape."""
 
     @staticmethod
-    def forward(ctx, x, N, mode, rows, bns, w1, g1, b1, w2, g2, b2, w3, g3, b3, w4, g4, b4, w5, g5, b5):
+    def forward(ctx, x, N, mode, rows, bns, glob_first, w1, g1, b1, w2, g2, b2, w3, g3, b3, w4, g4, b4, w5, g5, b5):
         R = x.shape[0]
         B = R // N
         W1, W2, W3, W4, W5 = (_w(w) for w in (w1, w2, w3, w4, w5))
-        C2 = W2.shape[0]
-        W4p, W4g = W4[:, :C2].contiguous(), W4[:, C2:].contiguous()       # cat order [y2, g] (geometry_transformer.py:128)
+        C2, C3 = W2.shape[0], W3.shape[0]
+        if glob_first:
+            W4g, W4p = W4[:, :C3].contiguous(), W4[:, C3:].contiguous()
+        else:
+            W4p, W4g = W4[:, :C2].contiguous(), W4[:, C2:].contiguous()
         z1, ps, _, _ = ops.pm_fwd(x, W1, FIRST_MODE)
         t1, s1 = _bn_table(ps, g1, b1, bns[0], R)
         z2, ps, _, _ = ops.pm_fwd(z1, W2, mode, t1)
@@ -208,6 +213,7 @@ class GrmMemoryPath(torch.autograd.Function):
         y5 = ops.pm_act(z5, t5)
         ctx.save_for_backward(x, z1, z2, z3, z4, z5, g)
         ctx.st = (N, mode, (W1, W2, W3, W4p, W4g, W5), (t1, t2, t3, t4, t5), (s1, s2, s3, s4, s5), sel3, zsel3, zsum4)
+        ctx.glob_first, ctx.shapes = glob_first, [w.shape for w in (w1, w2, w3, w4, w5)]
         return y5
 
     @staticmethod
@@ -243,17 +249,17 @@ class GrmMemoryPath(torch.autograd.Function):
         dbet1, dgam1 = ops.pm_reduce_tiles(ps)[0]
         _set_bwd(t1, dbet1, dgam1, R)
         dW1 = ops.pm_wgrad((dh1, None, None, z1, t1), x, mode)
+        dW4 = torch.cat([dW4g, dW4p] if ctx.glob_first else [dW4p, dW4g], dim=1)
+        w1, w2, w3, w4, w5 = (t.float().view(sh) for t, sh in zip((dW1, dW2, dW3, dW4, dW5), ctx.shapes))
         f = lambda t: t.float()                                          # noqa: E731
-        dW4 = torch.cat([dW4p, dW4g], dim=1)
-        return (None, None, None, None, None,
-                f(dW1).unsqueeze(-1), f(dgam1), f(dbet1), f(dW2).unsqueeze(-1), f(dgam2), f(dbet2),
-                f(dW3).unsqueeze(-1), f(dgam3), f(dbet3), f(dW4).unsqueeze(-1), f(dgam4), f(dbet4),
-                f(dW5).unsqueeze(-1), f(dgam5), f(dbet5))
+        return (None, None, None, None, None, None,
+                w1, f(dgam1), f(dbet1), w2, f(dgam2), f(dbet2), w3, f(dgam3), f(dbet3), w4, f(dgam4), f(dbet4), w5, f(dgam5), f(dbet5))
 
 
 class GrmQueryEncoder(torch.autograd.Function):
-    """query_encoder (4 -> 128 -> 128 -> 256) and the max over each query's P points: x (B*Q*P, c0) -> (B*Q, 256); ``rows`` receives
-    the pooled rows under 'query'"""
+    """query_encoder (GRM: 4 -> 128 -> 128 -> 256 Conv1d; PRM: 32 -> 128 -> 128 -> 256 Conv2d(1x1), BatchNorm2d) and the max over
+    each group of P points: x (groups*P, c0) -> (groups, 256); ``rows`` receives the pooled rows under 'query'.  Weight gradients
+    come back in each weight's own shape."""
 
     @staticmethod
     def forward(ctx, x, P, mode, rows, bns, w1, g1, b1, w2, g2, b2, w3, g3, b3):
@@ -269,6 +275,7 @@ class GrmQueryEncoder(torch.autograd.Function):
         rows['query'] = sel3
         ctx.save_for_backward(x, z1, z2, z3, pooled)
         ctx.st = (P, mode, (W1, W2, W3), (t1, t2, t3), (s1, s2, s3), sel3, zsel3)
+        ctx.shapes = [w.shape for w in (w1, w2, w3)]
         return pooled
 
     @staticmethod
@@ -288,26 +295,30 @@ class GrmQueryEncoder(torch.autograd.Function):
         dbet1, dgam1 = ops.pm_reduce_tiles(ps)[0]
         _set_bwd(t1, dbet1, dgam1, R)
         dW1 = ops.pm_wgrad((dh1, None, None, z1, t1), x, mode)
+        w1, w2, w3 = (t.float().view(sh) for t, sh in zip((dW1, dW2, dW3), ctx.shapes))
         f = lambda t: t.float()                                          # noqa: E731
-        return (None, None, None, None, None, f(dW1).unsqueeze(-1), f(dgam1), f(dbet1), f(dW2).unsqueeze(-1), f(dgam2), f(dbet2),
-                f(dW3).unsqueeze(-1), f(dgam3), f(dbet3))
+        return (None, None, None, None, None, w1, f(dgam1), f(dbet1), w2, f(dgam2), f(dbet2), w3, f(dgam3), f(dbet3))
 
 
-def _check_widths(name, seq, n_layers):
-    """the train-mode kernels take a stack of n_layers [Conv1d | BatchNorm1d | ReLU] layers whose output channels are multiples of
-    128 (the column tile of the forward and dgrad kernels)"""
-    convs = [m for m in seq if isinstance(m, torch.nn.Conv1d)]
+def _check_widths(name, seq, n_layers, model='GeometryTransformer'):
+    """the train-mode kernels take a stack of n_layers [Conv1d | BatchNorm1d | ReLU] or [Conv2d(1x1) | BatchNorm2d | ReLU] layers
+    whose output channels are multiples of 128 (the column tile of the forward and dgrad kernels)"""
+    conv = (torch.nn.Conv1d, torch.nn.Conv2d)
+    convs = [m for m in seq if isinstance(m, conv)]
     widths = [m.weight.shape[0] for m in convs]
-    if len(seq) != 3 * n_layers or len(convs) != n_layers or any(c % 128 for c in widths):
-        raise ValueError('train-mode GeometryTransformer supports a %s of %d Conv1d + BatchNorm1d + ReLU layers with output channels '
-                         'that are multiples of 128 (the shipped MEMORY_ENCODER / QUERY_ENCODER [128, 128], REGRESSION_MLP [512], '
-                         'EMBED_DIMS 256); got output channels %s' % (name, n_layers, widths))
+    layered = len(seq) == 3 * n_layers and all(
+        isinstance(seq[3 * i], conv) and isinstance(seq[3 * i + 1], (torch.nn.BatchNorm1d, torch.nn.BatchNorm2d))
+        and isinstance(seq[3 * i + 2], torch.nn.ReLU) and all(k == 1 for k in seq[3 * i].kernel_size) for i in range(n_layers))
+    if not layered or any(c % 128 for c in widths):
+        raise ValueError('train-mode %s supports a %s of %d Conv + BatchNorm + ReLU layers (1x1 convs) with output channels that '
+                         'are multiples of 128 (the shipped MEMORY_ENCODER / QUERY_ENCODER [128, 128], REGRESSION_MLP [512], '
+                         'EMBED_DIMS 256); got output channels %s' % (model, name, n_layers, widths))
 
 
-def _check_rows(what, n):
+def _check_rows(what, n, model='GeometryTransformer'):
     if n % ops.PM_TILE != 0 or n <= 0:
-        raise ValueError('train-mode GeometryTransformer needs the %s to be a positive multiple of %d (a row tile never straddles two '
-                         'groups); got %d' % (what, ops.PM_TILE, n))
+        raise ValueError('train-mode %s needs the %s to be a positive multiple of %d (a row tile never straddles two groups); got %d'
+                         % (model, what, ops.PM_TILE, n))
 
 
 def grm_memory(module, mpts):
@@ -318,7 +329,7 @@ def grm_memory(module, mpts):
     _check_widths('memory_encoder', e, 3)
     _check_widths('memory_mlp', m, 2)
     return GrmMemoryPath.apply(mpts.reshape(B * N, C).contiguous(), N, module.mode, module.pooled_rows, (e[1], e[4], e[7], m[1], m[4]),
-                               e[0].weight, e[1].weight, e[1].bias, e[3].weight, e[4].weight, e[4].bias,
+                               False, e[0].weight, e[1].weight, e[1].bias, e[3].weight, e[4].weight, e[4].bias,
                                e[6].weight, e[7].weight, e[7].bias, m[0].weight, m[1].weight, m[1].bias,
                                m[3].weight, m[4].weight, m[4].bias)
 
@@ -330,5 +341,44 @@ def grm_query(module, qpts):
     e = module.query_encoder
     _check_widths('query_encoder', e, 3)
     return GrmQueryEncoder.apply(qpts.reshape(B * Q * P, C).contiguous(), P, module.mode, module.pooled_rows, (e[1], e[4], e[7]),
+                                 e[0].weight, e[1].weight, e[1].bias, e[3].weight, e[4].weight, e[4].bias,
+                                 e[6].weight, e[7].weight, e[7].bias)
+
+
+# ---- PRM: the same two paths at the PRM's widths ----------------------------------------------------------------------------------
+# The kernels take the row count R as an int (every element offset inside them is 64-bit), so a PRM batch must keep B * L * P, the
+# query rows, below 2^31.
+MAX_ROWS = (1 << 31) - 1
+
+
+def prm_memory(module, mpts):
+    """PositionTransformer's train-mode memory_encoder (32 -> 128 -> 128 -> 256) -> max over the track's L * Pm rows (padded boxes
+    included, as position_transformer.py:116-118 pools them) -> memory_mlp on cat([g, y2]) (384 -> 512 -> 256): mpts (B, L, Pm, C)
+    -> (B*L*Pm, 256)"""
+    B, L, Pm, C = mpts.shape
+    N = L * Pm
+    _check_rows('memory rows per track L * MEMORY_POINTS_NUM', N, 'PositionTransformer')
+    if B * N > MAX_ROWS:
+        raise ValueError('train-mode PositionTransformer: %d memory rows exceed the kernels\' int row count' % (B * N))
+    e, m = module.memory_encoder, module.memory_mlp
+    _check_widths('memory_encoder', e, 3, 'PositionTransformer')
+    _check_widths('memory_mlp', m, 2, 'PositionTransformer')
+    return GrmMemoryPath.apply(mpts.reshape(B * N, C).contiguous(), N, module.mode, module.pooled_rows, (e[1], e[4], e[7], m[1], m[4]),
+                               True, e[0].weight, e[1].weight, e[1].bias, e[3].weight, e[4].weight, e[4].bias,
+                               e[6].weight, e[7].weight, e[7].bias, m[0].weight, m[1].weight, m[1].bias,
+                               m[3].weight, m[4].weight, m[4].bias)
+
+
+def prm_query(module, qpts):
+    """PositionTransformer's train-mode query_encoder (Conv2d(1x1) + BatchNorm2d + ReLU, 32 -> 128 -> 128 -> 256) and the max over
+    each box's P points: qpts (B, L, P, C) -> (B*L, 256).  BatchNorm2d over (B, C, L, P) takes its statistics over the B*L*P rows."""
+    B, L, P, C = qpts.shape
+    _check_rows('query points per box P', P, 'PositionTransformer')
+    if B * L * P > MAX_ROWS:
+        raise ValueError('train-mode PositionTransformer: B * L * P = %d query rows exceed the kernels\' int row count (2^31 - 1)'
+                         % (B * L * P))
+    e = module.query_encoder
+    _check_widths('query_encoder', e, 3, 'PositionTransformer')
+    return GrmQueryEncoder.apply(qpts.reshape(B * L * P, C).contiguous(), P, module.mode, module.pooled_rows, (e[1], e[4], e[7]),
                                  e[0].weight, e[1].weight, e[1].bias, e[3].weight, e[4].weight, e[4].bias,
                                  e[6].weight, e[7].weight, e[7].bias)

@@ -312,18 +312,25 @@ int dz_refine_inputs(int kind, const float* points, int pt_stride, const int32_t
  * (waymo_geometry_dataset.py:160-186).  lidar, world (B, L, 7) f64, rows past box_num zero. */
 int dz_refine_revert(int kind, const float* pred, const double* poses, int n_frames, const double* boxes, const int32_t* frame_of_box,
                      const int32_t* box_num, int B, int L, double* lidar, double* world, dz_stream_t stream);
-/* Training samples (the training branch of WaymoGeometryDataset / WaymoConfidenceDataset.extract_track_feature), csrc/refine_data.cu.
+/* Training samples (the training branch of WaymoPositionDataset / WaymoGeometryDataset / WaymoConfidenceDataset
+ * .extract_track_feature), csrc/refine_data.cu.
  * dz_crop_tracks: the crop of dz_refine_inputs once, copying the first `width` floats of every in-box point row; box slot t's points go
  *   to rows[row_base[t] ..] in frame order.  Called with rows = row_base = NULL it writes only counts (B, L), the in-box point count
  *   of every slot (0 past box_num); the caller sizes rows from them and calls again.
- * dz_refine_train_draw: per track, keyed on (seed, epoch, track_uid) only.  kind 2 (GRM): eligible slots are the matched ones
- *   (matched (B, L) u8); kind 1 (CRM): every valid slot.  kept (B, L) source slots in ascending order, -1 padded; n_kept (B) uniform on
- *   min(5, m) .. m of m eligible; GRM: query_slots (B, nq) min(nq, n_kept) distinct kept positions ascending, -1 padded, and flip
- *   (B, L) u8 bits per kept position; CRM: init_slot (B), a kept position.
+ * dz_refine_train_draw: per track, keyed on (seed, epoch, track_uid) only.  kind 0 (PRM) and kind 2 (GRM): eligible slots are the
+ *   matched ones (matched (B, L) u8); kind 1 (CRM): every valid slot.  kept (B, L) source slots in ascending order, -1 padded; n_kept
+ *   (B) uniform on min(5, m) .. m of m eligible; GRM: query_slots (B, nq) min(nq, n_kept) distinct kept positions ascending, -1
+ *   padded, and flip (B, L) u8 bits per kept position; PRM / CRM: init_slot (B), a kept position (query_slots, flip unused).
  * dz_refine_train_inputs: dz_refine_inputs on the kept slots of each track (a derived table of n_kept boxes) with the drawn query
- *   positions (GRM), init box (CRM) and flips (GRM, memory rows only), point samples keyed on the epoch's seed.  Outputs as
- *   dz_refine_inputs kinds 1 / 2, plus GRM: gt_box_f (B, q_out, 7) gt_geo_query_boxes (sizes of gt_boxes), gt_traj (B, L, 7) f32 kept
- *   gt_boxes; CRM: iou_out (B, L) the kept iou, -1 padded.  counts / sel as dz_refine_inputs, on the derived slots. */
+ *   positions (GRM), init box (CRM) and flips (GRM, memory rows only), point samples keyed on the epoch's seed.  Kinds 1 / 2 only.
+ *   Outputs as dz_refine_inputs kinds 1 / 2, plus GRM: gt_box_f (B, q_out, 7) gt_geo_query_boxes (sizes of gt_boxes), gt_traj
+ *   (B, L, 7) f32 kept gt_boxes; CRM: iou_out (B, L) the kept iou, -1 padded.  counts / sel as dz_refine_inputs, on the derived slots.
+ * dz_position_train_inputs: the same for the PRM (kind 0 of the draw), with the drawn init box in place of slot n_kept / 2.  An entry
+ *   point of its own because the PRM adds an output dz_refine_train_inputs has no parameter for (init_box, pos_init_box).
+ *   gt_boxes (B, L, 7) f64 world.  Outputs as dz_refine_inputs kind 0 without the class columns: q_pts (B, L, kq, 32), m_pts
+ *   (B, L, km, 32), traj (B, L, 7) pos_trajectory, padding_mask (B, L), init_box (B, 7) pos_init_box; plus gt_traj (B, L, 7) f32
+ *   gt_pos_trajectory, the kept gt_boxes in the init box's frame by the float64 transform of traj.  Rows past n_kept are zero
+ *   (padding_mask 1).  counts / sel (B, L, kq + km) as dz_refine_inputs, on the derived slots. */
 size_t dz_crop_tracks_ws_bytes(int B, int L, int max_frame_points);
 int dz_crop_tracks(const float* points, int pt_stride, int width, const int32_t* frame_offsets, int n_frames, int max_frame_points,
                    const double* poses, const double* boxes, const int32_t* frame_of_box, const int32_t* box_num, int B, int L,
@@ -342,6 +349,14 @@ int dz_refine_train_inputs(int kind, const float* points, int pt_stride, const i
                            const int32_t* query_slots, const int32_t* init_slot, const uint8_t* flip, float* q_pts, float* m_pts,
                            float* traj, float* box_f, float* gt_box_f, float* gt_traj, float* iou_out, int32_t* query_num,
                            int32_t* counts, int32_t* sel, void* ws, size_t ws_bytes, dz_stream_t stream);
+size_t dz_position_train_inputs_ws_bytes(int B, int L, int max_frame_points, int kq, int km);
+int dz_position_train_inputs(const float* points, int pt_stride, const int32_t* frame_offsets, int n_frames, int max_frame_points,
+                             const double* poses, const double* boxes, const int32_t* frame_of_box, const float* scores,
+                             const int32_t* cls, const int64_t* track_uid, const double* gt_boxes, int B, int L, int kq, int km,
+                             double enlarge_scale, int crop_on_bev, int crop, unsigned long long seed, long long epoch,
+                             const int32_t* kept, const int32_t* n_kept, const int32_t* init_slot, float* q_pts, float* m_pts,
+                             float* traj, float* gt_traj, float* padding_mask, float* init_box, int32_t* counts, int32_t* sel,
+                             void* ws, size_t ws_bytes, dz_stream_t stream);
 
 /* ---- combine: refined tracks -> per-frame result rows (csrc/combine.cu) ------------------------------------------------------- */
 /* convert_frame_format + combine_det as combine_final drives them (daemon/combine_output.py:27-41,44-99,102-167), for the B tracks

@@ -1,12 +1,13 @@
-"""Refiner training samples on the device, per epoch, beside one training step of each model.
+"""Refiner training samples on the device, per epoch, beside one step of each model.
 Setup (not timed): the 199-frame sequence of tools/bench_offboard.py (180 K background points per frame, about 300 tracks of the
 three classes), tracked (track.track_sequences) and assigned to its ground truth (track.assign_track_target, refine.data.track_targets),
 with synthetic CRM IoU labels (uniform on [0, 1]: the builders only gather them).  Prints JSON lines with:
   * the card's name and power limit, read in the same run;
   * crop_tracks of every box once (CUDA events, best of --reps, after a warm-up);
-  * per epoch, training_order plus every batch of each builder on the cropped rows (crop=False) at the shipped batch sizes (GRM
-    B = 128, CRM B = 256): milliseconds and tracks/s (CUDA events around the epoch, host work included);
-  * one device training step (forward, loss, backward) of each model in tf32 at the same B, on the first batch of the epoch.
+  * per epoch, training_order plus every batch of each builder on the cropped rows (crop=False) at the shipped batch sizes (PRM
+    B = 96, GRM B = 128, CRM B = 256): milliseconds and tracks/s (CUDA events around the epoch, host work included);
+  * one device training step (forward, loss, backward) of the GRM and CRM in tf32 at the same B, on the first batch of the epoch;
+    the PRM, which has no training step yet, gets its tf32 eval forward on that batch instead (prm_eval_forward_ms).
     python tools/bench_refine_train_inputs.py [--tracks 300] [--frames 199] [--background 180000] [--reps 5]
 """
 import argparse
@@ -52,7 +53,9 @@ def _timed(fn, reps):
 
 
 def _model(kind):
-    if kind == 'grm':
+    if kind == 'prm':
+        c, spec = ri.prm_cfg(), {'NAME': 'PositionRefineModel', 'QUERY_POINT_DIMS': 32, 'MEMORY_POINT_DIMS': 32}
+    elif kind == 'grm':
         c, spec = ri.grm_cfg(), {'NAME': 'GeometryRefineModel', 'QUERY_POINT_DIMS': 11, 'MEMORY_POINT_DIMS': 4}
     else:
         c, spec = ri.crm_cfg(), {'NAME': 'ConfidenceRefineModel', 'QUERY_POINT_DIMS': 32, 'MEMORY_POINT_DIMS': 32}
@@ -70,6 +73,7 @@ def main():
     ap.add_argument('--radius', type=float, default=150.0)
     ap.add_argument('--reps', type=int, default=5)
     ap.add_argument('--seed', type=int, default=1)
+    ap.add_argument('--prm-batch', type=int, default=96)
     ap.add_argument('--grm-batch', type=int, default=128)
     ap.add_argument('--crm-batch', type=int, default=256)
     a = ap.parse_args()
@@ -100,7 +104,7 @@ def main():
     print(json.dumps({'tracks': len(tb), 'boxes': int(tb.box_num.sum()), 'cropped_rows': int(bf.shape[0]),
                       'crop_tracks_ms': round(crop_ms, 3)}), flush=True)
 
-    for kind, B in (('grm', a.grm_batch), ('crm', a.crm_batch)):
+    for kind, B in (('prm', a.prm_batch), ('grm', a.grm_batch), ('crm', a.crm_batch)):
         state = {'epoch': 0}
 
         def epoch():
@@ -108,7 +112,10 @@ def main():
             first = None
             for i in range(0, len(order), B):
                 idx = order[i:i + B].tolist()
-                if kind == 'grm':
+                if kind == 'prm':
+                    o = D.position_training_inputs(bf, bo, bp, btb.select(idx), tg.select(idx), seed=a.seed, epoch=state['epoch'],
+                                                   crop=False)
+                elif kind == 'grm':
                     o = D.geometry_training_inputs(bf, bo, bp, btb.select(idx), tg.select(idx), seed=a.seed, epoch=state['epoch'],
                                                    crop=False)
                 else:
@@ -120,7 +127,19 @@ def main():
         epoch()
         ms = _timed(epoch, a.reps)
         m = _model(kind)
-        batch = state['first'] if kind == 'grm' else {'conf_points': state['first']['conf_points'], 'iou': state['first']['iou']}
+        batch = state['first'] if kind != 'crm' else {'conf_points': state['first']['conf_points'], 'iou': state['first']['iou']}
+        nb = len(state['first']['geo_query_num' if kind == 'grm' else 'box_num'])
+        row = {'kind': kind, 'batch': B, 'epoch_tracks': state['n'], 'epoch_ms': round(ms, 3),
+               'tracks_per_s': round(state['n'] / ms * 1e3, 1), 'build_ms_per_batch': round(ms / max(1, -(-state['n'] // B)), 3)}
+        if kind == 'prm':
+            m.eval()
+
+            def forward():
+                with torch.no_grad():
+                    m(dict(batch))
+            forward()
+            print(json.dumps(dict(row, prm_eval_forward_ms=round(_timed(forward, a.reps), 3), prm_eval_forward_batch=nb)), flush=True)
+            continue
 
         def step():
             m.zero_grad(set_to_none=True)
@@ -128,10 +147,7 @@ def main():
             ret['loss'].backward()
         step()
         step_ms = _timed(step, a.reps)
-        nb = len(state['first']['geo_query_num' if kind == 'grm' else 'box_num'])
-        print(json.dumps({'kind': kind, 'batch': B, 'epoch_tracks': state['n'], 'epoch_ms': round(ms, 3),
-                          'tracks_per_s': round(state['n'] / ms * 1e3, 1), 'build_ms_per_batch': round(ms / max(1, -(-state['n'] // B)), 3),
-                          'train_step_ms': round(step_ms, 3), 'train_step_batch': nb}), flush=True)
+        print(json.dumps(dict(row, train_step_ms=round(step_ms, 3), train_step_batch=nb)), flush=True)
 
 
 if __name__ == '__main__':
